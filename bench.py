@@ -14,17 +14,22 @@ Definitions (DESIGN.md section 4):
   * value     = inputs resident in HBM; e2e = the same metric through DiffusionInferer.sample() starting from pinned
                 HOST noise (H2D), the per-step timestep H2D the reference API does, the final D2H of the sample and —
                 at N > 1 — the all_gather of the finished samples.
-  * roofline  = tensor-pipe: algorithmic FLOPs of the 3x3x3-conv launches of igemm_tc_kernel<256,6,pair> in the timed
-                region / their CUDA-event time, against MEASURED_PEAKS.json's sustained bf16/fp16 GEMM throughput;
+  * roofline  = tensor-pipe: algorithmic FLOPs of the 3x3x3-conv launches of igemm_tc_kernel<128,4> in the timed
+                region / their CUDA-event time, against the H100 SXM data sheet's dense 16-bit tensor rate (989 TFLOP/s
+                at 700 W: a share of the data-sheet figure, not of a measured peak);
                 roofline.secondary[] = the attention kernel (tensor) and the HBM-bound kernels (GroupNorm apply,
-                DDIM step) timed the same way against the measured copy bandwidth.
+                DDIM step) timed the same way against the data sheet's 3.35 TB/s of HBM3 bandwidth.
+  * --dump-outputs DIR writes what the last timed step returned (prev_sample and pred_original_sample of
+                DDIMScheduler.step, float32 .npy; a fixed seeded sample of each when together they exceed 64 MB) so
+                that two builds can be compared output for output: the weights and the noise are drawn from fixed
+                seeds, so the same arguments give the same inputs.
   * other_configs = the other targets BASELINE.json names (C2 latent diffusion at batch 1 and 32, C4 VQVAE, C5
                 ControlNet + classifier-free guidance), each with its wall clock through the public API, algorithmic
                 TFLOP/s and (N = 1) the reference's CPU leg.
   * weak scaling: every GPU samples its own volume; the only collective is one all_gather of the finished samples.
-  * reference arm / cpu_baseline: the unmodified reference installed under baseline/_ref (oracle/make_ref.sh; MONAI's
+  * reference arm / cpu_baseline: the unmodified reference installed under oracle/_ref (oracle/make_ref.sh; MONAI's
                 layer wrappers come from oracle/monai_shim because MONAI is not installable offline), run through its
-                own DiffusionInferer.sample on the host cores; the oracle port only if baseline/_ref is absent.
+                own DiffusionInferer.sample on the host cores; the oracle port only if oracle/_ref is absent.
 """
 from __future__ import annotations
 
@@ -72,11 +77,8 @@ TF_C5_STEP = 4.11            # ControlNet + UNet on the doubled batch, per guide
 
 
 def peaks():
-    f = ROOT / "MEASURED_PEAKS.json"
-    if f.exists():
-        p = json.loads(f.read_text())
-        return p.get("bf16_tflops_sustained", 1449.3), p.get("hbm_gbs", 6582.5), "measured"
-    return 1400.0, 6650.0, "fallback"
+    """H100 SXM data sheet: dense FP16/BF16 tensor TFLOP/s and HBM3 GB/s (700 W part)."""
+    return 989.0, 3350.0, "H100 SXM data sheet"
 
 
 def redraw_zero_params(m, seed=1):
@@ -101,11 +103,11 @@ def build_model_state(seed=0):
 # ---------------------------------------------------------------------------------------------------------------
 # reference / CPU arm
 # ---------------------------------------------------------------------------------------------------------------
-REF_DIR = ROOT / "baseline" / "_ref"
+REF_DIR = ROOT / "oracle" / "_ref"
 
 
 def import_reference():
-    """The unmodified reference from baseline/_ref (pip-installed from /root/reference by oracle/make_ref.sh) on top
+    """The unmodified reference from oracle/_ref (installed by oracle/make_ref.sh) on top
     of the MONAI shim.  Returns the `generative` package or None when it did not travel."""
     if not (REF_DIR / "generative" / "__init__.py").exists():
         return None
@@ -200,8 +202,8 @@ def run_reference(args):
         return
     model = build_model_state()
     value, sec, cores, kind = cpu_c3_steps(model.state_dict(), args.steps, args.warmup)
-    what = ("the unmodified reference (baseline/_ref) through its DiffusionInferer.sample" if kind == "reference"
-            else "oracle port of the reference CPU path (baseline/_ref absent)")
+    what = ("the unmodified reference (oracle/_ref) through its DiffusionInferer.sample" if kind == "reference"
+            else "oracle port of the reference CPU path (oracle/_ref absent)")
     sample = (f"{what}: UNet forward + DDIM step on 1x1x{'x'.join(map(str, CPU_VOLUME))} "
               f"(the full 160x224x160 volume needs ~60 GB of fp32 activations and 2x29.9 GiB attention scores on CPU), "
               f"{args.steps} steps after {args.warmup} warm-up, {cores} threads")
@@ -218,7 +220,7 @@ def run_reference(args):
 
 
 def cpu_other_configs(states):
-    """Bounded CPU legs of C2 / C4 / C5 through the reference (baseline/_ref), a few seconds each; None without it."""
+    """Bounded CPU legs of C2 / C4 / C5 through the reference (oracle/_ref), a few seconds each; None without it."""
     import torch
     if import_reference() is None:
         return {}
@@ -274,7 +276,7 @@ def c5_mask():
 
 
 # ---------------------------------------------------------------------------------------------------------------
-# B200 arm
+# this package's arm
 # ---------------------------------------------------------------------------------------------------------------
 class ClockSampler:
     def __init__(self, index: int):
@@ -359,7 +361,7 @@ class Instrument:
         return counted
 
     def _igemm(self, p):
-        dominant = self.on and p.n_seg >= 27 and p.out_cols > 128              # 3x3x3 convs -> igemm_tc_kernel<256,4>
+        dominant = self.on and p.n_seg >= 27 and p.out_cols > 128              # 3x3x3 convs -> igemm_tc_kernel<128,4>
         if not dominant:
             return self.raw_igemm(p)
         rows = p.out_N * p.out_D * p.out_H * p.out_W
@@ -376,6 +378,25 @@ class Instrument:
 
     def ms(self, key):
         return sum(a.elapsed_time(b) for a, b in self.ev[key])
+
+
+DUMP_BYTES = 64 << 20          # --dump-outputs writes at most this much in all
+
+
+def dump_outputs(out_dir, arrays):
+    """Write each array as out_dir/<name>.npy in float32.  When the arrays together exceed DUMP_BYTES, each one is
+    replaced by the same fixed, seeded sample of its flattened elements (sorted indices; equal shapes give equal
+    indices), so two builds run with the same arguments still compare element for element."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    total = sum(t.numel() for t in arrays.values()) * 4
+    per = (DUMP_BYTES - 4096) // (4 * len(arrays))          # room for the .npy headers
+    for name, t in arrays.items():
+        a = t.detach().float().cpu().numpy()
+        if total > DUMP_BYTES and a.size > per:
+            idx = np.sort(np.random.default_rng(1234).choice(a.size, size=per, replace=False))
+            a = a.reshape(-1)[idx]
+        np.save(os.path.join(out_dir, f"{name}.npy"), a)
 
 
 def time_calls(fn, n, sync):
@@ -534,9 +555,12 @@ def run_b200(args):
     x = noise_host.cuda(non_blocking=True)
     inst = Instrument(lib, ops, _lib)
 
+    last = {}
+
     def one_step(x, t):
         eps = model(x, timesteps=torch.Tensor((t,)).to(x.device))
-        x, _ = sched.step(eps, t, x)
+        x, x0 = sched.step(eps, t, x)
+        last["pred_original_sample"] = x0
         return x
 
     def barrier():
@@ -579,6 +603,9 @@ def run_b200(args):
     times = {key: inst.ms(key) for key in inst.ev}
     work = dict(inst.work)
     counts = {key: len(v) for key, v in inst.ev.items()}
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {"prev_sample": x, "pred_original_sample": last["pred_original_sample"]})
+    last.clear()
 
     # ---- e2e through the public API: pinned host noise in, pinned host result out, the gather included ----
     ke = args.steps
@@ -615,7 +642,7 @@ def run_b200(args):
         if world == 1 and not args.no_cpu_baseline:
             v, sec, cores, kind = cpu_c3_steps(c3_state, 5, 1)
             cpu_line = {"value": v, "unit": "voxels/s", "cores": cores, "kind": kind,
-                        "sample": f"{'the unmodified reference (baseline/_ref)' if kind == 'reference' else 'oracle port'}: "
+                        "sample": f"{'the unmodified reference (oracle/_ref)' if kind == 'reference' else 'oracle port'}: "
                                   f"UNet forward + DDIM step on 1x1x{'x'.join(map(str, CPU_VOLUME))}, 5 steps after 1 "
                                   f"warm-up ({sec:.2f} s/step), {cores} threads"}
             if others is not None:
@@ -642,22 +669,16 @@ def run_b200(args):
             "config": {"workload": "C3: 3D DiffusionModelUNet (256,256,512) attn (F,F,T) heads (0,0,512), DDIM-50; "
                                    "one step = UNet forward + DDIMScheduler.step",
                        "volume": list(vol), "per_gpu_batch": args.batch, "samples_per_s": value / (voxels / args.batch),
-                       "operands": f"{_lib.ACT_DTYPE} x {_lib.ACT_DTYPE} -> fp32 accumulate (tcgen05 kind::f16)",
-                       "l2": "per-step working set (tens of GB of activations) >> 126 MB L2; no explicit flush",
+                       "operands": f"{_lib.ACT_DTYPE} x {_lib.ACT_DTYPE} -> fp32 accumulate (wgmma)",
+                       "l2": "per-step working set (GBs of activations) >> 50 MB L2; no explicit flush",
                        "finite_output": finite, "ms_per_step_per_rank": per_rank,
                        "algorithmic_tflop_per_forward": TF_C3_FORWARD,
                        "whole_step_tflops": TF_C3_FORWARD * (voxels / (C3_VOLUME[0] * C3_VOLUME[1] * C3_VOLUME[2]))
                                             / (ms_step * 1e-3)},
             "roofline": {"bound": "tensor", "achieved": achieved, "peak": peak_tf, "unit": "TFLOP/s",
                          "frac": achieved / peak_tf if peak_tf else None,
-                         # dram__bytes_read.sum + dram__bytes_write.sum of ONE launch of this kernel (the 256->256
-                         # 3x3x3 conv at 160x224x160; algorithmic 5.88e9 B) from the ncu --set full capture
-                         # profiles/r2_ncu_igemm_pair_conv256_fullres_final3_details.txt at the round's last commit
-                         # (4.33 GB read + 2.91 GB written, tensor pipe 99.5 % of active cycles, 13.02 ms at 1.31 GHz;
-                         # the capture earlier in the round, r2_ncu_igemm_pair_conv256_fullres_details.txt: 6.37e9)
-                         "traffic": 7.24e9,
-                         "kernel": "igemm_tc_kernel<256,6,pair> (3x3x3 convolutions, tcgen05 cta_group::2)",
-                         "peak_source": which + " sustained 16-bit GEMM",
+                         "kernel": "igemm_tc_kernel<128,4> (3x3x3 convolutions, wgmma)",
+                         "peak_source": which + " dense 16-bit tensor rate",
                          "share_of_step": times["conv"] / ms_local if ms_local else None,
                          "launches_timed": counts["conv"], "secondary": secondary},
             "cpu_baseline": cpu_line,
@@ -683,7 +704,11 @@ def main():
     ap.add_argument("--volume", type=int, nargs=3, default=None, help="override the C3 volume (debug only)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-other-configs", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's outputs to DIR/<name>.npy (float32)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     args.warmup = max(args.warmup, 0)
     if args.impl == "reference":
         run_reference(args)

@@ -1,4 +1,4 @@
-"""``generative`` — the reference's import path, served by the B200-native implementation.
+"""``generative`` — the reference's import path, served by the H100-native implementation.
 
 SURVEY.md section 8(b): callers of MONAI-GenerativeModels import ``generative.networks.nets``,
 ``generative.networks.layers``, ``generative.networks.schedulers``, ``generative.networks.blocks``,

@@ -1,4 +1,4 @@
-"""generativemodels_b200 — B200-native (sm_100a) diffusion sampling behind the MONAI GenerativeModels API.
+"""generativemodels_b200 — H100-native (sm_90a) diffusion sampling behind the MONAI GenerativeModels API.
 
 Only the sampling hot path is implemented (SURVEY.md §8): DiffusionModelUNet / ControlNet / AutoencoderKL / VQVAE
 forward, DDPM / DDIM / PNDM scheduler steps and the Diffusion / LatentDiffusion / ControlNet inferers' ``sample``.

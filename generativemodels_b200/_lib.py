@@ -1,6 +1,6 @@
 """ctypes binding of libb200gen.so (the C-ABI declared in include/b200gen.h).
 
-The library is the product: if it is missing, cannot be loaded or the device is not sm_100-class, every op
+The library is the product: if it is missing, cannot be loaded or the device is not an sm_90 (Hopper) GPU, every op
 raises — there is no CPU or PyTorch fallback anywhere in this package.
 """
 from __future__ import annotations
@@ -218,14 +218,14 @@ def check(rc: int, what: str) -> None:
 
 
 def require_device():
-    """Fail loudly unless the current CUDA device is sm_100-class."""
+    """Fail loudly unless the current CUDA device is sm_90 (H100)."""
     global _device_ok
     lib = load()
     if not _device_ok:
         import torch
 
         if not torch.cuda.is_available():
-            raise B200Error("generativemodels_b200 needs a CUDA device (sm_100a); none is visible and there is no CPU path")
+            raise B200Error("generativemodels_b200 needs a CUDA device (sm_90a); none is visible and there is no CPU path")
         check(lib.b200_device_check(), "b200_device_check")
         _device_ok = True
     return lib

@@ -1,5 +1,5 @@
 """App edge of the sampling path (SURVEY.md §8f rank 4): the reference's brain-LDM model-zoo bundle
-(model-zoo/models/brain_image_synthesis_latent_diffusion_model) running on the B200 classes — its ``Sampler`` and
+(model-zoo/models/brain_image_synthesis_latent_diffusion_model) running on this package's classes — its ``Sampler`` and
 ``NiftiSaver`` scripts, a resolver for the bundle's ``inference.json`` and a pre-packed weight cache file."""
 from .config import BundleConfig
 from .packed_cache import fingerprint, load_packed, save_packed

@@ -1,7 +1,7 @@
 """``python -m generativemodels_b200.bundle run <id> [<id> ...] --config_file configs/inference.json [--key value ...]``
 
 Mirrors ``python -m monai.bundle run`` for the brain-LDM bundle (its docs/README.md): resolves the requested items of
-the bundle's unmodified ``inference.json`` on the B200 classes.  ``--key value`` overrides a config item (JSON value
+the bundle's unmodified ``inference.json`` on this package's classes.  ``--key value`` overrides a config item (JSON value
 or ``$expression``), e.g. ``--age 0.7 --brain_vol 0.5``; with no checkpoint files at hand,
 ``--load_autoencoder '$None' --load_diffusion '$None'`` samples from randomly initialised networks.
 """

@@ -12,7 +12,7 @@ The bundle is driven by ``python -m monai.bundle run <id> --config_file configs/
   then instantiate ``Class(**resolved kwargs)``;
 * anything else is a literal, resolved recursively.
 
-``_target_`` paths are remapped so the unmodified file lands on the B200 classes:
+``_target_`` paths are remapped so the unmodified file lands on this package's classes:
 ``generative.…`` → ``generativemodels_b200.…`` and the bundle's ``scripts.sampler.Sampler`` / ``scripts.saver.
 NiftiSaver`` → :mod:`generativemodels_b200.bundle`.  Nothing here touches the GPU; it is the thin app edge of
 SURVEY.md §8f rank 4, not a re-implementation of MONAI's bundle machinery (no ``_mode_``, no macros ``%``, no YAML).

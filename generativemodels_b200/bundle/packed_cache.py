@@ -1,6 +1,6 @@
 """Pre-packed weight cache file (SURVEY.md §8f rank 4: ``state_dict`` → packed-weight file).
 
-Every convolution / linear layer is repacked once into the K-major h16 tap matrices the tcgen05 implicit-GEMM kernel
+Every convolution / linear layer is repacked once into the K-major h16 tap matrices the wgmma implicit-GEMM kernel
 reads (ops.PackedConv and friends) the first time the network runs.  ``save_packed`` writes those packed objects of a
 *warm* network to one file; ``load_packed`` installs them into a freshly constructed network whose ``state_dict`` has
 the same fingerprint, so a serving process goes from ``load_state_dict`` to its first sample without the repacking

@@ -3,7 +3,7 @@ sampler.py:13-52): DDIM loop over a concat+cross-attention conditioned 3-D laten
 ``decode_stage_2_outputs``.  Same class name and ``sampling_fn`` signature, so the bundle's ``inference.json`` runs
 unchanged through :mod:`generativemodels_b200.bundle.config`.
 
-B200 specifics: the latent is 3x20x28x20 (11 200 voxels), so one UNet step is ~250 launches of a few microseconds —
+Performance notes: the latent is 3x20x28x20 (11 200 voxels), so one UNet step is ~250 launches of a few microseconds —
 the network is wrapped in a CUDA graph (one capture, 50 replays); the conditioning planes are broadcast once, not per
 step; the decoder (15 TFLOP of 64..128-channel 3-D convolutions at up to 160x224x160) runs once on the implicit-GEMM
 kernel.  The reference decodes under ``autocast`` (fp16 convolutions); here the decoder is 16-bit (fp16 by default) with fp32 accumulation

@@ -1,4 +1,4 @@
-// Shared helpers for libb200gen.so (sm_100a only).
+// Shared helpers for libb200gen.so (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -44,13 +44,11 @@ int sm_count();
 // stream may be scheduled as soon as every CTA of this one is resident) and pdl_wait() before its first global-memory
 // access (blocks until the preceding grid has COMPLETED and its writes are visible — so the data dependencies are
 // exactly those of plain stream order).  What overlaps is the next kernel's launch latency and prologue (barrier
-// initialisation, tensor-memory allocation, tensor-map fetch) with this kernel's execution: a latent-UNet step is
-// 150-300 dependent kernels of a few microseconds each (DESIGN.md, latency-bound configurations).
-// MEASURED (round 2, same box, graph-replayed samplers): it does not pay here — C2 at batch 1 85.2 -> 93.2 ms per
-// sample, C5 564 -> 605 ms per guided sample with the attribute on, the C3 step unchanged — the persistent tensor-core
-// kernels hold ~200 KB of shared memory per CTA, so a dependent grid can only start on SMs the running grid left idle
-// and its early-resident CTAs then spin in griddepcontrol.wait.  The launches therefore go out WITHOUT the attribute
-// by default (the device-side instructions are no-ops then); B200_PDL=1 turns it on for experiments.
+// initialisation, tensor-map fetch) with this kernel's execution: a latent-UNet step is 150-300 dependent kernels of
+// a few microseconds each.  The persistent tensor-core kernels hold ~200 KB of shared memory per CTA, so a dependent
+// grid can only start on SMs the running grid left idle and its early-resident CTAs then spin in griddepcontrol.wait.
+// The launches therefore go out WITHOUT the attribute by default (the device-side instructions are no-ops then);
+// B200_PDL=1 turns it on for experiments.
 // ------------------------------------------------------------------------------------------------
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
@@ -85,7 +83,7 @@ inline cudaError_t launch_cluster(void (*kernel)(KArgs...), int cluster_x, dim3 
     attr[n].val.programmaticStreamSerializationAllowed = 1;
     ++n;
   }
-  if (cluster_x > 1) {        // thread-block cluster of cluster_x CTAs along x (CTA pairs for tcgen05 cta_group::2)
+  if (cluster_x > 1) {        // thread-block cluster of cluster_x CTAs along x
     attr[n].id = cudaLaunchAttributeClusterDimension;
     attr[n].val.clusterDim.x = cluster_x;
     attr[n].val.clusterDim.y = 1;
@@ -117,7 +115,7 @@ __device__ __forceinline__ float apply_act(float x, int act) {
 
 // ------------------------------------------------------------------------------------------------
 // The library's 16-bit storage type ("h16") for activations and packed weights.  Default: IEEE fp16 — 11 significand
-// bits against bfloat16's 8, at the same tcgen05 kind::f16 rate and the same bytes; the reference-generated C2
+// bits against bfloat16's 8, at the same wgmma rate and the same bytes; the reference-generated C2
 // fixture (DESIGN.md section 3) needs the extra bits: an all-bf16 data path is 7.9e-2 off the fp32 reference at its
 // ill-conditioned probe, an all-fp16 one 7.8e-3.  fp32 -> fp16 conversions saturate (F2FP.SATFINITE: +-65504 instead
 // of inf), so an out-of-range activation degrades instead of poisoning the sample with NaNs.

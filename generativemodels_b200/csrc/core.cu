@@ -23,7 +23,7 @@ int sm_count() {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    if (n <= 0) n = 148;
+    if (n <= 0) n = 132;
   }
   return n;
 }
@@ -49,8 +49,8 @@ extern "C" int b200_device_check(void) {
   int major = 0, minor = 0;
   cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev);
   cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev);
-  if (major != 10) {
-    b200::set_error("libb200gen needs an sm_100-class GPU (tcgen05/TMEM); device %d is sm_%d%d", dev, major,
+  if (major != 9 || minor != 0) {
+    b200::set_error("libb200gen needs an sm_90 GPU (wgmma/TMA, built for sm_90a); device %d is sm_%d%d", dev, major,
                     minor);
     return B200_ENODEV;
   }

@@ -1,7 +1,7 @@
 // Batch-of-a-few-rows kernels for autoregressive decoding (VQVAETransformerInferer.sample, inferer.py:1183-1245).
 //
 // One new token per sequence means every linear layer is a GEMV: 2 * K * O FLOPs against K * O * 2 bytes of weights,
-// i.e. HBM/L2-bound by a factor of ~1000 — the 128-row tcgen05 tile of b200_igemm spends ~10 us of pipeline latency
+// i.e. HBM/L2-bound by a factor of ~1000 — the 128-row tensor-core tile of b200_igemm spends its pipeline latency
 // on 0.5 MFLOP.  These kernels read each weight row once with 16-byte loads, keep the (optionally LayerNorm-ed)
 // activation rows in shared memory and finish with the same fused epilogue (bias, GELU, residual), so a decode step
 // is ~100 launches of a few microseconds that replay from one CUDA graph.

@@ -210,7 +210,7 @@ __global__ void softmax_rows_kernel(const float* __restrict__ s, long long M, in
   for (long long c = S + t; c < p_pitch; c += TPR) pr[c] = f2h(0.f);
 }
 
-// One-pass variant: the score GEMM's epilogue already left (max, sum exp) per 256-column tile of every row, so the
+// One-pass variant: the score GEMM's epilogue already left (max, sum exp) per 128-column tile of every row, so the
 // row maximum and denominator come from a few hundred partials and the scores are read exactly once.
 __global__ void softmax_rows_partials_kernel(const float* __restrict__ s, int S, long long s_pitch,
                                              const float2* __restrict__ part, int n_tiles,
@@ -286,7 +286,7 @@ __global__ void timestep_embedding_kernel(const float* __restrict__ t, int N, in
 
 // one warp per output feature; loops over the (few) rows.  VEC: K % 128 == 0 and 16-byte aligned rows — every lane
 // issues all its float4 weight loads before the first FMA (a time-embedding projection is one 4 KB row per warp: the
-// scalar form spent ~15 us per call waiting on 32 dependent-latency loads).
+// scalar form waits on 32 dependent-latency loads).
 template <bool VEC>
 __global__ void small_linear_kernel(const float* __restrict__ x, int M, int K, const float* __restrict__ W,
                                     const float* __restrict__ b, int O, int act_in, int act_out,

@@ -1,68 +1,46 @@
-// Flash-style attention on tcgen05 for the large-T self-attention of the 3-D UNet (T = S = 89 600, one head of 512)
-// and every other head_dim in {64, 128, 256, 512} with S >= 64.
+// Flash-style attention on Hopper wgmma for every head_dim in {64, 128, 256, 512} (the large-T self-attention of the
+// 3-D UNet: T = S = 89 600, one head of 512).
 //
 // Replaces torch.baddbmm -> softmax -> torch.bmm (diffusion_model_unet.py:143-153, 406-416; autoencoderkl.py:261-269),
 // which materialise the T x S score matrix (29.9 GiB fp32 at T = 89 600).  Here the scores never leave the SM:
 //
-//   work item = (batch, head, 128-query tile, 256-wide slice of the value/output dimension)
-//   per 64-key block:   S  = Q K^T        tcgen05.mma  M=128 N=64,  K = head_dim in 64-wide chunks   -> TMEM (2 buffers)
-//                       P  = exp2(S*c - m) (fp32, online max / sum per row, one thread per row)      -> TMEM (bf16x2, 2 buffers)
-//                       O += P V          tcgen05.mma  M=128 N<=256, K=64, A operand read from TMEM     -> TMEM (256 columns)
-//   epilogue:           out = O / l (+ residual), bf16
+//   work item = (batch, head, 64-query tile, slice of up to 256 value/output channels); one warpgroup per CTA
+//   per 64-key block:   S  = Q K^T        wgmma m64n64k16, A and B from shared memory, K = head_dim   -> registers
+//                       P  = exp2(S*c - m) (fp32 online max / sum; a row lives in the four lanes of a quad)
+//                       O += P V          wgmma m64nDVk16, A = P straight from the S registers (16-bit), B = V^T tile
+//   epilogue:           out = O / l (+ residual), 16-bit
 //
-// A 128 x 512 fp32 accumulator would fill all 512 TMEM columns, so for head_dim 512 the output dimension is split in two
-// 256-wide slices handled by two work items that each recompute S (1.5x the QK^T FLOPs, but no score traffic at all).
-// The running maximum is only raised when it grows by more than 2^8 (lazy rescale), so rewriting O in TMEM is rare.
-//
-// P lives in tensor memory (like the scores) so that all shared memory not holding Q goes to the K ring: the kernel is
-// bound by TMA latency x bytes in flight, not by the tensor pipe (Q alone is 128 KB at head_dim 512).
-// Warp roles (192 threads): warp 0 = TMA producer (Q once per item, K chunks through an 8-stage ring, V^T tile),
-// warp 1 = MMA issuer, warps 2..5 = softmax + epilogue (thread <-> TMEM lane <-> query row).
+// A 64 x 512 fp32 accumulator would not fit the registers of one warpgroup, so for head_dim 512 the output dimension is
+// split in two 256-wide slices handled by two work items that each recompute S (1.5x the QK^T FLOPs, no score traffic).
+// Q stays in shared memory for the whole item; K and V^T have one buffer each: the next block's K is requested as soon
+// as S has been computed (it lands during the softmax and PV), the next V^T as soon as PV has been issued and retired.
 #include "common.cuh"
+#include "wgmma.cuh"
 #include <cuda.h>
 #include <cudaTypedefs.h>
 #include <mutex>
+#include <string.h>
 
 namespace b200 {
 
 struct FlashDev {
-  alignas(64) CUtensorMap tmQ;    // [B][T][C]      box (64 ch, 128 rows)
+  alignas(64) CUtensorMap tmQ;    // [B][T][C]      box (64 ch, 64 rows)
   alignas(64) CUtensorMap tmK;    // [B][S][C]      box (64 ch, 64 rows)
   alignas(64) CUtensorMap tmVt;   // [B][C][S]      box (64 keys, DV rows)
-  alignas(64) CUtensorMap tmP;    // [grid][n_kv * 128][64] probability slabs (replay variant): one contiguous 16 KB tile
-                                  // per key block, box (64 keys, 128 rows)
   int B, T, S, heads, dh, d_chunks, dv, n_dv;
   int q_tiles, n_items, n_kv;
   float scale_log2;
-  float rescale_thr;               // lazy-rescale threshold in log2 units (see kRescaleThreshold)
   h16* out;
   long long out_bstride, out_pitch;
   const h16* res;
   long long res_bstride, res_pitch;
-  h16* pslab;           // replay workspace: [grid][n_kv][128 rows][64 keys] — tile-contiguous, so that the
-                                  // warps' row stores coalesce to 4 KB runs and every TMA tile is one 16 KB burst
-                                  // (row-major [128][S] slabs made every tile 128 scattered 128-byte DRAM accesses)
-  long long p_pitch;              // elements per CTA slab = n_kv * 128 * 64
-  float* ev_fac;                  // [grid][4 warps][n_kv][32] logged rescale factors
-  int* ev_blk;                    // [grid][4 warps][n_kv]     block index of each logged rescale
 };
 
 namespace fa {
 
-static constexpr int kThreads = 192;
-static constexpr int kBM = 128, kBKV = 64;
-static constexpr int kKRingBytes = 64 * 1024;           // K ring: 4 stages x 2 chunks (or 8 x 1 for head_dim 64)
-static constexpr int kMaxKStages = 8;
-static constexpr int kQChunkBytes = kBM * 64 * 2;      // 16 KB
-static constexpr int kKChunkBytes = kBKV * 64 * 2;     // 8 KB: 64 keys x 64 channels
-// Lazy rescale: the reference maximum of a row is only raised when a block's maximum exceeds it by more than 2^thr,
-// so probabilities reach at most 2^thr.  12 keeps them far inside fp16's range (65504) and its 11-bit precision holds
-// for every p >= 6e-5; rows whose maximum drifts slowly (the common case on real activations) then never rescale, and a
-// work item without rescales runs its pass 2 ungated.  B200_FLASH_RESCALE overrides (dev A/B).
-static constexpr float kRescaleThreshold = 12.0f;      // log2 domain
-// The chain S_j -> softmax -> P_j -> PV_j is a latency chain (TMEM read, barrier hand-offs, TMEM write); the tensor pipe
-// only stays busy if independent work is queued behind it: QK^T runs kLookahead blocks ahead of PV.
-static constexpr int kSBuf = 3, kLookahead = 2;
+static constexpr int kThreads = 128;
+static constexpr int kBM = 64, kBKV = 64;
+static constexpr int kChunkBytes = 64 * 64 * 2;        // 8 KB: 64 rows x 64 channels
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
@@ -72,9 +50,6 @@ __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
 }
 __device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
 }
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   uint32_t done;
@@ -88,12 +63,6 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
         : "memory");
   } while (!done);
 }
-// role warps (TMA / MMA): one lane polls, the warp re-converges — 32 lanes spinning on the same barrier word only
-// steal issue slots and shared-memory bandwidth from the epilogue / softmax warps
-__device__ __forceinline__ void mbar_wait_warp(uint32_t bar, uint32_t parity) {
-  if ((threadIdx.x & 31) == 0) mbar_wait(bar, parity);
-  __syncwarp();
-}
 __device__ __forceinline__ void tma_load_3d(const CUtensorMap* tm, uint32_t bar, uint32_t dst, int c0, int c1, int c2) {
   asm volatile(
       "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes"
@@ -101,1177 +70,171 @@ __device__ __forceinline__ void tma_load_3d(const CUtensorMap* tm, uint32_t bar,
       "l"(reinterpret_cast<uint64_t>(tm)), "r"(bar), "r"(c0), "r"(c1), "r"(c2)
       : "memory");
 }
-__device__ __forceinline__ void tma_prefetch_3d(const CUtensorMap* tm, int c0, int c1, int c2) {
-  asm volatile("cp.async.bulk.prefetch.tensor.3d.L2.global.tile [%0, {%1, %2, %3}];" ::"l"(
-                   reinterpret_cast<uint64_t>(tm)),
-               "r"(c0), "r"(c1), "r"(c2)
-               : "memory");
-}
-__device__ __forceinline__ void fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void umma_h16(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t acc) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(acc)
-      : "memory");
-}
-// A operand from tensor memory (row = lane, two bf16 per 32-bit column), B from shared memory
-__device__ __forceinline__ void umma_h16_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t bdesc, uint32_t idesc, uint32_t acc) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "r"(a_tmem), "l"(bdesc), "r"(idesc), "r"(acc)
-      : "memory");
-}
-__device__ __forceinline__ uint64_t smem_desc(uint32_t addr) {      // K-major, SWIZZLE_128B, 8-row groups 1024 B apart
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((addr & 0x3FFFFu) >> 4);
-  d |= static_cast<uint64_t>(1) << 16;
-  d |= static_cast<uint64_t>(1024 >> 4) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
-  return d;
-}
-// the same descriptor split in its loop-invariant high word and an address-dependent low word, so the issue loop
-// only does 32-bit immediate adds
-static constexpr uint32_t kDescHi = (1024u >> 4) | (1u << 14) | (2u << 29);
-__device__ __forceinline__ uint32_t desc_lo(uint32_t addr) { return ((addr & 0x3FFFFu) >> 4) | (1u << 16); }
-__device__ __forceinline__ uint64_t desc64(uint32_t lo) { return (static_cast<uint64_t>(kDescHi) << 32) | lo; }
-__device__ __forceinline__ uint32_t idesc_h16(int M, int N) {
-  return (1u << 4) | (B200_H16_FMT << 7) | (B200_H16_FMT << 10) | (static_cast<uint32_t>(N >> 3) << 17) | (static_cast<uint32_t>(M >> 4) << 24);
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]),
-        "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]),
-        "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]),
-        "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t* r) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-      "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]), "r"(r[18]),
-      "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]),
-      "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-// One lane of a fully converged warp.  Issuing TMA / tcgen05 instructions under `if (elect_one())` instead of
-// `if (lane == 0)` lets the compiler keep their operands in uniform registers without a per-instruction
-// elect-and-loop sequence (the single-thread MMA issue rate bounds this kernel: its MMAs are only N = 64 wide).
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred;
-  asm volatile(
-      "{\n\t.reg .pred P1;\n\t"
-      "elect.sync _|P1, 0xFFFFFFFF;\n\t"
-      "selp.u32 %0, 1, 0, P1;\n\t}"
-      : "=r"(pred));
-  return pred != 0;
-}
-
 __device__ __forceinline__ float ex2_approx(float x) {
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
-
-struct Item { int b, h, qt, dvi; };
-template <bool REPLAY>
-__device__ __forceinline__ Item decode(const FlashDev& p, int item) {
-  Item it;
-  if constexpr (REPLAY) {
-    it.dvi = 0;                       // both output slices are handled inside the item (two passes)
-  } else {
-    it.dvi = item % p.n_dv; item /= p.n_dv;
-  }
-  it.qt = item % p.q_tiles; item /= p.q_tiles;
-  it.h = item % p.heads;
-  it.b = item / p.heads;
-  return it;
+__device__ __forceinline__ uint32_t pack_h2(float lo, float hi) {
+  h162 v = f2h2(lo, hi);
+  return *reinterpret_cast<uint32_t*>(&v);
 }
 
-__device__ __forceinline__ void stg256(void* ptr, const uint32_t* w) {
-  asm volatile("st.global.v8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(ptr), "r"(w[0]), "r"(w[1]), "r"(w[2]),
-               "r"(w[3]), "r"(w[4]), "r"(w[5]), "r"(w[6]), "r"(w[7])
-               : "memory");
-}
-
-// REPLAY (head_dim 512 with a workspace): instead of recomputing S = Q K^T and the softmax for the second 256-wide
-// output slice, pass 1 also writes its probability tiles P (bf16, exactly the values its own PV MMAs consume) to a
-// per-CTA slab in global memory, and pass 2 streams them back through TMA as the shared-memory A operand of
-// O2 += P V2 — a pure GEMM stream with no QK^T and no exponentials (2/3 of the recompute variant's tensor work).
-// The rare lazy-rescale events of pass 1 are logged per warp (block index + per-row factor) and replayed on O2 at
-// the same block positions, so both slices see bit-identical P and the same normaliser l.
-// dev ablation (-DFA_ABLATE=6): every K / V^T load re-reads key block 0, i.e. always hits L2
-#if defined(FA_ABLATE) && FA_ABLATE == 6
-#define FA_KVROW(j) 0
-#else
-#define FA_KVROW(j) (j)
-#endif
-
-// dev ablations (-DFA_ABLATE=n; results are wrong on purpose, only the timing means something):
-//   1 no K / V^T / P tile loads   2 no exp2   3 no slab stores   4 softmax warps only hand-shake
-//   5 no QK^T MMAs                6 all K / V^T loads hit key block 0 (L2)   7 no PV MMAs
-#ifdef FA_ABLATE
-#define FA_ABL(n) (FA_ABLATE == (n))
-#else
-#define FA_ABL(n) 0
-#endif
-
-#ifdef FA_TIMING
-#define FA_T(i) do { long long fa_now = clock64(); fa_acc[i] += fa_now - fa_last; fa_last = fa_now; } while (0)
-#else
-#define FA_T(i) do { } while (0)
-#endif
-
-template <int DCH, bool REPLAY>      // DCH = head_dim / 64
+template <int DCH, int DV>      // DCH = head_dim / 64; DV = output channels per work item
 __global__ void __launch_bounds__(kThreads, 1) flash_attn_kernel(const __grid_constant__ FlashDev p) {
-  constexpr int CPS = DCH >= 2 ? 2 : 1;               // 64-channel K chunks per ring stage
-  constexpr int NSTEP = DCH / CPS;                    // ring stages consumed per key block
-  constexpr int kKStages = kKRingBytes / (CPS * kKChunkBytes);
-  constexpr int kKStageBytes = CPS * kKChunkBytes;
-  constexpr int kRStageBytes = kQChunkBytes + 256 * kBKV * 2;     // replay stage: P tile (16 KB) + V^T slice (32 KB)
-  static_assert(!REPLAY || (DCH == 8 && kKStages * kRStageBytes <= DCH * kQChunkBytes + kKRingBytes + 256 * kBKV * 2),
-                "replay stages overlay the Q / K / V regions");
-  pdl_launch_dependents();
   extern __shared__ uint8_t smem_raw[];
-  const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t sQ = base;
-  const uint32_t sK = sQ + DCH * kQChunkBytes;
-  const uint32_t sV = sK + kKRingBytes;
-  const uint32_t bars = sV + p.dv * kBKV * 2;
-  // barrier slots (8 bytes each)
-  const uint32_t q_full = bars, q_empty = bars + 8;
-  auto k_full = [&](int s) { return bars + 16 + 8u * s; };
-  auto k_empty = [&](int s) { return bars + 16 + 8u * (kMaxKStages + s); };
-  const uint32_t v_full = bars + 16 + 8u * (2 * kMaxKStages), v_empty = v_full + 8;
-  auto s_full = [&](int b) { return v_empty + 8 + 8u * b; };       // kSBuf score buffers
-  auto s_empty = [&](int b) { return v_empty + 32 + 8u * b; };
-  auto p_full = [&](int b) { return v_empty + 56 + 8u * b; };
-  auto p_empty = [&](int b) { return v_empty + 72 + 8u * b; };
-  const uint32_t o_full = v_empty + 88, o_empty = o_full + 8;
-  const uint32_t p1_done = o_empty + 8;       // REPLAY: the softmax warps have written (and fenced) all P tiles
-  const uint32_t r_done = p1_done + 8;        // REPLAY: every pass-2 MMA has completed (stage buffers free)
-  const uint32_t tmem_slot = r_done + 8;
-  volatile uint32_t* tmem_slot_ptr = reinterpret_cast<volatile uint32_t*>(smem_raw + (tmem_slot - smem_u32(smem_raw)));
-  volatile int* ev_flags = reinterpret_cast<volatile int*>(tmem_slot_ptr + 2);   // REPLAY: [4] "this warp logged rescales"
+  const uint32_t q_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  const uint32_t k_base = q_base + DCH * kChunkBytes;
+  const uint32_t v_base = k_base + DCH * kChunkBytes;
+  const uint32_t bar = v_base + DV * kBKV * 2;
+  const uint32_t q_bar = bar, k_bar = bar + 8, v_bar = bar + 16;
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (warp == 0 && lane == 0) {
-    mbar_init(q_full, 1); mbar_init(q_empty, 1);
-    for (int s = 0; s < kKStages; ++s) { mbar_init(k_full(s), 1); mbar_init(k_empty(s), 1); }
-    mbar_init(v_full, 1); mbar_init(v_empty, 1);
-    for (int b = 0; b < kSBuf; ++b) { mbar_init(s_full(b), 1); mbar_init(s_empty(b), 4); }
-    for (int b = 0; b < 2; ++b) { mbar_init(p_full(b), 4); mbar_init(p_empty(b), 1); }
-    mbar_init(o_full, 1); mbar_init(o_empty, 4);
-    mbar_init(p1_done, 4); mbar_init(r_done, 1);
+  const int tid = threadIdx.x;
+  const int warp = tid >> 5, lane = tid & 31;
+  int x = blockIdx.x;
+  const int dvi = x % p.n_dv; x /= p.n_dv;
+  const int qt = x % p.q_tiles; x /= p.q_tiles;
+  const int h = x % p.heads;
+  const int b = x / p.heads;
+  const int q0 = qt * kBM;
+  const int qc = h * p.dh;                  // first channel of this head
+  const int vc = qc + dvi * DV;             // first output channel of this item
+
+  pdl_launch_dependents();
+  if (tid == 0) {
+    mbar_init(q_bar, 1);
+    mbar_init(k_bar, 1);
+    mbar_init(v_bar, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot), "r"(512u) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  fence_before();
   __syncthreads();
-  fence_after();
-  const uint32_t tmem = *tmem_slot_ptr;
   pdl_wait();
-  const uint32_t tO = tmem;              // columns [0, 256)
-  const uint32_t tS = tmem + 256;        // kSBuf = 3 score buffers of 64 columns
-  const uint32_t tP = tmem + 448;        // two 32-column probability buffers (bf16 pairs): 512 columns in all
+  if (tid == 0) {
+    mbar_expect_tx(q_bar, DCH * kChunkBytes);
+    for (int c = 0; c < DCH; ++c) tma_load_3d(&p.tmQ, q_bar, q_base + c * kChunkBytes, qc + 64 * c, q0, b);
+    mbar_expect_tx(k_bar, DCH * kChunkBytes);
+    for (int c = 0; c < DCH; ++c) tma_load_3d(&p.tmK, k_bar, k_base + c * kChunkBytes, qc + 64 * c, 0, b);
+    mbar_expect_tx(v_bar, DV * kBKV * 2);
+    tma_load_3d(&p.tmVt, v_bar, v_base, 0, vc, b);
+  }
 
-  const int n_kv = p.n_kv;
+  // rows r0 = 16 warp + lane / 4 and r0 + 8 of the tile; this lane's columns 8 j + 2 (lane % 4) + {0, 1}
+  float o[DV / 2];
+#pragma unroll
+  for (int i = 0; i < DV / 2; ++i) o[i] = 0.f;
+  float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;     // l: this lane's share of the row sums
+  const float sc = p.scale_log2;
+  mbar_wait(q_bar, 0);
 
-  if (warp == 0) {
-    // =========================== TMA producer (whole warp runs the loop; one elected lane issues) =====
-    {
-      int kst = 0; uint32_t kph = 0;
-      uint32_t vcount = 0, icount = 0;
-      for (int item = blockIdx.x; item < p.n_items; item += gridDim.x, ++icount) {
-        const Item it = decode<REPLAY>(p, item);
-        const int ch0 = it.h * p.dh;
-        // Q tile: reused by every key block of the item
-        if constexpr (REPLAY) mbar_wait_warp(r_done, (icount & 1) ^ 1u);      // previous item's replay stages drained
-        else mbar_wait_warp(q_empty, (icount & 1) ^ 1u);
-        if (elect_one()) {
-          mbar_expect_tx(q_full, DCH * kQChunkBytes);
+  for (int j = 0; j < p.n_kv; ++j) {
+    const uint32_t ph = j & 1;
+    float s[32];
+    mbar_wait(k_bar, ph);
+    wgmma_fence();
 #pragma unroll
-          for (int c = 0; c < DCH; ++c)
-            tma_load_3d(&p.tmQ, q_full, sQ + c * kQChunkBytes, ch0 + c * 64, it.qt * kBM, it.b);
-        }
-        __syncwarp();
-        // order matches the MMA warp's consumption: K_0, K_1, K_2, V_0, K_3, V_1, ...
-        for (int j = 0; j < n_kv + kLookahead; ++j) {
-          if (j < n_kv) {
+    for (int c = 0; c < DCH; ++c) {
+      const uint64_t qd = wgmma_desc(q_base + c * kChunkBytes), kd = wgmma_desc(k_base + c * kChunkBytes);
 #pragma unroll
-            for (int step = 0; step < NSTEP; ++step) {
-              mbar_wait_warp(k_empty(kst), kph ^ 1u);
-              if (elect_one()) {
-                if (FA_ABL(1)) { mbar_arrive(k_full(kst)); } else {
-                mbar_expect_tx(k_full(kst), kKStageBytes);
+      for (int kk = 0; kk < 4; ++kk) wgmma_ss<64>(s, qd + 2u * kk, kd + 2u * kk, (c | kk) != 0 ? 1u : 0u);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_touch<32>(s);
+    __syncthreads();                          // every warp's S is done with the K buffer
+    if (tid == 0 && j + 1 < p.n_kv) {
+      mbar_expect_tx(k_bar, DCH * kChunkBytes);
+      for (int c = 0; c < DCH; ++c) tma_load_3d(&p.tmK, k_bar, k_base + c * kChunkBytes, qc + 64 * c, (j + 1) * kBKV, b);
+    }
+
+    // online softmax in the log2 domain; keys past S (zero-filled by TMA) are masked out
+    const int key0 = j * kBKV + 2 * (lane & 3);
+    float mx0 = -INFINITY, mx1 = -INFINITY;
 #pragma unroll
-                for (int cc = 0; cc < CPS; ++cc)
-                  tma_load_3d(&p.tmK, k_full(kst), sK + kst * kKStageBytes + cc * kKChunkBytes,
-                              ch0 + (step * CPS + cc) * 64, FA_KVROW(j) * kBKV, it.b);
-                }
-              }
-              __syncwarp();
-              if (++kst == kKStages) { kst = 0; kph ^= 1u; }
-            }
-          }
-          if (j >= kLookahead) {
-            mbar_wait_warp(v_empty, (vcount & 1) ^ 1u);
-            if (elect_one()) {
-              if (FA_ABL(1)) { mbar_arrive(v_full); } else {
-              mbar_expect_tx(v_full, p.dv * kBKV * 2);
-              tma_load_3d(&p.tmVt, v_full, sV, FA_KVROW(j - kLookahead) * kBKV, ch0 + it.dvi * p.dv, it.b);
-              }
-            }
-            __syncwarp();
-            ++vcount;
-          }
-        }
-        if constexpr (REPLAY) {
-          // ---- pass 2: stream P tiles (this CTA's slab) and the second V^T slice through 48 KB stages that overlay
-          //      the Q / K / V regions: all pass-1 MMAs have completed (q_empty) and all P tiles are visible ----
-          mbar_wait_warp(q_empty, icount & 1);
-          mbar_wait_warp(p1_done, icount & 1);
-          // the slab comes back from HBM (148 slabs of 128 x S probabilities never fit L2): pull the tiles into L2
-          // kPrefetch blocks ahead of the 4-stage shared-memory pipeline so that its loads see L2 latency only
-          constexpr int kPrefetch = 24;
-          if (elect_one()) {
-            for (int j = 0; j < kPrefetch && j < n_kv; ++j) tma_prefetch_3d(&p.tmP, 0, j * kBM, blockIdx.x);
-          }
-          __syncwarp();
-          for (int j = 0; j < n_kv; ++j) {
-            mbar_wait_warp(k_empty(kst), kph ^ 1u);
-            if (elect_one()) {
-              if (j + kPrefetch < n_kv) tma_prefetch_3d(&p.tmP, 0, (j + kPrefetch) * kBM, blockIdx.x);
-              const uint32_t st = sQ + kst * kRStageBytes;
-              if (FA_ABL(1)) { mbar_arrive(k_full(kst)); } else {
-              mbar_expect_tx(k_full(kst), kRStageBytes);
-              tma_load_3d(&p.tmP, k_full(kst), st, 0, j * kBM, blockIdx.x);
-              tma_load_3d(&p.tmVt, k_full(kst), st + kQChunkBytes, j * kBKV, ch0 + 256, it.b);
-              }
-            }
-            __syncwarp();
-            if (++kst == kKStages) { kst = 0; kph ^= 1u; }
-          }
-        }
+    for (int n = 0; n < 8; ++n) {
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const bool ok = key0 + 8 * n + e < p.S;
+        s[4 * n + e] = ok ? s[4 * n + e] * sc : -INFINITY;
+        s[4 * n + 2 + e] = ok ? s[4 * n + 2 + e] * sc : -INFINITY;
+        mx0 = fmaxf(mx0, s[4 * n + e]);
+        mx1 = fmaxf(mx1, s[4 * n + 2 + e]);
       }
     }
-  } else if (warp == 1) {
-    // =========================== MMA issuer (whole warp runs the loop; one elected lane issues) ========
-    {
-      const uint32_t idesc_s = idesc_h16(kBM, kBKV);
-      const uint32_t idesc_o = idesc_h16(kBM, p.dv);
-      const uint32_t q_lo = desc_lo(sQ), k_lo = desc_lo(sK), v_lo = desc_lo(sV);
-      int kst = 0; uint32_t kph = 0;
-      uint32_t scount = 0;      // number of S blocks issued so far (global across items)
-      uint32_t pvcount = 0;     // number of P hand-offs consumed so far (pass 1 blocks + gated pass-2 blocks)
-      uint32_t vcount = 0;      // number of V^T tiles consumed from the single-tile buffer (pass 1 only)
-      uint32_t icount = 0, ocount = 0;
-      for (int item = blockIdx.x; item < p.n_items; item += gridDim.x, ++icount) {
-        mbar_wait_warp(q_full, icount & 1);
-        mbar_wait_warp(o_empty, (ocount & 1) ^ 1u);        // previous epilogue has drained O
-        ++ocount;
-        fence_after();
-        for (int j = 0; j < n_kv + kLookahead; ++j) {
-          if (j < n_kv) {
-            const int sb = scount % kSBuf;
-            mbar_wait_warp(s_empty(sb), ((scount / kSBuf) & 1) ^ 1u);
-            fence_after();
-            const uint32_t d_s = tS + sb * kBKV;
+    mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 1));
+    mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 2));
+    mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 1));
+    mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 2));
+    const float nm0 = fmaxf(m0, mx0), nm1 = fmaxf(m1, mx1);
+    // a row with no valid key so far keeps a finite reference so that no inf - inf appears
+    const float u0 = nm0 == -INFINITY ? 0.f : nm0, u1 = nm1 == -INFINITY ? 0.f : nm1;
+    const float a0 = ex2_approx(m0 - u0), a1 = ex2_approx(m1 - u1);
+    m0 = nm0;
+    m1 = nm1;
+    uint32_t pa[16];
+    float ps0 = 0.f, ps1 = 0.f;
 #pragma unroll
-            for (int step = 0; step < NSTEP; ++step) {
-              mbar_wait_warp(k_full(kst), kph);
-              fence_after();
-              if (elect_one()) {
-                const uint32_t b_lo = k_lo + kst * (kKStageBytes >> 4);
-#pragma unroll
-                for (int cc = 0; cc < CPS; ++cc) {
-#pragma unroll
-                  for (int kk = 0; kk < 4; ++kk)
-                    if (!FA_ABL(5)) umma_h16(d_s, desc64(q_lo + (step * CPS + cc) * (kQChunkBytes >> 4) + 2 * kk),
-                              desc64(b_lo + cc * (kKChunkBytes >> 4) + 2 * kk), idesc_s,
-                              (step | cc | kk) != 0 ? 1u : 0u);
-                }
-                umma_commit(k_empty(kst));
-                if (step == NSTEP - 1) umma_commit(s_full(sb));
-              }
-              __syncwarp();
-              if (++kst == kKStages) { kst = 0; kph ^= 1u; }
-            }
-            ++scount;
-          }
-          if (j >= kLookahead) {
-            const int pb = pvcount & 1;
-            mbar_wait_warp(p_full(pb), (pvcount >> 1) & 1);
-            mbar_wait_warp(v_full, vcount & 1);
-            fence_after();
-            if (elect_one()) {
-              const uint32_t a_tmem = tP + pb * 32;          // 16 bf16 = 8 columns per K step
-#pragma unroll
-              for (int kk = 0; kk < 4; ++kk)
-                if (!FA_ABL(7)) umma_h16_ts(tO, a_tmem + 8u * kk, desc64(v_lo + 2 * kk), idesc_o,
-                             (j > kLookahead || kk > 0) ? 1u : 0u);
-              umma_commit(v_empty);
-              umma_commit(p_empty(pb));
-              if (j == n_kv + kLookahead - 1) {
-                umma_commit(o_full);
-                umma_commit(q_empty);
-              }
-            }
-            __syncwarp();
-            ++pvcount;
-            ++vcount;
-          }
-        }
-        if constexpr (REPLAY) {
-          // ---- pass 2: O2 += P_j V2_j with both operands from shared memory; the softmax warps only gate each
-          //      block through p_full (after replaying a logged rescale on O2, if any) ----
-          mbar_wait_warp(p1_done, icount & 1);             // rescale flags of the four softmax warps are visible
-          const bool gated = (ev_flags[0] | ev_flags[1] | ev_flags[2] | ev_flags[3]) != 0;
-          mbar_wait_warp(o_empty, (ocount & 1) ^ 1u);      // pass-1 epilogue has drained O
-          ++ocount;
-          fence_after();
-          for (int j = 0; j < n_kv; ++j) {
-            const int pb = pvcount & 1;
-            mbar_wait_warp(k_full(kst), kph);
-            if (gated) mbar_wait_warp(p_full(pb), (pvcount >> 1) & 1);
-            fence_after();
-            if (elect_one()) {
-              const uint32_t a_lo = q_lo + kst * (kRStageBytes >> 4);
-              const uint32_t b_lo = a_lo + (kQChunkBytes >> 4);
-#pragma unroll
-              for (int kk = 0; kk < 4; ++kk)
-                if (!FA_ABL(7)) umma_h16(tO, desc64(a_lo + 2 * kk), desc64(b_lo + 2 * kk), idesc_o, (j > 0 || kk > 0) ? 1u : 0u);
-              umma_commit(k_empty(kst));
-              if (gated) umma_commit(p_empty(pb));
-              if (j == n_kv - 1) {
-                umma_commit(o_full);
-                umma_commit(r_done);
-              }
-            }
-            __syncwarp();
-            if (++kst == kKStages) { kst = 0; kph ^= 1u; }
-            if (gated) ++pvcount;
-          }
-        }
-      }
+    for (int n = 0; n < 8; ++n) {
+      const float p00 = ex2_approx(s[4 * n] - u0), p01 = ex2_approx(s[4 * n + 1] - u0);
+      const float p10 = ex2_approx(s[4 * n + 2] - u1), p11 = ex2_approx(s[4 * n + 3] - u1);
+      ps0 += p00 + p01;
+      ps1 += p10 + p11;
+      // A fragment of k16 step n / 2: {row r0, k lo}, {row r0 + 8, k lo}, {row r0, k hi}, {row r0 + 8, k hi}
+      pa[4 * (n >> 1) + 2 * (n & 1)] = pack_h2(p00, p01);
+      pa[4 * (n >> 1) + 2 * (n & 1) + 1] = pack_h2(p10, p11);
     }
-  } else {
-    // =========================== softmax + epilogue warps ===========================
-    const int q = warp & 3;
-    const int row = q * 32 + lane;
-    const uint32_t lane_addr = static_cast<uint32_t>(q * 32) << 16;
-#ifdef FA_TIMING
-    long long fa_acc[8] = {0, 0, 0, 0, 0, 0, 0, 0}, fa_last = clock64();
-#endif
-    uint32_t scount = 0;       // S buffers consumed (pass 1 blocks)
-    uint32_t pcount = 0;       // P hand-offs to the MMA warp (pass 1 and pass 2 blocks)
-    uint32_t ocount = 0;       // epilogues done
-    uint32_t icount = 0;
-    // REPLAY: this CTA's probability slab and this warp's rescale log
-    h16* slab_row = REPLAY ? p.pslab + (long long)blockIdx.x * p.p_pitch + row * kBKV : nullptr;
-    float* ev_fac = REPLAY ? p.ev_fac + ((long long)blockIdx.x * 4 + q) * (long long)n_kv * 32 : nullptr;
-    int* ev_blk = REPLAY ? p.ev_blk + ((long long)blockIdx.x * 4 + q) * (long long)n_kv : nullptr;
-    for (int item = blockIdx.x; item < p.n_items; item += gridDim.x, ++icount) {
-      const Item it = decode<REPLAY>(p, item);
-      float m_used = -INFINITY, l_run = 0.f;
-      int n_ev = 0;
-      for (int j = 0; j < n_kv; ++j, ++scount, ++pcount) {
-        const int sb = scount % kSBuf;
-        FA_T(0);
-        mbar_wait(s_full(sb), (scount / kSBuf) & 1);
-        fence_after();
-        FA_T(1);
-        uint32_t raw[64];
-#if FA_ABL(4)
+    l0 = l0 * a0 + ps0;
+    l1 = l1 * a1 + ps1;
 #pragma unroll
-        for (int c = 0; c < 64; ++c) raw[c] = 0u;
-#else
-        tmem_ld32(tS + lane_addr + sb * kBKV, raw);
-        tmem_ld32(tS + lane_addr + sb * kBKV + 32, raw + 32);
-        tmem_ld_wait();
-#endif
-        fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(s_empty(sb));     // S buffer may be overwritten by block j + 2
-        FA_T(2);
-        const int kv_valid = p.S - j * kBKV;          // columns >= kv_valid are TMA zero-fill
-        // row maximum with 8 independent chains (one warp per scheduler here: instruction-level parallelism is the
-        // only latency hiding there is); raw[] keeps the UNSCALED scores, the scale is folded into the exp2 FFMA
-        float mx8[8];
+    for (int n = 0; n < DV / 8; ++n) {
+      o[4 * n] *= a0; o[4 * n + 1] *= a0;
+      o[4 * n + 2] *= a1; o[4 * n + 3] *= a1;
+    }
+
+    mbar_wait(v_bar, ph);
+    wgmma_fence();
+    const uint64_t vd = wgmma_desc(v_base);
 #pragma unroll
-        for (int e = 0; e < 8; ++e) mx8[e] = -INFINITY;
-        if (kv_valid >= kBKV) {
-#pragma unroll
-          for (int c = 0; c < 64; ++c) mx8[c & 7] = fmaxf(mx8[c & 7], __uint_as_float(raw[c]));
-        } else {
-#pragma unroll
-          for (int c = 0; c < 64; ++c) {
-            const float sv = c < kv_valid ? __uint_as_float(raw[c]) : -INFINITY;
-            raw[c] = __float_as_uint(sv);
-            mx8[c & 7] = fmaxf(mx8[c & 7], sv);
-          }
-        }
-        const float mx = fmaxf(fmaxf(fmaxf(mx8[0], mx8[1]), fmaxf(mx8[2], mx8[3])),
-                               fmaxf(fmaxf(mx8[4], mx8[5]), fmaxf(mx8[6], mx8[7]))) * p.scale_log2;
-        // lazy rescale: only raise the reference maximum when it would grow by more than 2^8
-        const bool need = (mx > m_used + p.rescale_thr);
-        const float m_new = need ? mx : m_used;
-        const float factor = (need && m_used > -INFINITY) ? exp2f(m_used - m_new) : 1.0f;
-        const unsigned any = __ballot_sync(0xffffffffu, need && m_used > -INFINITY);
-        const int pb = pcount & 1;
-        FA_T(3);
-        FA_T(4);
-        if (any) {
-          // O holds blocks < j; PV of block j - 1 must have completed before it is rewritten
-          if (j >= 1) {
-            const uint32_t prev = pcount - 1;
-            mbar_wait(p_empty(prev & 1), (prev >> 1) & 1);
-          }
-          fence_after();
-          for (int c0 = 0; c0 < p.dv; c0 += 32) {
-            uint32_t o[32];
-            tmem_ld32(tO + lane_addr + c0, o);
-            tmem_ld_wait();
-#pragma unroll
-            for (int c = 0; c < 32; ++c) o[c] = __float_as_uint(__uint_as_float(o[c]) * factor);
-            tmem_st32(tO + lane_addr + c0, o);
-          }
-          tmem_st_wait();
-          fence_before();
-          if constexpr (REPLAY) {
-            ev_fac[(long long)n_ev * 32 + lane] = factor;
-            if (lane == 0) ev_blk[n_ev] = j;
-            ++n_ev;
-          }
-        }
-        l_run *= factor;
-        m_used = m_new;
-        // P (bf16 pairs) into tensor memory, where the PV MMA reads it as its A operand: this thread owns row `row`
-        // (= TMEM lane), word w holds keys 2w (low half) and 2w + 1.  p = 2^(s * c - m): one FFMA + one MUFU.EX2
-        // per element, 8 independent sum chains.
-        const float neg_m = -m_used;
-        float sum8[8];
-#pragma unroll
-        for (int e = 0; e < 8; ++e) sum8[e] = 0.f;
-        uint32_t pw[32];
-#pragma unroll
-        for (int w = 0; w < 32; ++w) {
-#if FA_ABL(4)
-          pw[w] = 0x3c003c00u; sum8[w & 7] += 2.0f; continue;
-#endif
-#if FA_ABL(2)
-          const float p0 = fmaf(__uint_as_float(raw[2 * w]), p.scale_log2, neg_m);
-          const float p1 = fmaf(__uint_as_float(raw[2 * w + 1]), p.scale_log2, neg_m);
-#else
-          const float p0 = ex2_approx(fmaf(__uint_as_float(raw[2 * w]), p.scale_log2, neg_m));
-          const float p1 = ex2_approx(fmaf(__uint_as_float(raw[2 * w + 1]), p.scale_log2, neg_m));
-#endif
-          sum8[(2 * w) & 7] += p0;
-          sum8[(2 * w + 1) & 7] += p1;
-          h162 h = f2h2(p0, p1);
-          pw[w] = *reinterpret_cast<uint32_t*>(&h);
-        }
-        FA_T(5);
-        // P buffer pb must have been consumed by the PV MMA two hand-offs ago; with QK^T running two blocks ahead that
-        // MMA sits behind QK_j in the pipe, so the wait comes as late as possible — after the exponentials
-        if (pcount >= 2) mbar_wait(p_empty(pb), ((pcount >> 1) & 1) ^ 1u);
-        if (!FA_ABL(4)) tmem_st32(tP + lane_addr + pb * 32, pw);
-        tmem_st_wait();
-        const float lsum = ((sum8[0] + sum8[1]) + (sum8[2] + sum8[3])) + ((sum8[4] + sum8[5]) + (sum8[6] + sum8[7]));
-        l_run += lsum;
-        fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(p_full(pb));
-        if constexpr (REPLAY) {
-          // the same 64 probabilities to this row of the slab (128 contiguous bytes), for pass 2 — after the hand-off,
-          // so that the releasing arrive above does not have to cover these stores
-          h16* dst = slab_row + (long long)j * (kBM * kBKV);
-#pragma unroll
-          for (int g = 0; g < 4; ++g) { if (!FA_ABL(3) && !FA_ABL(4)) stg256(dst + g * 16, pw + g * 8); }
-        }
-        FA_T(6);
-      }
-#ifdef FA_TIMING
-      if (blockIdx.x == 0 && warp == 2 && lane == 0 && item == blockIdx.x && REPLAY) {
-        for (int i = 0; i < 8; ++i) p.ev_fac[(long long)gridDim.x * 4 * n_kv * 32 - 8 + i] = (float)fa_acc[i];
-      }
-#endif
-      if constexpr (REPLAY) {
-        // make the slab visible to the TMA (async proxy) reads of pass 2, then release the producer
-        if (lane == 0) ev_flags[q] = n_ev > 0 ? 1 : 0;
-        __threadfence();
-        asm volatile("fence.proxy.async.global;" ::: "memory");
-        __syncwarp();
-        if (lane == 0) mbar_arrive(p1_done);
-      }
-      bool gated = false;
-      if constexpr (REPLAY) {
-        mbar_wait(p1_done, icount & 1);
-        gated = (ev_flags[0] | ev_flags[1] | ev_flags[2] | ev_flags[3]) != 0;
-      }
-      const float inv = 1.0f / l_run;
-      const int t = it.qt * kBM + row;
-      const bool ok = t < p.T;
-#pragma unroll 1
-      for (int pass = 0; pass < (REPLAY ? 2 : 1); ++pass) {
-        if (pass == 1 && gated) {
-          // ---- pass 2 of an item in which some warp logged a rescale: every block is gated through p_full (after
-          //      replaying this warp's own rescales on O2); items without rescales run pass 2 ungated ----
-          int e_next = 0;
-          int next_blk = (n_ev > 0) ? ev_blk[0] : 0x7fffffff;
-          for (int j = 0; j < n_kv; ++j, ++pcount) {
-            const int pb = pcount & 1;
-            if (pcount >= 2) mbar_wait(p_empty(pb), ((pcount >> 1) & 1) ^ 1u);
-            if (j == next_blk) {                      // warp-uniform; j >= 1 by construction
-              const uint32_t prev = pcount - 1;
-              mbar_wait(p_empty(prev & 1), (prev >> 1) & 1);
-              fence_after();
-              const float factor = ev_fac[(long long)e_next * 32 + lane];
-              for (int c0 = 0; c0 < p.dv; c0 += 32) {
-                uint32_t o[32];
-                tmem_ld32(tO + lane_addr + c0, o);
-                tmem_ld_wait();
-#pragma unroll
-                for (int c = 0; c < 32; ++c) o[c] = __float_as_uint(__uint_as_float(o[c]) * factor);
-                tmem_st32(tO + lane_addr + c0, o);
-              }
-              tmem_st_wait();
-              fence_before();
-              ++e_next;
-              next_blk = (e_next < n_ev) ? ev_blk[e_next] : 0x7fffffff;
-            }
-            __syncwarp();
-            if (lane == 0) mbar_arrive(p_full(pb));
-          }
-        }
-        // ---- epilogue: O / l (+ residual) -> bf16 ----
-        mbar_wait(o_full, ocount & 1);
-        ++ocount;
-        fence_after();
-        const long long col0 = (long long)it.h * p.dh + (long long)(REPLAY ? pass : it.dvi) * p.dv;
-        h16* orow = p.out + it.b * p.out_bstride + (long long)t * p.out_pitch + col0;
-        const h16* rrow = p.res ? p.res + it.b * p.res_bstride + (long long)t * p.res_pitch + col0 : nullptr;
-        for (int c0 = 0; c0 < p.dv; c0 += 32) {
-          uint32_t o[32];
-          tmem_ld32(tO + lane_addr + c0, o);
-          tmem_ld_wait();
-          if (ok) {
-#pragma unroll
-            for (int g = 0; g < 4; ++g) {
-              float f[8];
-#pragma unroll
-              for (int e = 0; e < 8; ++e) f[e] = __uint_as_float(o[g * 8 + e]) * inv;
-              if (rrow) {
-                float rf[8];
-                unpack8(__ldg(reinterpret_cast<const uint4*>(rrow + c0 + g * 8)), rf);
-#pragma unroll
-                for (int e = 0; e < 8; ++e) f[e] += rf[e];
-              }
-              *reinterpret_cast<uint4*>(orow + c0 + g * 8) = pack8(f);
-            }
-          }
-        }
-        fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(o_empty);
-      }
+    for (int kk = 0; kk < 4; ++kk) wgmma_rs<DV>(o, pa + 4 * kk, vd + 2u * kk, 1u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_touch<DV / 2>(o);
+    __syncthreads();                          // every warp's PV is done with the V^T buffer
+    if (tid == 0 && j + 1 < p.n_kv) {
+      mbar_expect_tx(v_bar, DV * kBKV * 2);
+      tma_load_3d(&p.tmVt, v_bar, v_base, (j + 1) * kBKV, vc, b);
     }
   }
-  fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(512u) : "memory");
-  }
-}
 
-// ================================================================================================================
-// CTA-pair variant for head_dim 512 (the 3-D UNet's T = S = 89 600 self-attention): tcgen05.mma.cta_group::2 over 256
-// queries per pair.
-//
-// Why: the single-CTA kernel above moves ~160 GB per call through the L2 -> SM path at T = S = 89 600 (every K and
-// V^T tile is fetched once per 128 queries, plus the probability replay) — ~10 TB/s, the fabric's limit, which is why
-// no tensor-side or latency-side change moved it (profiles/r1_attention_experiments.txt).  With a pair, each CTA keeps
-// its own 128 query rows (Q tile, scores, probabilities and output in its own shared / tensor memory) but the B
-// operands of every MMA are SPLIT across the pair: for QK^T each CTA stages 32 of the block's 64 keys, for PV the V^T
-// rows of 128 of the 256 output channels.  K / V^T traffic per query halves (160 -> 96 GB per call), the same 96 KB of
-// rings holds two key blocks in flight instead of one, and one issuing thread drives both SMs' tensor pipes.
-// Protocol: every barrier the issuing thread waits on lives in the leader CTA (rank 0) — TMA of both CTAs completes on
-// the leader's barrier (cp.async.bulk.tensor.cta_group::2), the peer's softmax warps arrive remotely — and every
-// barrier the softmax / producer warps wait on is signalled in BOTH CTAs by tcgen05.commit ... multicast::cluster.
-// The two-pass structure (pass 1: flash loop for output channels 0..255 + P tiles to a per-CTA slab; pass 2: replay
-// P x V^T[256..511]) and the rescale-event log are those of flash_attn_kernel<8, true>.
-// ================================================================================================================
-#ifndef B200_FLASH_PAIR_DEFAULT
-#define B200_FLASH_PAIR_DEFAULT 1
-#endif
-static constexpr uint32_t kPeerMask = 0xFEFFFFFFu;      // clears the CTA-rank bit of a shared::cluster address -> leader
-
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// arrive on a barrier given by its shared::cluster address.  The per-block hand-offs (s_empty / p_full / o_empty) publish
-// nothing through memory — scores and probabilities travel through tensor memory, ordered by tcgen05.wait + fence — so
-// they use the default semantics (release at CTA scope).  A release at CLUSTER scope makes the arrive wait until the
-// thread's earlier global stores (the probability slab, 128 B per thread and block) are visible cluster-wide: measured
-// 4.6 ms of a 20.5 ms call (profiles/r2_attention_ablations.txt).  Only p1_done, which publishes the remote flag
-// words and the slab, uses the cluster-scope form.
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t bar_cluster_addr) {
-  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(bar_cluster_addr) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive_cluster_release(uint32_t bar_cluster_addr) {
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(bar_cluster_addr) : "memory");
-}
-__device__ __forceinline__ void mbar_wait_cluster(uint32_t bar, uint32_t parity) {
-  uint32_t done;
-  do {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(done)
-        : "r"(bar), "r"(parity)
-        : "memory");
-  } while (!done);
-}
-__device__ __forceinline__ void mbar_wait_cluster_warp(uint32_t bar, uint32_t parity) {
-  if ((threadIdx.x & 31) == 0) mbar_wait_cluster(bar, parity);
-  __syncwarp();
-}
-__device__ __forceinline__ uint32_t mapa_u32(uint32_t addr, uint32_t rank) {
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(addr), "r"(rank));
-  return r;
-}
-__device__ __forceinline__ void st_cluster_u32(uint32_t addr, uint32_t v) {
-  asm volatile("st.shared::cluster.u32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
-}
-// TMA load of this CTA's half of a pair operand: data into OWN shared memory, bytes counted on the LEADER's barrier
-__device__ __forceinline__ void tma_load_3d_pair(const CUtensorMap* tm, uint32_t bar, uint32_t dst, int c0, int c1, int c2) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4, %5}], [%2];" ::"r"(dst),
-      "l"(reinterpret_cast<uint64_t>(tm)), "r"(bar & kPeerMask), "r"(c0), "r"(c1), "r"(c2)
-      : "memory");
-}
-__device__ __forceinline__ void umma2_commit(uint32_t bar) {      // arrives on the same barrier offset in both CTAs
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(bar),
-               "h"((uint16_t)3)
-               : "memory");
-}
-__device__ __forceinline__ void umma2_h16(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t acc) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(acc)
-      : "memory");
-}
-__device__ __forceinline__ void umma2_h16_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t bdesc, uint32_t idesc, uint32_t acc) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], [%1], %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "r"(a_tmem), "l"(bdesc), "r"(idesc), "r"(acc)
-      : "memory");
-}
-
-static constexpr int kPKeysCta = kBKV / 2;                    // keys of a block staged by each CTA
-static constexpr int kPKChunkBytes = kPKeysCta * 64 * 2;      // 4 KB: 32 keys x 64 channels
-static constexpr int kPKStageBytes = 4 * kPKChunkBytes;       // 16 KB: four channel chunks
-static constexpr int kPKStages = kKRingBytes / kPKStageBytes; // 4 stages = two key blocks in flight
-static constexpr int kPVRows = 128;                           // V^T rows (output channels) staged by each CTA
-static constexpr int kPVBytes = kPVRows * kBKV * 2;           // 16 KB
-static constexpr int kPVStages = 2;
-static constexpr int kPRStageBytes = kQChunkBytes + kPVBytes; // pass-2 stage: own P tile 16 KB + V^T half 16 KB
-static constexpr int kPRStages = 7;                           // 224 KB overlaying Q | K ring | V^T
-static_assert(kPRStages * kPRStageBytes <= 8 * kQChunkBytes + kKRingBytes + kPVStages * kPVBytes, "pass-2 overlay");
-template <int DCH>
-constexpr int pair_smem() { return DCH * kQChunkBytes + kKRingBytes + kPVStages * kPVBytes + 1024 + 1024; }
-
-// DCH = head_dim / 64 (8: head_dim 512, two passes with the probability replay; 4: head_dim 256, one pass, no slab)
-template <int DCH, bool REPLAY>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(kThreads, 1)
-flash_pair_kernel(const __grid_constant__ FlashDev p) {
-  static_assert((DCH == 8 && REPLAY) || (DCH == 4 && !REPLAY), "pair kernel: head_dim 512 with replay or head_dim 256");
-  constexpr int kPDCH = DCH;
-  constexpr int kPKSteps = DCH / 4;                     // ring stages per key block
-  pdl_launch_dependents();
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t sQ = base;
-  const uint32_t sK = sQ + kPDCH * kQChunkBytes;
-  const uint32_t sV = sK + kKRingBytes;
-  const uint32_t bars = sV + kPVStages * kPVBytes;
-  // barrier slots (8 bytes each, identical offsets in both CTAs).  "leader": only rank 0's copy is used.
-  int off = 0;
-  auto take = [&](int n) { const uint32_t a = bars + 8u * off; off += n; return a; };
-  const uint32_t q_full = take(1), q_empty = take(1);            // leader (TMA of both CTAs) / both (commit)
-  const uint32_t k_full0 = take(kPKStages), k_empty0 = take(kPKStages);
-  const uint32_t v_full0 = take(kPVStages), v_empty0 = take(kPVStages);
-  const uint32_t r_full0 = take(kPRStages), r_empty0 = take(kPRStages);
-  const uint32_t s_full0 = take(kSBuf), s_empty0 = take(kSBuf);   // both (commit) / leader (8 softmax warps)
-  const uint32_t p_full0 = take(2), p_empty0 = take(2);           // leader (8) / both (commit)
-  const uint32_t o_full = take(1), o_empty = take(1);             // both (commit) / leader (8)
-  const uint32_t p1_done = take(1);   // both, 8 arrivals each: every P tile of the pair is written, flags exchanged
-  const uint32_t r_done = take(1);    // both (commit): every pass-2 MMA has completed
-  const uint32_t tmem_slot = take(1);
-  const uint32_t ev_flags_addr = take(4);                          // int[8]: warps of rank 0, then rank 1
-  auto k_full = [&](int s) { return k_full0 + 8u * s; };
-  auto k_empty = [&](int s) { return k_empty0 + 8u * s; };
-  auto v_full = [&](int s) { return v_full0 + 8u * s; };
-  auto v_empty = [&](int s) { return v_empty0 + 8u * s; };
-  auto r_full = [&](int s) { return r_full0 + 8u * s; };
-  auto r_empty = [&](int s) { return r_empty0 + 8u * s; };
-  auto s_full = [&](int b) { return s_full0 + 8u * b; };
-  auto s_empty = [&](int b) { return s_empty0 + 8u * b; };
-  auto p_full = [&](int b) { return p_full0 + 8u * b; };
-  auto p_empty = [&](int b) { return p_empty0 + 8u * b; };
-  volatile uint32_t* tmem_slot_ptr = reinterpret_cast<volatile uint32_t*>(smem_raw + (tmem_slot - smem_u32(smem_raw)));
-  volatile int* ev_flags = reinterpret_cast<volatile int*>(smem_raw + (ev_flags_addr - smem_u32(smem_raw)));
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  const bool leader = rank == 0;
-  const int pair_id = blockIdx.x >> 1, n_pairs = gridDim.x >> 1;
-  if (warp == 0 && lane == 0) {
-    mbar_init(q_full, 1); mbar_init(q_empty, 1);
-    for (int s = 0; s < kPKStages; ++s) { mbar_init(k_full(s), 1); mbar_init(k_empty(s), 1); }
-    for (int s = 0; s < kPVStages; ++s) { mbar_init(v_full(s), 1); mbar_init(v_empty(s), 1); }
-    for (int s = 0; s < kPRStages; ++s) { mbar_init(r_full(s), 1); mbar_init(r_empty(s), 1); }
-    for (int b = 0; b < kSBuf; ++b) { mbar_init(s_full(b), 1); mbar_init(s_empty(b), 8); }
-    for (int b = 0; b < 2; ++b) { mbar_init(p_full(b), 8); mbar_init(p_empty(b), 1); }
-    mbar_init(o_full, 1); mbar_init(o_empty, 8);
-    mbar_init(p1_done, 8); mbar_init(r_done, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-  }
-  if (warp == 1) {      // the same warp of both CTAs: one pair-wide allocation of all 512 columns
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot), "r"(512u) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-  }
-  fence_before();
-  __syncthreads();
-  cluster_sync_all();                    // the peer's barriers exist before anything signals them remotely
-  fence_after();
-  const uint32_t tmem = *tmem_slot_ptr;
-  pdl_wait();
-  const uint32_t tO = tmem, tS = tmem + 256, tP = tmem + 448;
-  const int n_kv = p.n_kv;
-  const int pair_tiles = (p.q_tiles + 1) >> 1;               // pair items per (batch, head)
-
-  if (warp == 0) {
-    // =========================== TMA producer (both CTAs: own Q rows, own half of every B operand) ===========
-    int kst = 0; uint32_t kph = 0;
-    int rst = 0; uint32_t rph = 0;
-    uint32_t vcount = 0, icount = 0;
-    for (int item = pair_id; item < p.n_items; item += n_pairs, ++icount) {
-      const int pt = item % pair_tiles, bh = item / pair_tiles;
-      const int h = bh % p.heads, b = bh / p.heads;
-      const int qt = 2 * pt + (int)rank;
-      const int ch0 = h * p.dh;
-      // previous item's smem is free: all pass-2 MMAs (replay) / all pass-1 MMAs done — signalled in both CTAs
-      mbar_wait_warp(REPLAY ? r_done : q_empty, (icount & 1) ^ 1u);
-      if (elect_one()) {
-        if (leader) mbar_expect_tx(q_full, 2 * kPDCH * kQChunkBytes);
+  l0 += __shfl_xor_sync(0xffffffffu, l0, 1);
+  l0 += __shfl_xor_sync(0xffffffffu, l0, 2);
+  l1 += __shfl_xor_sync(0xffffffffu, l1, 1);
+  l1 += __shfl_xor_sync(0xffffffffu, l1, 2);
+  const float inv0 = 1.f / l0, inv1 = 1.f / l1;
+  const int r0 = 16 * warp + (lane >> 2);
 #pragma unroll
-        for (int c = 0; c < kPDCH; ++c)
-          tma_load_3d_pair(&p.tmQ, q_full, sQ + c * kQChunkBytes, ch0 + c * 64, qt * kBM, b);
+  for (int half = 0; half < 2; ++half) {
+    const int t = q0 + r0 + 8 * half;
+    if (t >= p.T) continue;
+    const float inv = half ? inv1 : inv0;
+    h16* orow = p.out + (long long)b * p.out_bstride + (long long)t * p.out_pitch + vc;
+    const h16* rrow = p.res ? p.res + (long long)b * p.res_bstride + (long long)t * p.res_pitch + vc : nullptr;
+#pragma unroll
+    for (int n = 0; n < DV / 8; ++n) {
+      const int col = 8 * n + 2 * (lane & 3);
+      float v0 = o[4 * n + 2 * half] * inv, v1 = o[4 * n + 2 * half + 1] * inv;
+      if (rrow) {
+        const float2 r = h22f2(*reinterpret_cast<const h162*>(rrow + col));
+        v0 += r.x;
+        v1 += r.y;
       }
-      __syncwarp();
-      for (int j = 0; j < n_kv + kLookahead; ++j) {
-        if (j < n_kv) {
-#pragma unroll
-          for (int step = 0; step < kPKSteps; ++step) {
-            mbar_wait_warp(k_empty(kst), kph ^ 1u);
-            if (elect_one()) {
-              if (FA_ABL(1)) { if (leader) mbar_arrive(k_full(kst)); } else {
-              if (leader) mbar_expect_tx(k_full(kst), 2 * kPKStageBytes);
-#pragma unroll
-              for (int cc = 0; cc < 4; ++cc)
-                tma_load_3d_pair(&p.tmK, k_full(kst), sK + kst * kPKStageBytes + cc * kPKChunkBytes,
-                                 ch0 + (step * 4 + cc) * 64, FA_KVROW(j) * kBKV + (int)rank * kPKeysCta, b);
-              }
-            }
-            __syncwarp();
-            if (++kst == kPKStages) { kst = 0; kph ^= 1u; }
-          }
-        }
-        if (j >= kLookahead) {
-          const int vs = vcount & 1;
-          mbar_wait_warp(v_empty(vs), ((vcount >> 1) & 1) ^ 1u);
-          if (elect_one()) {
-            if (FA_ABL(1)) { if (leader) mbar_arrive(v_full(vs)); } else {
-            if (leader) mbar_expect_tx(v_full(vs), 2 * kPVBytes);
-            tma_load_3d_pair(&p.tmVt, v_full(vs), sV + vs * kPVBytes, FA_KVROW(j - kLookahead) * kBKV,
-                             ch0 + (int)rank * kPVRows, b);
-            }
-          }
-          __syncwarp();
-          ++vcount;
-        }
-      }
-      if constexpr (REPLAY) {
-      // ---- pass 2: own P tiles + own half of V^T[256..511] through 32 KB stages overlaying Q | K ring | V^T ----
-      mbar_wait_warp(q_empty, icount & 1);                   // every pass-1 MMA of the pair has completed
-      mbar_wait_cluster_warp(p1_done, icount & 1);           // all P tiles written and fenced
-      constexpr int kPrefetch = 24;
-      if (elect_one()) {
-        for (int j = 0; j < kPrefetch && j < n_kv; ++j) tma_prefetch_3d(&p.tmP, 0, j * kBM, blockIdx.x);
-      }
-      __syncwarp();
-      for (int j = 0; j < n_kv; ++j) {
-        mbar_wait_warp(r_empty(rst), rph ^ 1u);
-        if (elect_one()) {
-          if (j + kPrefetch < n_kv) tma_prefetch_3d(&p.tmP, 0, (j + kPrefetch) * kBM, blockIdx.x);
-          const uint32_t st = sQ + rst * kPRStageBytes;
-          if (FA_ABL(1)) { if (leader) mbar_arrive(r_full(rst)); } else {
-          if (leader) mbar_expect_tx(r_full(rst), 2 * kPRStageBytes);
-          tma_load_3d_pair(&p.tmP, r_full(rst), st, 0, j * kBM, blockIdx.x);
-          tma_load_3d_pair(&p.tmVt, r_full(rst), st + kQChunkBytes, FA_KVROW(j) * kBKV, ch0 + 256 + (int)rank * kPVRows, b);
-          }
-        }
-        __syncwarp();
-        if (++rst == kPRStages) { rst = 0; rph ^= 1u; }
-      }
-      }
-    }
-  } else if (warp == 1) {
-    // =========================== MMA issuer: the leader's warp drives both SMs ===========================
-    if (leader) {
-      const uint32_t idesc_s = idesc_h16(2 * kBM, kBKV);          // S[256 x 64]: 128 rows and 32 keys per CTA
-      const uint32_t idesc_o = idesc_h16(2 * kBM, 256);           // O[256 x 256]: 128 rows and 128 channels per CTA
-      const uint32_t q_lo = desc_lo(sQ), k_lo = desc_lo(sK), v_lo = desc_lo(sV);
-      int kst = 0; uint32_t kph = 0;
-      int rst = 0; uint32_t rph = 0;
-      uint32_t scount = 0, pvcount = 0, vcount = 0, icount = 0, ocount = 0;
-      for (int item = pair_id; item < p.n_items; item += n_pairs, ++icount) {
-        mbar_wait_warp(q_full, icount & 1);
-        mbar_wait_warp(o_empty, (ocount & 1) ^ 1u);    // both CTAs' epilogues have drained O
-        ++ocount;
-        fence_after();
-        for (int j = 0; j < n_kv + kLookahead; ++j) {
-          if (j < n_kv) {
-            const int sb = scount % kSBuf;
-            mbar_wait_warp(s_empty(sb), ((scount / kSBuf) & 1) ^ 1u);
-            fence_after();
-            const uint32_t d_s = tS + sb * kBKV;
-#pragma unroll
-            for (int step = 0; step < kPKSteps; ++step) {
-              mbar_wait_warp(k_full(kst), kph);
-              fence_after();
-              if (elect_one()) {
-                const uint32_t b_lo = k_lo + kst * (kPKStageBytes >> 4);
-#pragma unroll
-                for (int cc = 0; cc < 4; ++cc) {
-#pragma unroll
-                  for (int kk = 0; kk < 4; ++kk)
-                    if (!FA_ABL(5)) umma2_h16(d_s, desc64(q_lo + (step * 4 + cc) * (kQChunkBytes >> 4) + 2 * kk),
-                              desc64(b_lo + cc * (kPKChunkBytes >> 4) + 2 * kk), idesc_s,
-                              (step | cc | kk) != 0 ? 1u : 0u);
-                }
-                umma2_commit(k_empty(kst));
-                if (step == kPKSteps - 1) umma2_commit(s_full(sb));
-              }
-              __syncwarp();
-              if (++kst == kPKStages) { kst = 0; kph ^= 1u; }
-            }
-            ++scount;
-          }
-          if (j >= kLookahead) {
-            const int pb = pvcount & 1, vs = vcount & 1;
-            mbar_wait_warp(p_full(pb), (pvcount >> 1) & 1);
-            mbar_wait_warp(v_full(vs), (vcount >> 1) & 1);
-            fence_after();
-            if (elect_one()) {
-              const uint32_t a_tmem = tP + pb * 32;
-              const uint32_t b_lo = v_lo + vs * (kPVBytes >> 4);
-#pragma unroll
-              for (int kk = 0; kk < 4; ++kk)
-                if (!FA_ABL(7)) umma2_h16_ts(tO, a_tmem + 8u * kk, desc64(b_lo + 2 * kk), idesc_o, (j > kLookahead || kk > 0) ? 1u : 0u);
-              umma2_commit(v_empty(vs));
-              umma2_commit(p_empty(pb));
-              if (j == n_kv + kLookahead - 1) {
-                umma2_commit(o_full);
-                umma2_commit(q_empty);
-              }
-            }
-            __syncwarp();
-            ++pvcount;
-            ++vcount;
-          }
-        }
-        if constexpr (REPLAY) {
-        // ---- pass 2 ----
-        mbar_wait_cluster_warp(p1_done, icount & 1);           // rescale flags of all eight softmax warps are visible
-        bool gated = false;
-#pragma unroll
-        for (int e = 0; e < 8; ++e) gated |= ev_flags[e] != 0;
-        mbar_wait_warp(o_empty, (ocount & 1) ^ 1u);    // pass-1 epilogues have drained O
-        ++ocount;
-        fence_after();
-        for (int j = 0; j < n_kv; ++j) {
-          const int pb = pvcount & 1;
-          mbar_wait_warp(r_full(rst), rph);
-          if (gated) mbar_wait_warp(p_full(pb), (pvcount >> 1) & 1);
-          fence_after();
-          if (elect_one()) {
-            const uint32_t a_lo = q_lo + rst * (kPRStageBytes >> 4);
-            const uint32_t b_lo = a_lo + (kQChunkBytes >> 4);
-#pragma unroll
-            for (int kk = 0; kk < 4; ++kk)
-              if (!FA_ABL(7)) umma2_h16(tO, desc64(a_lo + 2 * kk), desc64(b_lo + 2 * kk), idesc_o, (j > 0 || kk > 0) ? 1u : 0u);
-            umma2_commit(r_empty(rst));
-            if (gated) umma2_commit(p_empty(pb));
-            if (j == n_kv - 1) {
-              umma2_commit(o_full);
-              umma2_commit(r_done);
-            }
-          }
-          __syncwarp();
-          if (++rst == kPRStages) { rst = 0; rph ^= 1u; }
-          if (gated) ++pvcount;
-        }
-        }
-      }
-    }
-  } else {
-    // =========================== softmax + epilogue warps (both CTAs, own 128 rows) ===========================
-    const int q = warp & 3;
-    const int row = q * 32 + lane;
-    const uint32_t lane_addr = static_cast<uint32_t>(q * 32) << 16;
-    // shared::cluster addresses of the LEADER's copies of the barriers these warps arrive on, and of both CTAs'
-    // p1_done / flag words
-    const uint32_t l_s_empty0 = s_empty0 & kPeerMask, l_p_full0 = p_full0 & kPeerMask, l_o_empty = o_empty & kPeerMask;
-    const uint32_t p1_done_a[2] = {mapa_u32(p1_done, 0), mapa_u32(p1_done, 1)};
-    const uint32_t flag_a[2] = {mapa_u32(ev_flags_addr + 4u * (rank * 4 + q), 0), mapa_u32(ev_flags_addr + 4u * (rank * 4 + q), 1)};
-    uint32_t scount = 0, pcount = 0, ocount = 0, icount = 0;
-    h16* slab_row = REPLAY ? p.pslab + (long long)blockIdx.x * p.p_pitch + row * kBKV : nullptr;
-    float* ev_fac = REPLAY ? p.ev_fac + ((long long)blockIdx.x * 4 + q) * (long long)n_kv * 32 : nullptr;
-    int* ev_blk = REPLAY ? p.ev_blk + ((long long)blockIdx.x * 4 + q) * (long long)n_kv : nullptr;
-    for (int item = pair_id; item < p.n_items; item += n_pairs, ++icount) {
-      const int pt = item % pair_tiles, bh = item / pair_tiles;
-      const int h = bh % p.heads, b = bh / p.heads;
-      const int qt = 2 * pt + (int)rank;
-      float m_used = -INFINITY, l_run = 0.f;
-      int n_ev = 0;
-      for (int j = 0; j < n_kv; ++j, ++scount, ++pcount) {
-        const int sb = scount % kSBuf;
-        mbar_wait(s_full(sb), (scount / kSBuf) & 1);
-        fence_after();
-        uint32_t raw[64];
-#if FA_ABL(4)
-#pragma unroll
-        for (int c = 0; c < 64; ++c) raw[c] = 0u;
-#else
-        tmem_ld32(tS + lane_addr + sb * kBKV, raw);
-        tmem_ld32(tS + lane_addr + sb * kBKV + 32, raw + 32);
-        tmem_ld_wait();
-#endif
-        fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive_cluster(l_s_empty0 + 8u * sb);
-        const int kv_valid = p.S - j * kBKV;
-        float mx8[8];
-#pragma unroll
-        for (int e = 0; e < 8; ++e) mx8[e] = -INFINITY;
-        if (kv_valid >= kBKV) {
-#pragma unroll
-          for (int c = 0; c < 64; ++c) mx8[c & 7] = fmaxf(mx8[c & 7], __uint_as_float(raw[c]));
-        } else {
-#pragma unroll
-          for (int c = 0; c < 64; ++c) {
-            const float sv = c < kv_valid ? __uint_as_float(raw[c]) : -INFINITY;
-            raw[c] = __float_as_uint(sv);
-            mx8[c & 7] = fmaxf(mx8[c & 7], sv);
-          }
-        }
-        const float mx = fmaxf(fmaxf(fmaxf(mx8[0], mx8[1]), fmaxf(mx8[2], mx8[3])),
-                               fmaxf(fmaxf(mx8[4], mx8[5]), fmaxf(mx8[6], mx8[7]))) * p.scale_log2;
-        const bool need = (mx > m_used + p.rescale_thr);
-        const float m_new = need ? mx : m_used;
-        const float factor = (need && m_used > -INFINITY) ? exp2f(m_used - m_new) : 1.0f;
-        const unsigned any = __ballot_sync(0xffffffffu, need && m_used > -INFINITY);
-        const int pb = pcount & 1;
-        if (any) {
-          if (j >= 1) {            // O holds blocks < j: the PV of block j - 1 must have completed before O is rewritten
-            const uint32_t prev = pcount - 1;
-            mbar_wait(p_empty(prev & 1), (prev >> 1) & 1);
-          }
-          fence_after();
-          for (int c0 = 0; c0 < 256; c0 += 32) {
-            uint32_t o[32];
-            tmem_ld32(tO + lane_addr + c0, o);
-            tmem_ld_wait();
-#pragma unroll
-            for (int c = 0; c < 32; ++c) o[c] = __float_as_uint(__uint_as_float(o[c]) * factor);
-            tmem_st32(tO + lane_addr + c0, o);
-          }
-          tmem_st_wait();
-          fence_before();
-          if constexpr (REPLAY) {
-            ev_fac[(long long)n_ev * 32 + lane] = factor;
-            if (lane == 0) ev_blk[n_ev] = j;
-            ++n_ev;
-          }
-        }
-        l_run *= factor;
-        m_used = m_new;
-        const float neg_m = -m_used;
-        float sum8[8];
-#pragma unroll
-        for (int e = 0; e < 8; ++e) sum8[e] = 0.f;
-        uint32_t pw[32];
-#pragma unroll
-        for (int w = 0; w < 32; ++w) {
-#if FA_ABL(4)
-          pw[w] = 0x3c003c00u; sum8[w & 7] += 2.0f; continue;
-#endif
-#if FA_ABL(2)
-          const float p0 = fmaf(__uint_as_float(raw[2 * w]), p.scale_log2, neg_m);
-          const float p1 = fmaf(__uint_as_float(raw[2 * w + 1]), p.scale_log2, neg_m);
-#else
-          const float p0 = ex2_approx(fmaf(__uint_as_float(raw[2 * w]), p.scale_log2, neg_m));
-          const float p1 = ex2_approx(fmaf(__uint_as_float(raw[2 * w + 1]), p.scale_log2, neg_m));
-#endif
-          sum8[(2 * w) & 7] += p0;
-          sum8[(2 * w + 1) & 7] += p1;
-          h162 hh = f2h2(p0, p1);
-          pw[w] = *reinterpret_cast<uint32_t*>(&hh);
-        }
-        if (pcount >= 2) mbar_wait(p_empty(pb), ((pcount >> 1) & 1) ^ 1u);
-        if (!FA_ABL(4)) tmem_st32(tP + lane_addr + pb * 32, pw);
-        tmem_st_wait();
-        const float lsum = ((sum8[0] + sum8[1]) + (sum8[2] + sum8[3])) + ((sum8[4] + sum8[5]) + (sum8[6] + sum8[7]));
-        l_run += lsum;
-        fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive_cluster(l_p_full0 + 8u * pb);
-        if constexpr (REPLAY) {   // the slab copy of the same probabilities (pass 2) goes out AFTER the hand-off
-          h16* dst = slab_row + (long long)j * (kBM * kBKV);
-#pragma unroll
-          for (int g = 0; g < 4; ++g) { if (!FA_ABL(3) && !FA_ABL(4)) stg256(dst + g * 16, pw + g * 8); }
-        }
-      }
-      bool gated = false;
-      if constexpr (REPLAY) {
-      // publish this warp's "logged a rescale" flag to both CTAs, make the slab visible to the TMA reads of pass 2,
-      // then arrive on both CTAs' p1_done
-      __threadfence();
-      asm volatile("fence.proxy.async.global;" ::: "memory");
-      __syncwarp();
-      if (lane == 0) {
-        st_cluster_u32(flag_a[0], n_ev > 0 ? 1u : 0u);
-        st_cluster_u32(flag_a[1], n_ev > 0 ? 1u : 0u);
-        mbar_arrive_cluster_release(p1_done_a[0]);
-        mbar_arrive_cluster_release(p1_done_a[1]);
-      }
-      mbar_wait_cluster(p1_done, icount & 1);
-#pragma unroll
-      for (int e = 0; e < 8; ++e) gated |= ev_flags[e] != 0;
-      }
-      const float inv = 1.0f / l_run;
-      const int t = qt * kBM + row;
-      const bool ok = t < p.T;
-#pragma unroll 1
-      for (int pass = 0; pass < (REPLAY ? 2 : 1); ++pass) {
-        if (pass == 1 && gated) {
-          int e_next = 0;
-          int next_blk = (n_ev > 0) ? ev_blk[0] : 0x7fffffff;
-          for (int j = 0; j < n_kv; ++j, ++pcount) {
-            const int pb = pcount & 1;
-            if (pcount >= 2) mbar_wait(p_empty(pb), ((pcount >> 1) & 1) ^ 1u);
-            if (j == next_blk) {
-              const uint32_t prev = pcount - 1;
-              mbar_wait(p_empty(prev & 1), (prev >> 1) & 1);
-              fence_after();
-              const float factor = ev_fac[(long long)e_next * 32 + lane];
-              for (int c0 = 0; c0 < 256; c0 += 32) {
-                uint32_t o[32];
-                tmem_ld32(tO + lane_addr + c0, o);
-                tmem_ld_wait();
-#pragma unroll
-                for (int c = 0; c < 32; ++c) o[c] = __float_as_uint(__uint_as_float(o[c]) * factor);
-                tmem_st32(tO + lane_addr + c0, o);
-              }
-              tmem_st_wait();
-              fence_before();
-              ++e_next;
-              next_blk = (e_next < n_ev) ? ev_blk[e_next] : 0x7fffffff;
-            }
-            __syncwarp();
-            if (lane == 0) mbar_arrive_cluster(l_p_full0 + 8u * pb);
-          }
-        }
-        // ---- epilogue: O / l (+ residual) -> h16 ----
-        mbar_wait(o_full, ocount & 1);
-        ++ocount;
-        fence_after();
-        const long long col0 = (long long)h * p.dh + (long long)pass * 256;
-        h16* orow = p.out + b * p.out_bstride + (long long)t * p.out_pitch + col0;
-        const h16* rrow = p.res ? p.res + b * p.res_bstride + (long long)t * p.res_pitch + col0 : nullptr;
-        for (int c0 = 0; c0 < 256; c0 += 32) {
-          uint32_t o[32];
-          tmem_ld32(tO + lane_addr + c0, o);
-          tmem_ld_wait();
-          if (ok) {
-#pragma unroll
-            for (int g = 0; g < 4; ++g) {
-              float f[8];
-#pragma unroll
-              for (int e = 0; e < 8; ++e) f[e] = __uint_as_float(o[g * 8 + e]) * inv;
-              if (rrow) {
-                float rf[8];
-                unpack8(__ldg(reinterpret_cast<const uint4*>(rrow + c0 + g * 8)), rf);
-#pragma unroll
-                for (int e = 0; e < 8; ++e) f[e] += rf[e];
-              }
-              *reinterpret_cast<uint4*>(orow + c0 + g * 8) = pack8(f);
-            }
-          }
-        }
-        fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive_cluster(l_o_empty);
-      }
+      *reinterpret_cast<h162*>(orow + col) = f2h2(v0, v1);
     }
   }
-  fence_before();
-  __syncthreads();
-  cluster_sync_all();            // neither CTA may leave (or free tensor memory) while the other still uses the pair
-  if (warp == 1) {
-    fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(512u) : "memory");
-  }
 }
+
+template <int DCH, int DV>
+constexpr int smem_bytes() { return 1024 + 2 * DCH * kChunkBytes + DV * kBKV * 2 + 64; }
 
 static PFN_cuTensorMapEncodeTiled g_encode = nullptr;
 static std::once_flag g_once;
@@ -1299,45 +262,19 @@ static int encode3(CUtensorMap* tm, const void* ptr, cuuint64_t d0, cuuint64_t d
   return B200_OK;
 }
 
-// Few query tiles (latent UNets: T = 256 .. 1024 tokens): the call is a latency chain on a handful of SMs, not a
-// throughput problem.  Such calls skip the two-pass replay and cut the output dimension into 64-wide slices instead —
-// every slice is its own work item that recomputes the (tiny) score tiles — so 8x more SMs share the chain's PV half
-// and nothing round-trips through global memory.
-static bool small_problem(const b200_flash_params* a) {
-  const long long q_tiles = (a->T + kBM - 1) / kBM;
-  return (long long)a->B * a->heads * q_tiles * 4 <= sm_count();
-}
-
-// which head_dim-512 replay kernel runs: the CTA-pair kernel (1) or the single-CTA one (0).  B200_FLASH_PAIR overrides.
-static bool pair_mode() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("B200_FLASH_PAIR");
-    v = e ? (e[0] != '0') : B200_FLASH_PAIR_DEFAULT;
-  }
-  return v != 0;
-}
-
-struct ReplayPlan { int grid, n_kv; long long slab_bytes, fac_bytes, blk_bytes, total; };
-static ReplayPlan replay_plan(const b200_flash_params* a) {
-  ReplayPlan r;
-  memset(&r, 0, sizeof(r));
-  if (a->dh != 512 || small_problem(a)) return r;
-  const long long q_tiles = (a->T + kBM - 1) / kBM;
-  if (pair_mode()) {   // CTA pairs: one work item = 256 queries (two 128-row tiles), one CTA per tile
-    const long long items = (long long)a->B * a->heads * ((q_tiles + 1) / 2);
-    const long long pairs = sm_count() / 2;
-    r.grid = 2 * (int)(items < pairs ? items : pairs);
-  } else {
-    const long long items = (long long)a->B * a->heads * q_tiles;
-    r.grid = (int)(items < sm_count() ? items : sm_count());
-  }
-  r.n_kv = (a->S + kBKV - 1) / kBKV;
-  r.slab_bytes = (long long)r.grid * kBM * r.n_kv * kBKV * 2;
-  r.fac_bytes = (long long)r.grid * 4 * r.n_kv * 32 * 4;
-  r.blk_bytes = (((long long)r.grid * 4 * r.n_kv * 4) + 255) / 256 * 256;
-  r.total = r.slab_bytes + r.fac_bytes + r.blk_bytes;
-  return r;
+template <int DCH, int DV>
+static int launch(const FlashDev& d, cudaStream_t stream) {
+  constexpr int smem = smem_bytes<DCH, DV>();
+  static_assert(smem <= 227 * 1024, "attention_flash: shared memory over the 227 KB a block may use");
+  static std::once_flag attr_once;
+  static cudaError_t attr_rc = cudaSuccess;
+  std::call_once(attr_once, [] {
+    attr_rc = cudaFuncSetAttribute(flash_attn_kernel<DCH, DV>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+  });
+  B200_CUDA(attr_rc);
+  B200_CUDA(b200::launch_pdl(flash_attn_kernel<DCH, DV>, d.n_items, kThreads, smem, stream, d));
+  B200_LAUNCH_CHECK("flash_attn_kernel");
+  return B200_OK;
 }
 
 }  // namespace fa
@@ -1345,9 +282,10 @@ static ReplayPlan replay_plan(const b200_flash_params* a) {
 
 using namespace b200;
 
+// No workspace: the kernel keeps every probability tile on chip.
 extern "C" int64_t b200_attention_flash_workspace_bytes(const b200_flash_params* a) {
-  if (!a || a->B < 1 || a->T < 1 || a->S < 1 || a->heads < 1) return 0;
-  return fa::replay_plan(a).total;
+  (void)a;
+  return 0;
 }
 
 extern "C" int b200_attention_flash(const b200_flash_params* a, void* stream_v) {
@@ -1370,35 +308,13 @@ extern "C" int b200_attention_flash(const b200_flash_params* a, void* stream_v) 
   d.B = a->B; d.T = a->T; d.S = a->S; d.heads = a->heads; d.dh = a->dh;
   d.d_chunks = a->dh / 64;
   d.dv = a->dh < 256 ? a->dh : 256;
-  if (fa::small_problem(a) && a->dh >= 128) d.dv = 64;
   d.n_dv = a->dh / d.dv;
   d.q_tiles = (a->T + fa::kBM - 1) / fa::kBM;
   d.n_kv = (a->S + fa::kBKV - 1) / fa::kBKV;
-  const fa::ReplayPlan rp = fa::replay_plan(a);
-  const bool replay = a->dh == 512 && a->workspace != nullptr && !fa::small_problem(a);
-  if (replay) {
-    B200_CHECK_ARG(a->workspace_bytes >= rp.total, "attention_flash: workspace of %lld bytes, need %lld",
-                   (long long)a->workspace_bytes, rp.total);
-    B200_CHECK_ARG(((uintptr_t)a->workspace & 255) == 0, "attention_flash: workspace must be 256-byte aligned");
-  }
-  // CTA pairs: head_dim 512 with the replay workspace, and head_dim 256 (one pass, no workspace), unless the call is a
-  // small problem
-  const bool pair256 = a->dh == 256 && fa::pair_mode() && !fa::small_problem(a);
-  const bool pair = (replay && fa::pair_mode()) || pair256;
-  const long long items = pair ? (long long)a->B * a->heads * ((d.q_tiles + 1) / 2)
-                               : (long long)a->B * a->heads * d.q_tiles * (replay ? 1 : d.n_dv);
+  const long long items = (long long)a->B * a->heads * d.q_tiles * d.n_dv;
   B200_CHECK_ARG(items < (1ll << 31), "attention_flash: too many work items");
   d.n_items = (int)items;
   d.scale_log2 = a->scale * 1.4426950408889634f;
-  {
-    static float thr = -1.f;
-    if (thr < 0.f) {
-      const char* e = getenv("B200_FLASH_RESCALE");
-      thr = e ? (float)atof(e) : fa::kRescaleThreshold;
-      if (!(thr >= 1.f && thr <= 14.f)) thr = fa::kRescaleThreshold;
-    }
-    d.rescale_thr = thr;
-  }
   d.out = reinterpret_cast<h16*>(a->out);
   d.out_pitch = a->out_pitch; d.out_bstride = (long long)a->T * a->out_pitch;
   d.res = reinterpret_cast<const h16*>(a->res);
@@ -1406,74 +322,14 @@ extern "C" int b200_attention_flash(const b200_flash_params* a, void* stream_v) 
   int rc;
   if ((rc = fa::encode3(&d.tmQ, a->q, C, a->T, a->B, (cuuint64_t)a->q_pitch * 2, (cuuint64_t)a->T * a->q_pitch * 2, 64,
                         fa::kBM, "Q"))) return rc;
-  // pair kernel: each CTA stages half of every B operand (32 of a block's 64 keys; 128 of the 256 V^T rows)
   if ((rc = fa::encode3(&d.tmK, a->k, C, a->S, a->B, (cuuint64_t)a->k_pitch * 2, (cuuint64_t)a->S * a->k_pitch * 2, 64,
-                        pair ? fa::kPKeysCta : fa::kBKV, "K"))) return rc;
+                        fa::kBKV, "K"))) return rc;
   if ((rc = fa::encode3(&d.tmVt, a->vt, a->S, C, a->B, (cuuint64_t)a->vt_pitch * 2, (cuuint64_t)C * a->vt_pitch * 2,
-                        fa::kBKV, pair ? fa::kPVRows : d.dv, "V^T"))) return rc;
-
-  const int smem = d.d_chunks * fa::kQChunkBytes + fa::kKRingBytes + d.dv * fa::kBKV * 2 + 1024 + 512;
-  const int smem_max = d.d_chunks * fa::kQChunkBytes + fa::kKRingBytes + 256 * fa::kBKV * 2 + 1024 + 512;
-  const int grid = replay ? rp.grid
-                   : pair ? 2 * (d.n_items < sm_count() / 2 ? d.n_items : sm_count() / 2)
-                          : (d.n_items < sm_count() ? d.n_items : sm_count());
-  if (replay) {
-    B200_CHECK_ARG(grid == rp.grid && d.n_kv == rp.n_kv, "attention_flash: internal replay plan mismatch");
-    uint8_t* ws = static_cast<uint8_t*>(a->workspace);
-    d.pslab = reinterpret_cast<h16*>(ws);
-    d.p_pitch = (long long)d.n_kv * fa::kBM * fa::kBKV;
-    d.ev_fac = reinterpret_cast<float*>(ws + rp.slab_bytes);
-    d.ev_blk = reinterpret_cast<int*>(ws + rp.slab_bytes + rp.fac_bytes);
-    if ((rc = fa::encode3(&d.tmP, d.pslab, fa::kBKV, (cuuint64_t)d.n_kv * fa::kBM, grid, (cuuint64_t)fa::kBKV * 2,
-                          (cuuint64_t)d.p_pitch * 2, fa::kBKV, fa::kBM, "P slab"))) return rc;
-  }
-#define B200_FLASH_LAUNCH(DCH, RP)                                                                                    \
-  do {                                                                                                                \
-    static std::once_flag attr_once;                                                                                  \
-    static cudaError_t attr_rc = cudaSuccess;                                                                         \
-    const int smem_attr = smem_max;   /* the widest output slice: later calls may need it */                          \
-    std::call_once(attr_once, [smem_attr] {                                                                           \
-      attr_rc = cudaFuncSetAttribute(fa::flash_attn_kernel<DCH, RP>, cudaFuncAttributeMaxDynamicSharedMemorySize,     \
-                                     smem_attr);                                                                      \
-    });                                                                                                               \
-    B200_CUDA(attr_rc);                                                                                               \
-    B200_CUDA(b200::launch_pdl(fa::flash_attn_kernel<DCH, RP>, grid, fa::kThreads, smem, stream, d));                                          \
-  } while (0)
+                        fa::kBKV, d.dv, "V^T"))) return rc;
   switch (d.d_chunks) {
-    case 1: B200_FLASH_LAUNCH(1, false); break;
-    case 2: B200_FLASH_LAUNCH(2, false); break;
-    case 4:
-      if (pair) {
-        static std::once_flag pair4_once;
-        static cudaError_t pair4_rc = cudaSuccess;
-        std::call_once(pair4_once, [] {
-          pair4_rc = cudaFuncSetAttribute(fa::flash_pair_kernel<4, false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                          fa::pair_smem<4>());
-        });
-        B200_CUDA(pair4_rc);
-        B200_CUDA(b200::launch_pdl(fa::flash_pair_kernel<4, false>, grid, fa::kThreads, fa::pair_smem<4>(), stream, d));
-      } else {
-        B200_FLASH_LAUNCH(4, false);
-      }
-      break;
-    default:
-      if (pair) {
-        static std::once_flag pair_once;
-        static cudaError_t pair_rc = cudaSuccess;
-        std::call_once(pair_once, [] {
-          pair_rc = cudaFuncSetAttribute(fa::flash_pair_kernel<8, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         fa::pair_smem<8>());
-        });
-        B200_CUDA(pair_rc);
-        B200_CUDA(b200::launch_pdl(fa::flash_pair_kernel<8, true>, grid, fa::kThreads, fa::pair_smem<8>(), stream, d));   // clusters of 2 (__cluster_dims__)
-      } else if (replay) {
-        B200_FLASH_LAUNCH(8, true);
-      } else {
-        B200_FLASH_LAUNCH(8, false);
-      }
-      break;
+    case 1: return fa::launch<1, 64>(d, stream);
+    case 2: return fa::launch<2, 128>(d, stream);
+    case 4: return fa::launch<4, 256>(d, stream);
+    default: return fa::launch<8, 256>(d, stream);
   }
-#undef B200_FLASH_LAUNCH
-  B200_LAUNCH_CHECK("flash_attn_kernel");
-  return B200_OK;
 }

@@ -1,25 +1,25 @@
-// Implicit-GEMM convolution / GEMM on Blackwell tcgen05 tensor cores.
+// Implicit-GEMM convolution / GEMM on Hopper wgmma tensor cores.
 //
 // Replaces every dense contraction of the reference sampling path (the cuDNN / cuBLAS calls behind
 // monai Convolution, nn.Linear, torch.baddbmm/bmm — see include/b200gen.h for the call sites).
 //
-// Design (B200-first, not a translation of any library kernel):
-//   * activations live in HBM as channels-last bf16; a CTA tile is a BW x BH x BD box of 128 output
+// Design:
+//   * activations live in HBM as channels-last 16-bit rows; a CTA tile is a BW x BH x BD box of 128 output
 //     voxels x BN output channels.  For every filter tap and every 64-channel chunk the producer
 //     thread issues ONE tiled-TMA box load of the shifted input box: out-of-range coordinates
 //     (the zero padding, ragged edges, channel tails) are zero-filled by the TMA unit, stride-2
 //     convolutions use the tensor map's traversal stride.  No im2col buffer ever exists.
-//   * the box lands in shared memory as a 128-row x 128-byte SWIZZLE_128B K-major tile — exactly the
-//     canonical UMMA operand layout — and one elected thread issues tcgen05.mma (M=128, N=BN, K=16)
-//     accumulating in TMEM.  Weights are a K-major [Cout][taps*Cin] bf16 matrix, also TMA-staged.
-//   * warp-specialised persistent kernel: warp 0 = TMA producer, warp 1 = MMA issuer (+TMEM alloc),
-//     warps 2..5 = epilogue.  smem ring of STAGES {A,B} tiles (full/empty mbarriers), TMEM
-//     accumulator double-buffered (2 x BN columns) so the epilogue of tile i overlaps the main loop
-//     of tile i+1.
-//   * fused epilogue straight out of TMEM: +bias, +per-sample row vector (time embedding),
-//     activation, scale, +residual, activation, bf16/fp32 store with arbitrary voxel strides
-//     (so transposed-conv phases and channel-slice outputs need no extra pass).
+//   * the box lands in shared memory as a 128-row x 128-byte SWIZZLE_128B K-major tile — the canonical
+//     wgmma operand layout — and two warpgroups issue wgmma (M=64 each, N=BN, K=16) accumulating in
+//     registers.  Weights are a K-major [Cout][taps*Cin] 16-bit matrix, also TMA-staged.
+//   * warp-specialised persistent kernel: 4 epilogue warps, 2 MMA warpgroups, 1 TMA producer warp; smem ring of
+//     STAGES {A,B} tiles (full/empty mbarriers); the finished accumulator goes through one fp32 shared-memory tile so
+//     the epilogue of tile i overlaps the main loop of tile i+1.
+//   * fused epilogue: +bias, +per-sample row vector (time embedding), activation, scale, +residual, activation,
+//     16-bit/fp32 store with arbitrary voxel strides (so transposed-conv phases and channel-slice outputs need no
+//     extra pass).
 #include "common.cuh"
+#include "wgmma.cuh"
 #include <cuda.h>
 #include <cudaTypedefs.h>
 #include <mutex>
@@ -28,10 +28,12 @@
 
 namespace b200 {
 
-static constexpr int kBM = 128;           // rows (output voxels) per tile == UMMA_M
-static constexpr int kBK = 64;            // channels per K chunk == 128 bytes of bf16 == swizzle span
+static constexpr int kBM = 128;           // rows (output voxels) per tile: two wgmma M=64 warpgroups
+static constexpr int kBK = 64;            // channels per K chunk == 128 bytes of 16-bit data == swizzle span
 static constexpr int kABytes = kBM * kBK * 2;
-static constexpr int kThreads = 192;      // 6 warps: TMA, MMA, 4 x epilogue
+static constexpr int kMmaWarp0 = 4;       // warps 0..3 epilogue, 4..11 two MMA warpgroups, 12 TMA producer
+static constexpr int kTmaWarp = 12;
+static constexpr int kThreads = 13 * 32;
 
 struct SegDev {
   int8_t src, dw, dh, dd;
@@ -135,125 +137,16 @@ __device__ __forceinline__ void tma_load_3d(const CUtensorMap* tm, uint32_t bar,
       "l"(reinterpret_cast<uint64_t>(tm)), "r"(bar), "r"(c0), "r"(c1), "r"(c2)
       : "memory");
 }
-// One lane of a fully converged warp (elect.sync): the whole warp runs the role loop and only the asynchronous
-// issue instructions are guarded, so their operands stay in uniform registers without per-instruction elect loops.
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred;
-  asm volatile(
-      "{\n\t.reg .pred P1;\n\t"
-      "elect.sync _|P1, 0xFFFFFFFF;\n\t"
-      "selp.u32 %0, 1, 0, P1;\n\t}"
-      : "=r"(pred));
-  return pred != 0;
+// CH consecutive fp32 accumulator values of one tile row from the shared-memory hand-off tile
+template <int CH>
+__device__ __forceinline__ void acc_ld(const float* src, uint32_t* r) {
+#pragma unroll
+  for (int j = 0; j < CH; j += 4) {
+    const float4 t = *reinterpret_cast<const float4*>(src + j);
+    r[j] = __float_as_uint(t.x); r[j + 1] = __float_as_uint(t.y);
+    r[j + 2] = __float_as_uint(t.z); r[j + 3] = __float_as_uint(t.w);
+  }
 }
-__device__ __forceinline__ void tcgen05_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tcgen05_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tcgen05_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar)
-               : "memory");
-}
-// D[tmem] (+)= A[smem] * B[smem]^T, bf16 x bf16 -> fp32
-__device__ __forceinline__ void umma_h16(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                          uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// K-major, SWIZZLE_128B shared-memory matrix descriptor (cute::UMMA::SmemDescriptor bit layout):
-//   [0,14) start address >> 4, [16,30) leading byte offset >> 4 (unused for swizzled K-major: 1),
-//   [32,46) stride byte offset >> 4 (8 rows x 128 B = 1024), [46,48) version = 1, [61,64) layout = 2.
-__device__ __forceinline__ uint64_t make_smem_desc(uint32_t smem_addr) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4);
-  d |= static_cast<uint64_t>(1) << 16;
-  d |= static_cast<uint64_t>(1024 >> 4) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
-  return d;
-}
-// kind::f16 instruction descriptor: c=f32 (bit4), a=bf16 (bit7), b=bf16 (bit10), K-major both,
-// N>>3 at [17,23), M>>4 at [24,29).
-__host__ __device__ constexpr uint32_t make_idesc(int M, int N) {
-  return (1u << 4) | (B200_H16_FMT << 7) | (B200_H16_FMT << 10) | (static_cast<uint32_t>(N >> 3) << 17) |
-         (static_cast<uint32_t>(M >> 4) << 24);
-}
-
-// ---- CTA-pair (cta_group::2) variants: see igemm_tc_kernel<BN, STAGES, true> ----
-static constexpr uint32_t kPeerMask = 0xFEFFFFFFu;      // clears the CTA-rank bit of a shared::cluster address -> leader
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// default semantics (release at CTA scope): the hand-off publishes nothing through memory (the accumulator lives in
-// tensor memory, ordered by tcgen05.wait + fence) — a cluster-scope release would wait for the epilogue's global stores
-__device__ __forceinline__ void mbar_arrive_leader(uint32_t bar) {
-  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(bar & kPeerMask) : "memory");
-}
-__device__ __forceinline__ void tma_load_5d_pair(const CUtensorMap* tm, uint32_t bar, uint32_t dst, int c0, int c1,
-                                                 int c2, int c3, int c4) {
-  asm volatile(
-      "cp.async.bulk.tensor.5d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4, %5, %6, %7}], [%2];" ::"r"(dst),
-      "l"(reinterpret_cast<uint64_t>(tm)), "r"(bar & kPeerMask), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_3d_pair(const CUtensorMap* tm, uint32_t bar, uint32_t dst, int c0, int c1,
-                                                 int c2) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4, %5}], [%2];" ::"r"(dst),
-      "l"(reinterpret_cast<uint64_t>(tm)), "r"(bar & kPeerMask), "r"(c0), "r"(c1), "r"(c2)
-      : "memory");
-}
-__device__ __forceinline__ void tcgen05_commit2(uint32_t bar) {      // same barrier offset in both CTAs
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(bar),
-               "h"((uint16_t)3)
-               : "memory");
-}
-__device__ __forceinline__ void umma2_h16(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                          uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]),
-        "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]),
-        "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]),
-        "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]),
-        "=r"(r[15])
-      : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 
 // first reduction chunk of range `ks` when `num_k` chunks are cut into `splits` near-equal ranges
 __host__ __device__ __forceinline__ int split_begin(int num_k, int splits, int ks) {
@@ -364,15 +257,14 @@ __device__ __forceinline__ void store_direct(const IgemmDev& p, const float* v, 
 // the additive vector comes from shared memory (filled once per (sample, column tile)), the activation switches are
 // hoisted out of the element loops and the residual / output move as 256-bit (or 128-bit) vectors.
 // ------------------------------------------------------------------------------------------------
+// 32 bytes as two 16-byte accesses (sm_90 has no 256-bit global load / store)
 __device__ __forceinline__ void ldg256(const void* ptr, uint4& a, uint4& b) {
-  asm volatile("ld.global.nc.v8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-               : "=r"(a.x), "=r"(a.y), "=r"(a.z), "=r"(a.w), "=r"(b.x), "=r"(b.y), "=r"(b.z), "=r"(b.w)
-               : "l"(ptr));
+  a = __ldg(reinterpret_cast<const uint4*>(ptr));
+  b = __ldg(reinterpret_cast<const uint4*>(ptr) + 1);
 }
 __device__ __forceinline__ void stg256(void* ptr, const uint4& a, const uint4& b) {
-  asm volatile("st.global.v8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(ptr), "r"(a.x), "r"(a.y), "r"(a.z),
-               "r"(a.w), "r"(b.x), "r"(b.y), "r"(b.z), "r"(b.w)
-               : "memory");
+  reinterpret_cast<uint4*>(ptr)[0] = a;
+  reinterpret_cast<uint4*>(ptr)[1] = b;
 }
 template <int CH>
 __device__ __forceinline__ void act_inplace(float* v, int act) {
@@ -488,8 +380,7 @@ __device__ __forceinline__ void epilogue_row(const IgemmDev& p, float* v, int nb
 // output — every nn.Linear of the transformer blocks, 1x1 projections.  Same arithmetic and order as epilogue_fast
 // with act1 = act2 = none and scale = 1 (bit-identical), but none of its run-time switches: with one epilogue warp per
 // scheduler the ~20 uniform branches per chunk of the general body (activation chains, scale, output type, statistics)
-// and its instruction footprint were what a K = 256 GEMM spent its time on (ncu source view: branch_resolving /
-// no_inst stalls spread over the whole body; 12.7k cycles per 128 x 256 tile against ~1k of issue work).
+// and its instruction footprint, not the tensor cores, bound a GEMM with a short (K = 256) reduction.
 template <int CH, bool HAS_RES>
 __device__ __forceinline__ void epilogue_lean(const IgemmDev& p, const uint32_t* raw, const float* addv,
                                               const uint4* rv, long long out_off, int col0) {
@@ -554,91 +445,58 @@ __device__ __forceinline__ void store_staged(const IgemmDev& p, const float* v, 
 }
 
 // ------------------------------------------------------------------------------------------------
-// The tcgen05 kernel
+// The wgmma kernel
 // ------------------------------------------------------------------------------------------------
-// PAIR = true: the CTA-pair (tcgen05.mma.cta_group::2) variant for the big 256-column convolutions.  Two CTAs form one
-// 256-row x BN tile: each owns 128 output voxels (its A box, its accumulator in its own tensor memory, its epilogue) but
-// stages only HALF of the weight tile — the B operand of an M = 256 MMA is split across the pair — so the per-SM operand
-// bytes per tensor cycle drop from 48 KB to 32 KB per 64-channel chunk (less shared-memory and L2 -> SM traffic under
-// the power cap, six stages instead of four in the same 192 KB).  The leader CTA's issuing thread drives both tensor
-// pipes; TMA of both CTAs completes on the leader's barriers; commits are multicast to both CTAs.
-template <int BN, int STAGES, bool PAIR = false>
+// Warp roles (416 threads): warps 0..3 = epilogue (thread <-> tile row), warps 4..11 = two MMA warpgroups (rows 0..63
+// and 64..127 of the tile), warp 12 = TMA producer.  The MMA warpgroups hold the accumulator of the tile in flight in
+// registers and hand the finished tile to the epilogue through one fp32 shared-memory buffer, so the epilogue of tile i
+// overlaps the main loop of tile i + 1.
+template <int BN, int STAGES>
 __global__ void __launch_bounds__(kThreads, 1) igemm_tc_kernel(const __grid_constant__ IgemmDev p) {
-  constexpr int kBBytes = (PAIR ? BN / 2 : BN) * kBK * 2;
+  constexpr int kBBytes = BN * kBK * 2;
   constexpr int kStageBytes = kABytes + kBBytes;
-  constexpr int kTmemCols = (2 * BN < 32) ? 32 : 2 * BN;   // power of two for BN in {16..256}
+  constexpr int kAccLd = BN + 4;          // padded fp32 row: row-per-thread 16-byte reads are conflict-free
   constexpr int CH = (BN >= 32) ? 32 : 16;
 
   if (!p.pdl_late) pdl_launch_dependents();   // the next kernel's prologue may overlap this kernel (it blocks in its own pdl_wait)
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t bar_base = smem_base + STAGES * kStageBytes;
+  const uint32_t acc_base = smem_base + STAGES * kStageBytes;
+  float* acc_smem = reinterpret_cast<float*>(smem_raw + (acc_base - smem_u32(smem_raw)));      // [kBM][kAccLd]
+  const uint32_t bar_base = acc_base + kBM * kAccLd * 4;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };
-  auto tfull_bar = [&](int b) { return bar_base + 8u * (2 * STAGES + b); };
-  auto tempty_bar = [&](int b) { return bar_base + 8u * (2 * STAGES + 2 + b); };
-  const uint32_t tmem_slot = bar_base + 8u * (2 * STAGES + 4);
+  const uint32_t tfull_bar = bar_base + 8u * (2 * STAGES);
+  const uint32_t tempty_bar = bar_base + 8u * (2 * STAGES + 1);
   float* stage_tiles = reinterpret_cast<float*>(smem_raw + (bar_base + 256u - smem_u32(smem_raw)));   // 4 x [32][CH+1]
   float* add_tiles = stage_tiles + 4 * 32 * 33;                                                      // 4 x 2 x [BN]
-  volatile uint32_t* tmem_slot_ptr =
-      reinterpret_cast<volatile uint32_t*>(smem_raw + (tmem_slot - smem_u32(smem_raw)));
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const uint32_t rank = PAIR ? cluster_ctarank() : 0u;
-  const bool leader = rank == 0;
-  // PAIR: one work unit per CTA pair; `tile` below is the pair-level tile index
-  const int worker = PAIR ? (int)(blockIdx.x >> 1) : (int)blockIdx.x;
-  const int n_workers = PAIR ? (int)(gridDim.x >> 1) : (int)gridDim.x;
+  const int worker = (int)blockIdx.x;
+  const int n_workers = (int)gridDim.x;
 
-  if (warp == 0 && lane == 0) {
+  if (warp == kTmaWarp && lane == 0) {
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(full_bar(s), 1);
-      mbar_init(empty_bar(s), 1);
+      mbar_init(empty_bar(s), 8);          // one arrival per MMA warp
     }
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(tfull_bar(b), 1);
-      mbar_init(tempty_bar(b), PAIR ? 8 : 4);       // PAIR: the four epilogue warps of both CTAs, on the leader's copy
-    }
+    mbar_init(tfull_bar, 8);
+    mbar_init(tempty_bar, 4);              // one arrival per epilogue warp
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
   }
-  if (warp == 1) {
-    if constexpr (PAIR) {      // the same warp of both CTAs: one pair-wide allocation
-      asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot),
-                   "r"((uint32_t)kTmemCols)
-                   : "memory");
-      asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-    } else {
-      asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot),
-                   "r"((uint32_t)kTmemCols)
-                   : "memory");
-      asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-  }
-  tcgen05_fence_before();
   __syncthreads();
-  if constexpr (PAIR) cluster_sync_all();       // the peer's barriers exist before anything signals them remotely
-  tcgen05_fence_after();
-  const uint32_t tmem_base = *tmem_slot_ptr;
-  pdl_wait();                       // barriers and tensor memory are set up: now wait for the producer of our inputs
+  pdl_wait();                       // barriers are set up: now wait for the producer of our inputs
 
   const int num_k = p.num_k_chunks;
-  // work-unit index -> (k-split, column tile, spatial tile, sample).  PAIR: the unit is a pair of M tiles (2 * mp + rank)
-  // sharing one column tile; an odd tile count leaves the last pair's second CTA a dead tile (nb == N: its TMA boxes
-  // are zero-filled, its rows are never stored).
+  // work-unit index -> (k-split, column tile, spatial tile, sample)
   struct TileIdx { int ks, nt, wt, ht, dt, nb; };
   auto decode_tile = [&](int tile) {
     TileIdx t;
     int x = tile;
-    if constexpr (PAIR) {
-      t.ks = 0;
-      t.nt = x % p.tiles_n; x /= p.tiles_n;
-      x = 2 * x + (int)rank;
-    } else {
-      t.ks = x % p.k_splits; x /= p.k_splits;
-      t.nt = x % p.tiles_n; x /= p.tiles_n;
-    }
+    t.ks = x % p.k_splits; x /= p.k_splits;
+    t.nt = x % p.tiles_n; x /= p.tiles_n;
     t.wt = x % p.tiles_w; x /= p.tiles_w;
     t.ht = x % p.tiles_h; x /= p.tiles_h;
     t.dt = x % p.tiles_d; x /= p.tiles_d;
@@ -646,10 +504,8 @@ __global__ void __launch_bounds__(kThreads, 1) igemm_tc_kernel(const __grid_cons
     return t;
   };
 
-  if (warp == 0) {
+  if (warp == kTmaWarp) {
     // ============================== TMA producer ==============================
-    // (single-lane role: measured ~5 % faster for this kernel than the warp-converged elect.sync form used in
-    //  flash_attn.cu — its MMAs are 128 cycles each, so the issue thread is never the bottleneck here)
     if (lane == 0) {
       int stage = 0;
       uint32_t phase = 0;
@@ -671,63 +527,71 @@ __global__ void __launch_bounds__(kThreads, 1) igemm_tc_kernel(const __grid_cons
             if (kglob < k_begin || kglob >= k_end) continue;
             mbar_wait(empty_bar(stage), phase ^ 1u);
             const uint32_t a_dst = smem_base + stage * kStageBytes;
-            if constexpr (PAIR) {
-              // both CTAs load their own A box and their half of the weight tile; all bytes land on the LEADER's barrier
-              if (leader) mbar_arrive_expect_tx(full_bar(stage), 2 * kStageBytes);
-              tma_load_5d_pair(tm, full_bar(stage), a_dst, (sg.c0 + c) * kBK, cw, ch, cd, a_nb);
-              tma_load_3d_pair(&p.tmB, full_bar(stage), a_dst + kABytes, kglob * kBK, n0 + (int)rank * (BN / 2), wb);
-            } else {
-              mbar_arrive_expect_tx(full_bar(stage), kStageBytes);
-              tma_load_5d(tm, full_bar(stage), a_dst, (sg.c0 + c) * kBK, cw, ch, cd, a_nb);
-              tma_load_3d(&p.tmB, full_bar(stage), a_dst + kABytes, kglob * kBK, n0, wb);
-            }
+            mbar_arrive_expect_tx(full_bar(stage), kStageBytes);
+            tma_load_5d(tm, full_bar(stage), a_dst, (sg.c0 + c) * kBK, cw, ch, cd, a_nb);
+            tma_load_3d(&p.tmB, full_bar(stage), a_dst + kABytes, kglob * kBK, n0, wb);
             if (++stage == STAGES) { stage = 0; phase ^= 1u; }
           }
         }
       }
       if (p.pdl_late) pdl_launch_dependents();     // every operand load of this CTA is issued
     }
-  } else if (warp == 1) {
-    // ============================== MMA issuer ==============================
-    if (lane == 0 && leader) {
-      constexpr uint32_t idesc = make_idesc(PAIR ? 2 * kBM : kBM, BN);
-      int stage = 0;
-      uint32_t phase = 0;
-      int it = 0;
-      for (int tile = worker; tile < p.num_tiles; tile += n_workers, ++it) {
-        const int buf = it & 1;
-        const uint32_t acc_phase = (it >> 1) & 1;
-        mbar_wait(tempty_bar(buf), acc_phase ^ 1u);
-        tcgen05_fence_after();
-        const uint32_t d_tmem = tmem_base + buf * BN;
-        const int ks = PAIR ? 0 : tile % p.k_splits;
-        const int nk = split_begin(num_k, p.k_splits, ks + 1) - split_begin(num_k, p.k_splits, ks);
-        for (int k = 0; k < nk; ++k) {
-          mbar_wait(full_bar(stage), phase);
-          tcgen05_fence_after();
-          const uint32_t a_addr = smem_base + stage * kStageBytes;
-          const uint64_t adesc = make_smem_desc(a_addr);
-          const uint64_t bdesc = make_smem_desc(a_addr + kABytes);
+  } else if (warp >= kMmaWarp0) {
+    // ============================== MMA warpgroups ==============================
+    const int wg = (warp - kMmaWarp0) >> 2;       // rows 64 * wg .. 64 * wg + 63 of the tile
+    const int wq = (warp - kMmaWarp0) & 3;        // 16-row slice of those inside the warpgroup
+    float acc[BN / 2];
 #pragma unroll
-          for (int kk = 0; kk < kBK / 16; ++kk) {
-            // advance 16 elements (32 bytes) along K inside the 128-byte swizzle row: +2 in >>4 units
-            if constexpr (PAIR) umma2_h16(d_tmem, adesc + 2u * kk, bdesc + 2u * kk, idesc, (k | kk) != 0 ? 1u : 0u);
-            else umma_h16(d_tmem, adesc + 2u * kk, bdesc + 2u * kk, idesc, (k | kk) != 0 ? 1u : 0u);
-          }
-          if constexpr (PAIR) tcgen05_commit2(empty_bar(stage)); else tcgen05_commit(empty_bar(stage));
-          if (++stage == STAGES) { stage = 0; phase ^= 1u; }
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+    int stage = 0;
+    uint32_t phase = 0;
+    int it = 0;
+    for (int tile = worker; tile < p.num_tiles; tile += n_workers, ++it) {
+      const int ks = tile % p.k_splits;
+      const int nk = split_begin(num_k, p.k_splits, ks + 1) - split_begin(num_k, p.k_splits, ks);
+      int prev = -1;
+      for (int k = 0; k < nk; ++k) {
+        mbar_wait(full_bar(stage), phase);
+        const uint32_t a_addr = smem_base + stage * kStageBytes + wg * (64 * kBK * 2);
+        const uint64_t adesc = wgmma_desc(a_addr);
+        const uint64_t bdesc = wgmma_desc(smem_base + stage * kStageBytes + kABytes);
+        wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < kBK / 16; ++kk)
+          wgmma_ss<BN>(acc, adesc + 2u * kk, bdesc + 2u * kk, (k | kk) != 0 ? 1u : 0u);
+        wgmma_commit();
+        wgmma_wait<1>();            // the group of the previous chunk has finished reading its stage
+        if (prev >= 0) {
+          __syncwarp();
+          if (lane == 0) mbar_arrive(empty_bar(prev));
         }
-        if constexpr (PAIR) tcgen05_commit2(tfull_bar(buf)); else tcgen05_commit(tfull_bar(buf));
+        prev = stage;
+        if (++stage == STAGES) { stage = 0; phase ^= 1u; }
       }
+      wgmma_wait<0>();
+      wgmma_touch<BN / 2>(acc);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(empty_bar(prev));
+      // hand the tile to the epilogue once it has finished reading the previous one
+      mbar_wait(tempty_bar, (it & 1) ^ 1u);
+      const int r0 = wg * 64 + wq * 16 + (lane >> 2);
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) {
+        const int col = 8 * j + 2 * (lane & 3);
+        *reinterpret_cast<float2*>(acc_smem + r0 * kAccLd + col) = make_float2(acc[4 * j], acc[4 * j + 1]);
+        *reinterpret_cast<float2*>(acc_smem + (r0 + 8) * kAccLd + col) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+      }
+      __syncwarp();
+      if (lane == 0) mbar_arrive(tfull_bar);
     }
   } else {
     // ============================== epilogue warps ==============================
-    const int q = warp & 3;                 // TMEM lane quadrant this warp may access
-    const int r = q * 32 + lane;            // row of the tile
+    const int r = warp * 32 + lane;         // row of the tile
+    const float* acc_row = acc_smem + r * kAccLd;
     const int rw = r & (p.BW - 1);
     const int rh = (r >> p.bw_log2) & (p.BH - 1);
     const int rd = r >> (p.bw_log2 + p.bh_log2);
-    float* addv = add_tiles + (warp - 2) * 2 * BN;      // two buffers: the current vector and the prefetched next one
+    float* addv = add_tiles + warp * 2 * BN;      // two buffers: the current vector and the prefetched next one
     float* addv_other = addv + BN;
     int next_key = -1;
     int add_key = -1;
@@ -738,14 +602,14 @@ __global__ void __launch_bounds__(kThreads, 1) igemm_tc_kernel(const __grid_cons
     // GroupNorm partial sums for the consumer of this tensor: per warp [BN/8 groups][sum, sumsq] in shared memory
     // (aliases the staged-store tiles, which this mode excludes), flushed to this warp's private global slot
     // whenever the (sample, column tile) changes and at the end — deterministic, no atomics.
-    float* gacc = stage_tiles + (warp - 2) * (32 * 33);
+    float* gacc = stage_tiles + warp * (32 * 33);
     const bool gn_on = (p.gn_partial != nullptr);
     int gn_nb = -1, gn_n0 = 0;
     auto gn_flush = [&]() {
       if (gn_nb >= 0) {
         const int sh = p.gn_sh;
         float* dst = p.gn_partial +
-                     (((long long)gn_nb * p.gn_slots + p.gn_slot0 + blockIdx.x * 4 + (warp - 2)) * (p.cout >> sh)) * 2 +
+                     (((long long)gn_nb * p.gn_slots + p.gn_slot0 + blockIdx.x * 4 + warp) * (p.cout >> sh)) * 2 +
                      (gn_n0 >> sh) * 2;
         for (int e = lane; e < (BN >> sh) * 2; e += 32) {
           if (gn_n0 + ((e >> 1) << sh) < p.cout) dst[e] += gacc[e];
@@ -759,31 +623,25 @@ __global__ void __launch_bounds__(kThreads, 1) igemm_tc_kernel(const __grid_cons
     for (int tile = worker; tile < p.num_tiles; tile += n_workers, ++it) {
       const TileIdx ti = decode_tile(tile);
       const int ks = ti.ks, nt = ti.nt, wt = ti.wt, ht = ti.ht, dt = ti.dt;
-      const bool live = ti.nb < p.N;               // PAIR: the second CTA of the last pair may hold a dead tile
-      const int nb = live ? ti.nb : p.N - 1;
+      const int nb = ti.nb;
       const int ow = wt * p.BW + rw, oh = ht * p.BH + rh, od = dt * p.BD + rd;
-      const bool row_ok = live && (ow < p.OW) && (oh < p.OH) && (od < p.OD);
+      const bool row_ok = (ow < p.OW) && (oh < p.OH) && (od < p.OD);
       const long long out_off = nb * p.out_sN + od * p.out_sD + oh * p.out_sH + ow * p.out_sW + ks * p.split_stride;
       const long long res_off = nb * p.res_sN + od * p.res_sD + oh * p.res_sH + ow * p.res_sW;
       const int n0 = nt * BN;
 
-      if constexpr (!PAIR) {
+      {
         if (p.split_counters) {
           // ---- one-launch split-K: this range's raw accumulators go to the workspace; the CTA that draws the last
           //      ticket of the output tile sums the ranges in order and applies the call's epilogue ----
-          const int buf = it & 1;
-          mbar_wait(tfull_bar(buf), (it >> 1) & 1);
-          tcgen05_fence_after();
-          const uint32_t taddr = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + buf * BN;
+          mbar_wait(tfull_bar, it & 1);
           const long long lin_row = (((long long)nb * p.OD + od) * p.OH + oh) * p.OW + ow;
           float* wrow = p.split_ws + ((long long)ks * p.split_rows + lin_row) * p.ws_cols;
 #pragma unroll 1
           for (int c0 = 0; c0 < BN; c0 += CH) {
             if (n0 + c0 >= p.ws_cols) break;             // warp-uniform
             uint32_t raw[CH];
-            if constexpr (CH == 32) tmem_ld32(taddr + c0, raw);
-            else tmem_ld16(taddr + c0, raw);
-            tmem_ld_wait();
+            acc_ld<CH>(acc_row + c0, raw);
             if (row_ok) {
 #pragma unroll
               for (int g = 0; g < CH / 4; ++g)
@@ -793,9 +651,8 @@ __global__ void __launch_bounds__(kThreads, 1) igemm_tc_kernel(const __grid_cons
                                   __uint_as_float(raw[g * 4 + 2]), __uint_as_float(raw[g * 4 + 3]));
             }
           }
-          tcgen05_fence_before();
           __syncwarp();
-          if (lane == 0) mbar_arrive(tempty_bar(buf));           // the accumulator buffer may be refilled
+          if (lane == 0) mbar_arrive(tempty_bar);                // the accumulator buffer may be refilled
           // ---- cooperative reduction: every CTA of the output tile draws a ticket once its partial rows are visible,
           //      waits until all k_splits tickets are drawn (the k_splits CTAs of a tile are distinct CTAs of one wave:
           //      the grid never exceeds one CTA per SM, and a CTA only ever waits for CTAs working on lower or equal
@@ -806,7 +663,7 @@ __global__ void __launch_bounds__(kThreads, 1) igemm_tc_kernel(const __grid_cons
           int* counter = p.split_counters + out_tile;
           __threadfence();                                        // this thread's partial rows are visible device-wide
           asm volatile("bar.sync 1, 128;" ::: "memory");          // ... and so are the other 127 epilogue threads'
-          if (warp == 2 && lane == 0) {
+          if (warp == 0 && lane == 0) {
             atomicAdd(counter, 1);
             int seen;
             do {
@@ -816,7 +673,7 @@ __global__ void __launch_bounds__(kThreads, 1) igemm_tc_kernel(const __grid_cons
           asm volatile("bar.sync 1, 128;" ::: "memory");
           __threadfence();
           {
-            const int et = (warp - 2) * 32 + lane;                // 0..127 (warps 2..5)
+            const int et = warp * 32 + lane;                      // 0..127 (warps 0..3)
             const int r_begin = split_begin(kBM, p.k_splits, ks), r_end = split_begin(kBM, p.k_splits, ks + 1);
             int ncols = p.out_cols - n0;
             if (ncols > BN) ncols = BN;
@@ -877,7 +734,7 @@ __global__ void __launch_bounds__(kThreads, 1) igemm_tc_kernel(const __grid_cons
             }
           }
           asm volatile("bar.sync 1, 128;" ::: "memory");          // every thread is done reading the partials
-          if (warp == 2 && lane == 0) {
+          if (warp == 0 && lane == 0) {
             if (atomicAdd(counter, 1) == 2 * p.k_splits - 1) *counter = 0;     // leave the tickets zero for the next call
           }
           continue;
@@ -899,8 +756,7 @@ __global__ void __launch_bounds__(kThreads, 1) igemm_tc_kernel(const __grid_cons
         __syncwarp();
         {
           // all loads first: with the column tile as the fastest tile index a GEMM-shaped call refreshes this vector
-          // for EVERY tile, and a load -> add chain per element cost eight L2 round trips per tile (a third of the
-          // epilogue of the K = 256 linears of the transformer blocks, ncu source view of round 2)
+          // for EVERY tile, and a load -> add chain per element would cost eight L2 round trips per tile
           float bv[PER], rw[PER];
 #pragma unroll
           for (int i = 0; i < PER; ++i) {
@@ -916,7 +772,7 @@ __global__ void __launch_bounds__(kThreads, 1) igemm_tc_kernel(const __grid_cons
         __syncwarp();
       }
       // the NEXT tile's vector, if it differs: requested now, written to the other buffer after this tile's chunks (one
-      // L2 round trip per tile otherwise — 15 % of the lean epilogue's samples in the ncu source view)
+      // exposed L2 round trip per tile otherwise)
       float nbv[PER], nrw[PER];
       int want_key = -1;
       if (fast_ok && p.bias_prefetch && tile + n_workers < p.num_tiles) {
@@ -940,13 +796,9 @@ __global__ void __launch_bounds__(kThreads, 1) igemm_tc_kernel(const __grid_cons
       uint4 rv_next[CH / 8];
       if (res_fast && n0 + CH <= p.cout) load_res_fast<CH>(p, rv_next, res_off, n0);
 
-      const int buf = it & 1;
-      const uint32_t acc_phase = (it >> 1) & 1;
-      mbar_wait(tfull_bar(buf), acc_phase);
-      tcgen05_fence_after();
-      const uint32_t taddr = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + buf * BN;
+      mbar_wait(tfull_bar, it & 1);
       float run_max = -INFINITY, run_sum = 0.f;
-      float* my_tile = stage_tiles + (warp - 2) * (32 * (CH + 1));
+      float* my_tile = stage_tiles + warp * (32 * (CH + 1));
       int c0 = 0;
       if constexpr (CH == 32 && BN >= 64) {
         if (p.geglu) {
@@ -956,9 +808,8 @@ __global__ void __launch_bounds__(kThreads, 1) igemm_tc_kernel(const __grid_cons
 #pragma unroll 1
           for (; c0 + 64 <= BN && n0 + c0 + 64 <= p.cout; c0 += 64) {
             uint32_t ra[32], rg[32];
-            tmem_ld32(taddr + c0, ra);
-            tmem_ld32(taddr + c0 + 32, rg);
-            tmem_ld_wait();
+            acc_ld<32>(acc_row + c0, ra);
+            acc_ld<32>(acc_row + c0 + 32, rg);
             if (row_ok) {
               float v[32];
 #pragma unroll
@@ -990,12 +841,6 @@ __global__ void __launch_bounds__(kThreads, 1) igemm_tc_kernel(const __grid_cons
         }
       }
       if (lean_ok) {
-        // (A shared-memory transposed variant — two chunks staged per warp, eight lanes writing each row's whole
-        //  128-byte line — measured no faster: 65 -> 71 us on the 32768 x 2048 x 256 feed-forward GEMM; the
-        //  row-per-thread 256-bit stores stay.)
-        // (Issuing the accumulator read of chunk k + 1 before chunk k is converted and stored — two register
-        //  buffers, loop unrolled by two — measured neutral: 57.3 vs 58.5 us; the tcgen05.ld latency is not
-        //  what the single epilogue warp per scheduler waits for.)
 #pragma unroll 1
         for (; c0 < BN && n0 + c0 + CH <= p.cout; c0 += CH) {       // warp-uniform: full chunks of real columns
           uint4 rv[CH / 8];
@@ -1004,9 +849,7 @@ __global__ void __launch_bounds__(kThreads, 1) igemm_tc_kernel(const __grid_cons
           if (res_fast && c0 + CH < BN && n0 + c0 + 2 * CH <= p.cout)
             load_res_fast<CH>(p, rv_next, res_off, n0 + c0 + CH);
           uint32_t raw[CH];
-          if constexpr (CH == 32) tmem_ld32(taddr + c0, raw);
-          else tmem_ld16(taddr + c0, raw);
-          tmem_ld_wait();
+          acc_ld<CH>(acc_row + c0, raw);
           if (row_ok) {
             if (p.res_ptr) epilogue_lean<CH, true>(p, raw, addv + c0, rv, out_off, n0 + c0);
             else epilogue_lean<CH, false>(p, raw, addv + c0, rv, out_off, n0 + c0);
@@ -1023,9 +866,7 @@ __global__ void __launch_bounds__(kThreads, 1) igemm_tc_kernel(const __grid_cons
           if (res_fast && c0 + CH < BN && n0 + c0 + 2 * CH <= p.cout)
             load_res_fast<CH>(p, rv_next, res_off, n0 + c0 + CH);      // next chunk's residual, one chunk ahead
           uint32_t raw[CH];
-          if constexpr (CH == 32) tmem_ld32(taddr + c0, raw);
-          else tmem_ld16(taddr + c0, raw);
-          tmem_ld_wait();
+          acc_ld<CH>(acc_row + c0, raw);
           float gs[16] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
           if (row_ok) {
             if (p.row_bias) {                       // operand-swapped GEMMs (V^T = W X^T): the bias runs along the rows
@@ -1094,9 +935,7 @@ __global__ void __launch_bounds__(kThreads, 1) igemm_tc_kernel(const __grid_cons
           continue;
         }
         uint32_t raw[CH];
-        if constexpr (CH == 32) tmem_ld32(taddr + c0, raw);
-        else tmem_ld16(taddr + c0, raw);
-        tmem_ld_wait();
+        acc_ld<CH>(acc_row + c0, raw);
         float v[CH];
 #pragma unroll
         for (int j = 0; j < CH; ++j) v[j] = __uint_as_float(raw[j]);
@@ -1130,27 +969,13 @@ __global__ void __launch_bounds__(kThreads, 1) igemm_tc_kernel(const __grid_cons
           if (lane + 32 * i < BN) addv_other[lane + 32 * i] = nbv[i] + nrw[i];
         next_key = want_key;
       }
-      tcgen05_fence_before();
       __syncwarp();
-      if (lane == 0) {
-        if constexpr (PAIR) mbar_arrive_leader(tempty_bar(buf)); else mbar_arrive(tempty_bar(buf));
-      }
+      if (lane == 0) mbar_arrive(tempty_bar);
     }
     if (gn_on) { __syncwarp(); gn_flush(); }
   }
 
-  tcgen05_fence_before();
   __syncthreads();
-  if constexpr (PAIR) cluster_sync_all();     // neither CTA may leave (or free tensor memory) while the pair is in use
-  if (warp == 1) {
-    tcgen05_fence_after();
-    if constexpr (PAIR)
-      asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)kTmemCols)
-                   : "memory");
-    else
-      asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)kTmemCols)
-                   : "memory");
-  }
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1289,8 +1114,8 @@ __global__ void __launch_bounds__(256) igemm_split_reduce_kernel(const IgemmDev 
   float v[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
   const float* src = ws + row * ws_cols + col0;
   int s = 0;
-  // eight (then four) ranges' loads in flight per thread, additions in range order: the plain load -> add loop was one
-  // L2 round trip per range (8-12 us per call in the ncu lists of the latent UNets, as long as the GEMM it completes)
+  // eight (then four) ranges' loads in flight per thread, additions in range order: the plain load -> add loop is one
+  // L2 round trip per range
   for (; s + 8 <= splits; s += 8, src += 8 * ws_stride) {
     float4 a[8], b[8];
 #pragma unroll
@@ -1348,10 +1173,9 @@ struct Plan {
 };
 // dev knobs (read once): the shortest reduction, in 64-element chunks, for which an under-filled grid narrows its
 // column tile within one wave (B200_NARROW_MIN_CHUNKS, default 4), and the fewest ranges a split reduction must have to be worth its
-// fp32 partials + second kernel (B200_SPLIT_MIN, default 3: every two-range split measured lost to the one-pass kernel), and the shortest range, in chunks, a split may leave each
-// CTA (B200_SPLIT_RANGE_MIN, default 32: measured per shape and on graph-replayed UNet steps with 4 / 12 / 24 — a
-// split only pays when every range still has ~2 000 elements of reduction to hide its partial stores and the second
-// kernel behind; C2 step 1.74 -> 1.59 ms, C5 5.18 -> 5.08 ms, brain-LDM 6.89 -> 6.65 ms from 4 to 24)
+// fp32 partials + second kernel (B200_SPLIT_MIN, default 3), and the shortest range, in chunks, a split may leave each
+// CTA (B200_SPLIT_RANGE_MIN, default 32: a split only pays when every range still has ~2 000 elements of reduction to
+// hide its partial stores and the second kernel behind)
 static int env_int(const char* name, int dflt) {
   const char* e = getenv(name);
   return (e && *e) ? atoi(e) : dflt;
@@ -1375,12 +1199,12 @@ static Plan make_plan(const b200_igemm_params* p, bool allow_split, int nsm = 0)
   pl.splits = 1;
   pl.ws_cols = ((p->out_cols + 7) / 8) * 8;
   pl.ws_bytes = 0;
-  // N tile: as wide as the output needs
+  // N tile: as wide as the output needs, up to 128 columns (the widest tile whose fp32 hand-off buffer and a 4-deep
+  // operand ring fit the 227 KB of shared memory a block may use)
   const int cols16 = (((p->act1 == B200_ACT_GEGLU ? p->cout : p->out_cols) + 15) / 16) * 16;   // GEGLU: tile the GEMM's columns
-  int BN = cols16 <= 16 ? 16 : cols16 <= 32 ? 32 : cols16 <= 64 ? 64 : cols16 <= 128 ? 128 : 256;
-  if (p->stat_ptr) BN = 256;      // the caller sizes the partials buffer for 256-column tiles
-  // A grid that cannot fill the SMs: keep the wide tile (operand traffic from L2 per FLOP falls with the tile width —
-  // measured: 64-wide tiles of a 1400-row x 13824-deep convolution stream 456 MB at the L2's ~6.4 TB/s) and cut the
+  int BN = cols16 <= 16 ? 16 : cols16 <= 32 ? 32 : cols16 <= 64 ? 64 : 128;
+  if (p->stat_ptr) BN = 128;      // the caller sizes the partials buffer for 128-column tiles
+  // A grid that cannot fill the SMs: keep the wide tile (operand traffic from L2 per FLOP falls with the tile width) and cut the
   // reduction into ranges instead, when the caller brought a workspace and the reduction is long enough for at least
   // two ranges of four 64-element chunks.
   const long long wide_tiles = pl.m_tiles * ((cols16 + BN - 1) / BN);
@@ -1396,16 +1220,13 @@ static Plan make_plan(const b200_igemm_params* p, bool allow_split, int nsm = 0)
   }
   // otherwise narrower tiles, down to 64 columns, to put more CTAs on the problem
   if (pl.splits == 1) {
-    if (!narrow_one_wave())   // the round-1 rule (B200_NARROW_ONE_WAVE=0): narrow while the grid is under-filled, into a second wave
+    if (!narrow_one_wave())   // B200_NARROW_ONE_WAVE=0: narrow while the grid is under-filled, into a second wave
       while (!p->stat_ptr && BN > 64 && pl.m_tiles * ((cols16 + BN - 1) / BN) < nsm && pl.kchunks >= 8) BN >>= 1;
-    else      // stop at ONE wave: a second wave of 64-column tiles streams every A tile four times from L2 — measured
-              // 8192 x 256 x 2304: 24.8 -> 15.5 us, 8192 x 256 x 4608: 43.2 -> 26.4 us (faster than its two-range split:
-              // 36.5), 8192 x 512 x 4608: 47.1 -> 35.6 us; UNet steps: C2 at batch 32 4.30 -> 3.95 ms, brain-LDM 6.18 -> 5.86 ms
+    else      // stop at ONE wave: a second wave of 64-column tiles streams every A tile four times from L2
       while (!p->stat_ptr && BN > 64 && pl.kchunks >= 8 &&
              pl.m_tiles * ((cols16 + BN / 2 - 1) / (BN / 2)) <= nsm) BN >>= 1;
     // short reductions (K = 256 / 384: the transformer linears) are epilogue-bound: halve the column tile while the
-    // narrower tiles still fit ONE wave (measured: 8192 x 256 x 256 + residual 8.9 -> 7.3 us, 1024 x 256 x 256
-    // 7.3 -> 5.2 us; going past one wave — 8192 x 512 — loses)
+    // narrower tiles still fit ONE wave
     while (!p->stat_ptr && BN > 64 && pl.kchunks >= narrow_min_chunks() && pl.kchunks < 8 &&
            pl.m_tiles * ((cols16 + BN / 2 - 1) / (BN / 2)) <= nsm) BN >>= 1;
   }
@@ -1415,39 +1236,21 @@ static Plan make_plan(const b200_igemm_params* p, bool allow_split, int nsm = 0)
   return pl;
 }
 
-template <int BN, int STAGES, bool PAIR = false>
+template <int BN, int STAGES>
 static int launch_tc(const IgemmDev& d, cudaStream_t stream) {
-  constexpr int kStageBytes = kABytes + (PAIR ? BN / 2 : BN) * kBK * 2;
-  constexpr int smem = STAGES * kStageBytes + 1024 + 256 + 4 * 32 * 33 * 4 + 8 * BN * 4;
+  constexpr int kStageBytes = kABytes + BN * kBK * 2;
+  constexpr int smem = 1024 + STAGES * kStageBytes + kBM * (BN + 4) * 4 + 256 + 4 * 32 * 33 * 4 + 8 * BN * 4;
+  static_assert(smem <= 227 * 1024, "igemm: shared memory over the 227 KB a block may use");
   static std::once_flag attr_once;          // per instantiation; read-only afterwards (re-entrant entry point)
   static cudaError_t attr_rc = cudaSuccess;
   std::call_once(attr_once, [] {
-    attr_rc = cudaFuncSetAttribute(igemm_tc_kernel<BN, STAGES, PAIR>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    attr_rc = cudaFuncSetAttribute(igemm_tc_kernel<BN, STAGES>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
   });
   B200_CUDA(attr_rc);
-  if constexpr (PAIR) {
-    const int pairs = sm_count() / 2;
-    const int grid = 2 * (d.num_tiles < pairs ? d.num_tiles : pairs);
-    B200_CUDA(b200::launch_cluster(igemm_tc_kernel<BN, STAGES, PAIR>, 2, grid, kThreads, smem, stream, d));
-  } else {
-    int grid = d.num_tiles < sm_count() ? d.num_tiles : sm_count();
-    B200_CUDA(b200::launch_pdl(igemm_tc_kernel<BN, STAGES, PAIR>, grid, kThreads, smem, stream, d));
-  }
+  const int grid = d.num_tiles < sm_count() ? d.num_tiles : sm_count();
+  B200_CUDA(b200::launch_pdl(igemm_tc_kernel<BN, STAGES>, grid, kThreads, smem, stream, d));
   B200_LAUNCH_CHECK("igemm_tc_kernel");
   return B200_OK;
-}
-
-// the CTA-pair variant of the 256-column kernel (0 / 1; B200_IGEMM_PAIR overrides the build default)
-#ifndef B200_IGEMM_PAIR_DEFAULT
-#define B200_IGEMM_PAIR_DEFAULT 1
-#endif
-static bool igemm_pair_mode() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("B200_IGEMM_PAIR");
-    v = e ? (e[0] != '0') : B200_IGEMM_PAIR_DEFAULT;
-  }
-  return v != 0;
 }
 
 static int env_impl() {
@@ -1472,18 +1275,17 @@ extern "C" int64_t b200_igemm_split_workspace_bytes(const b200_igemm_params* p) 
 }
 
 // Host-only planning query (no CUDA call): the column tile, the split factor and the tile count b200_igemm would use
-// for this call on a GPU with `sm_count` SMs — lets the binding layer's CPU tests pin the planner's rules.
+// for this call on a GPU with `sm_count` SMs — lets the binding layer's CPU tests pin the planner's rules.  out[3] is
+// always 0 (reserved: the kernel has a single-CTA variant only).
 extern "C" int b200_igemm_plan(const b200_igemm_params* p, int32_t sm_count_, int32_t with_workspace, int32_t out[4]) {
   if (!p || !out || sm_count_ < 1 || p->n_seg < 1 || p->n_seg > B200_IGEMM_MAX_SEG || p->out_N < 1 || p->out_D < 1 ||
       p->out_H < 1 || p->out_W < 1 || p->out_cols < 1)
     return B200_EINVAL;
   const Plan pl = make_plan(p, with_workspace != 0, sm_count_);
-  const bool pair = igemm_pair_mode() && (pl.BN == 256 || pl.BN == 128) && pl.splits == 1 && !p->stat_ptr &&
-                    pl.m_tiles >= 2 && pl.ntiles >= sm_count_ && (!p->w_batched || ((pl.m_tiles / p->out_N) % 2 == 0));
   out[0] = pl.BN;
   out[1] = pl.splits;
   out[2] = (int32_t)pl.ntiles;
-  out[3] = pair ? 1 : 0;
+  out[3] = 0;
   return B200_OK;
 }
 
@@ -1629,14 +1431,6 @@ extern "C" int b200_igemm(const b200_igemm_params* p, void* stream_v) {
   }
   B200_CHECK_ARG(pl.ntiles * splits < (1ll << 31), "igemm: too many tiles");
   d.num_tiles = (int)pl.ntiles;
-  // CTA pairs for the 256- and 128-column calls that fill the machine (at least one tile per SM — pairs of M tiles over pairs
-  // of SMs quantise like single tiles over single SMs), no split-K / score statistics / staged stores
-  const bool pair = igemm_pair_mode() && (BN == 256 || BN == 128) && splits == 1 && !p->stat_ptr && !d.out_staged &&
-                    pl.m_tiles >= 2 && pl.ntiles >= sm_count() &&
-                    // a pair shares ONE column tile of ONE weight batch: with per-sample weights the two M tiles of a
-                    // pair must belong to the same sample
-                    (!p->w_batched || ((pl.m_tiles / p->out_N) % 2 == 0));
-  if (pair) d.num_tiles = (int)(((pl.m_tiles + 1) / 2) * pl.tiles_n);
 
   // ---- tensor maps ----
   for (int s = 0; s < 2; ++s) {
@@ -1666,7 +1460,7 @@ extern "C" int b200_igemm(const b200_igemm_params* p, void* stream_v) {
     cuuint64_t bs = p->w_bstride ? (cuuint64_t)p->w_bstride * 2 : (cuuint64_t)p->w_rows * p->w_pitch * 2;
     cuuint64_t strides[2] = {(cuuint64_t)p->w_pitch * 2, bs};
     B200_CHECK_ARG(bs % 16 == 0, "igemm: weight batch stride not 16-byte aligned");
-    cuuint32_t box[3] = {(cuuint32_t)kBK, (cuuint32_t)(pair ? BN / 2 : BN), 1};     // pair: each CTA stages half the rows
+    cuuint32_t box[3] = {(cuuint32_t)kBK, (cuuint32_t)BN, 1};
     cuuint32_t estr[3] = {1, 1, 1};
     CUresult r = g_encode(&d.tmB, B200_H16_TMAP, 3, const_cast<void*>(p->w_ptr), dims,
                           strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
@@ -1682,9 +1476,8 @@ extern "C" int b200_igemm(const b200_igemm_params* p, void* stream_v) {
     switch (BN) {
       case 16:  return launch_tc<16, 8>(dev, stream);
       case 32:  return launch_tc<32, 8>(dev, stream);
-      case 64:  return launch_tc<64, 8>(dev, stream);
-      case 128: return pair ? launch_tc<128, 8, true>(dev, stream) : launch_tc<128, 6>(dev, stream);
-      default:  return pair ? launch_tc<256, 6, true>(dev, stream) : launch_tc<256, 4>(dev, stream);
+      case 64:  return launch_tc<64, 6>(dev, stream);
+      default:  return launch_tc<128, 4>(dev, stream);
     }
   };
   if (splits == 1) return launch(d);

@@ -104,8 +104,8 @@ __global__ void gn_finalize_kernel(const float* __restrict__ partial, int chunks
   const int g = blockIdx.x, n = blockIdx.y;
   const int cpg = C / groups;
   double s = 0.0, q = 0.0;
-  // four (sum, sum of squares) pairs in flight per thread: a plain load -> add loop was ~9 dependent L2 round trips per
-  // thread (10-26 us for a few kilobytes of partials in the ncu lists of C5's 256 x 256 level); same addition order
+  // four (sum, sum of squares) pairs in flight per thread: a plain load -> add loop is ~9 dependent L2 round trips per
+  // thread for a few kilobytes of partials; same addition order
   const int total = chunks * cpg;
   int i = threadIdx.x;
   for (; i + 3 * (int)blockDim.x < total; i += 4 * blockDim.x) {
@@ -336,7 +336,7 @@ __device__ __forceinline__ void gn_store_vec(h16* p, const float* f) {
 
 // KREG > 0 (VEC == 8 only): every thread keeps its (at most KREG) row vectors in registers between the statistics and
 // the normalisation, so the tensor is read once (the second pass of the KREG = 0 form re-reads it from L1 / L2 behind
-// one more dependent-latency chain: 4096-row tensors of C5's 64 x 64 level took 15 us per call).
+// one more dependent-latency chain).
 template <int VEC, int KREG = 0>
 __global__ void __launch_bounds__(512) gn_fused_small_kernel(const h16* __restrict__ x0,
                                                              const h16* __restrict__ x1, int C0, int C1,

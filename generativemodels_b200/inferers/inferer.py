@@ -46,8 +46,8 @@ def _with_seg(diffusion_model, seg):
 
 
 # Replay the network from a CUDA graph inside ``sample`` when one step is launch-latency-bound (a latent UNet step is
-# 150-500 dependent launches of a few microseconds: C2 at batch 1 goes from 3.4 to 8.7 samples/s).  On by default since
-# round 2 (the -m gpu suite runs with it; graph-replayed and eager sampling are bit-identical, incl. PNDM's history).
+# 150-500 dependent launches of a few microseconds).  On by default (the -m gpu suite runs with it; graph-replayed and
+# eager sampling are bit-identical, incl. PNDM's history).
 # ``B200_AUTO_GRAPH=0`` or setting this flag to False turns it off.
 AUTO_CUDA_GRAPH = os.environ.get("B200_AUTO_GRAPH", "1") != "0"
 _AUTO_GRAPH_MAX_NUMEL = 1 << 18          # per-sample elements of the network input (64^3, 512^2): above, work dominates

@@ -2,7 +2,7 @@
 
 The modules keep the reference's module tree and ``state_dict`` keys (SURVEY.md §8b) by holding their parameters in
 ordinary ``torch.nn`` layers that are never *called*: ``forward`` hands the weights — repacked once into the K-major
-h16 layout the tcgen05 kernel wants and cached against the parameter's version — to the C-ABI operators.
+h16 layout the wgmma kernel wants and cached against the parameter's version — to the C-ABI operators.
 """
 from __future__ import annotations
 
@@ -44,7 +44,7 @@ def act_code(act) -> int:
         raise NotImplementedError(f"activation {act!r} with non-default arguments is not supported")
     code = _ACT_CODES.get(str(name).upper())
     if code is None:
-        raise NotImplementedError(f"activation {name!r} is not supported on the B200 path ({sorted(_ACT_CODES)})")
+        raise NotImplementedError(f"activation {name!r} is not supported on the CUDA path ({sorted(_ACT_CODES)})")
     return code
 
 
@@ -166,7 +166,7 @@ def f32(p: torch.Tensor) -> torch.Tensor:
 
 def require_cuda(x: torch.Tensor, module: nn.Module):
     if not x.is_cuda:
-        raise RuntimeError(f"{type(module).__name__}: generativemodels_b200 runs on sm_100a CUDA devices only "
+        raise RuntimeError(f"{type(module).__name__}: generativemodels_b200 runs on sm_90a (H100) CUDA devices only "
                            "(input tensor is on the CPU and there is no CPU path)")
 
 

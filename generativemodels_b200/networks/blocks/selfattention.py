@@ -1,4 +1,4 @@
-"""SABlock — ``generative/networks/blocks/selfattention.py:33-148`` on the B200 kernels: multi-head (causal) self- or
+"""SABlock — ``generative/networks/blocks/selfattention.py:33-148`` on the H100 kernels: multi-head (causal) self- or
 cross-attention with bias-free q / k / v projections and an output projection.  Token rows stay packed
 [B*T, hidden]; heads are channel slices, the causal mask is an index comparison inside the attention kernel (the
 ``causal_mask`` buffer is kept only so that reference state_dicts load strictly)."""

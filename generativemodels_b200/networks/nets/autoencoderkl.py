@@ -1,4 +1,4 @@
-"""AutoencoderKL on the B200 kernels — classes, arguments and state_dict keys of
+"""AutoencoderKL on the H100 kernels — classes, arguments and state_dict keys of
 generative/networks/nets/autoencoderkl.py (reference lines cited per class)."""
 from __future__ import annotations
 

@@ -1,4 +1,4 @@
-"""ControlNet on the B200 kernels — classes, arguments and state_dict keys of
+"""ControlNet on the H100 kernels — classes, arguments and state_dict keys of
 generative/networks/nets/controlnet.py (reference lines cited per class)."""
 from __future__ import annotations
 

@@ -1,11 +1,11 @@
-"""DiffusionModelUNet on the B200 kernels — same classes, constructor arguments, attribute names and ``state_dict``
+"""DiffusionModelUNet on the H100 kernels — same classes, constructor arguments, attribute names and ``state_dict``
 keys as generative/networks/nets/diffusion_model_unet.py (reference lines cited per class), different insides:
 
 * activations stay channels-last h16 (:class:`~generativemodels_b200.ops.CL`) from ``conv_in`` to the output head;
-* every ResnetBlock is  GN-stats -> GN-apply+SiLU -> tcgen05 conv (+bias +time-embedding row vector in the epilogue)
-  -> GN -> tcgen05 conv (+bias +skip/residual in the epilogue);
+* every ResnetBlock is  GN-stats -> GN-apply+SiLU -> wgmma conv (+bias +time-embedding row vector in the epilogue)
+  -> GN -> wgmma conv (+bias +skip/residual in the epilogue);
 * the up path never materialises ``torch.cat([h, skip])`` raw: GroupNorm and the 1x1 skip conv read both tensors;
-* attention runs as tcgen05 GEMMs (QK^T, PV with V^T from an operand-swapped projection) or, for tiny heads /
+* attention runs as the flash-style wgmma kernel, as wgmma GEMMs (QK^T, PV with V^T from an operand-swapped projection) or, for tiny heads /
   a handful of context tokens, the CUDA-core online-softmax kernel.
 Inference only (``torch.no_grad`` semantics); there is no CPU path.
 """
@@ -52,8 +52,8 @@ def _context_cl(context: torch.Tensor) -> CL:
 
 def _few_rows_linear(x: CL, pl) -> torch.Tensor:
     """Projection of a token matrix to packed rows [N, S, pitch].  A handful of tokens in total (the context of a
-    classifier-free-guidance step: one token per sample) goes through the GEMV kernel — a tcgen05 launch costs ~9 us
-    for two rows, 14 of them per C5 UNet forward."""
+    classifier-free-guidance step: one token per sample) goes through the GEMV kernel — a 128-row tensor-core tile
+    spends its pipeline latency on two rows, 14 of them per C5 UNet forward."""
     rows = x.N * x.spatial
     if rows <= 8 and x.C * rows * 2 <= 32 * 1024:
         y = ops.rows_linear(x.t.reshape(rows, x.pitch), x.C, pl)
@@ -258,7 +258,7 @@ class TimeEmb:
     """The time embedding of one forward together with every ResnetBlock's ``time_emb_proj(silu(emb))`` row
     (diffusion_model_unet.py:686-689), which depend on the timestep only: all of them come out of ONE GEMV launch over
     the row-concatenated projection weights instead of one launch per block (a latent UNet step is ~300-500 dependent
-    launches of a few microseconds each — see DESIGN.md, latency-bound configurations).  ``proj[id(block)]`` is a
+    launches of a few microseconds each).  ``proj[id(block)]`` is a
     column slice ``[rows, out_channels]`` of that result; the conv epilogue reads it through its row stride."""
 
     __slots__ = ("emb", "proj")

@@ -1,4 +1,4 @@
-"""SPADEAutoencoderKL — ``generative/networks/nets/spade_autoencoderkl.py:292-484`` on the B200 kernels: AutoencoderKL
+"""SPADEAutoencoderKL — ``generative/networks/nets/spade_autoencoderkl.py:292-484`` on the H100 kernels: AutoencoderKL
 whose decoder ResBlocks use SPADE norms (GroupNorm without affine at PyTorch's default eps, modulated by the
 segmentation map); the encoder is the plain one.  Same state_dict keys, ``decode(z, seg)`` / ``forward(x, seg)``."""
 from __future__ import annotations

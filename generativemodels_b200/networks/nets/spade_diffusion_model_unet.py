@@ -1,4 +1,4 @@
-"""SPADEDiffusionModelUNet — ``generative/networks/nets/spade_diffusion_model_unet.py:612-912`` on the B200 kernels.
+"""SPADEDiffusionModelUNet — ``generative/networks/nets/spade_diffusion_model_unet.py:612-912`` on the H100 kernels.
 
 The reference class is DiffusionModelUNet whose up path uses ResnetBlocks with SPADE norms (semantic conditioning
 by a segmentation map, Park et al. 2019); encoder, middle block, attention and heads are identical and so are the

@@ -1,4 +1,4 @@
-"""DecoderOnlyTransformer — ``generative/networks/nets/transformer.py:20-106`` on the B200 kernels (SURVEY.md §8f rank 3).
+"""DecoderOnlyTransformer — ``generative/networks/nets/transformer.py:20-106`` on the H100 kernels (SURVEY.md §8f rank 3).
 
 Same constructor, ``forward(x, context)`` -> logits [B, T, num_tokens] (fp32) and state_dict keys as the reference.
 Beyond that interface the class offers the incremental form the sampler wants: ``new_cache`` / ``step`` keep every

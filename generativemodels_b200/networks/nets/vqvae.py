@@ -1,4 +1,4 @@
-"""VQVAE on the B200 kernels — classes, arguments and state_dict keys of generative/networks/nets/vqvae.py."""
+"""VQVAE on the H100 kernels — classes, arguments and state_dict keys of generative/networks/nets/vqvae.py."""
 from __future__ import annotations
 
 from collections.abc import Sequence
@@ -189,7 +189,7 @@ class VQVAE(nn.Module):
     @torch.no_grad()
     def forward(self, images: torch.Tensor) -> tuple[torch.Tensor, torch.Tensor]:
         if self.training:
-            raise RuntimeError("VQVAE.forward on the B200 kernels is inference-only; call .eval() first")
+            raise RuntimeError("VQVAE.forward on the H100 kernels is inference-only; call .eval() first")
         r = self.quantizer.forward_cl(self._encode_cl(images), want_f32=False)
         return self._decode_cl(r["q"]), r["loss"]
 

@@ -234,8 +234,7 @@ class PackedConv:
         elif (taps > 1 and len(self.splits) == 1 and self.cout <= 4 and taps * self.cout <= 128 and cin >= 64
               and self.stride == (1, 1, 1)):
             # [tap*cout + co][c]; the GEMM's column count is rounded up to 32 (zero rows): full 32-column chunks take
-            # the vectorised epilogue (27 columns went through the per-element path: 2.3 ms for the C3 output
-            # convolution's 5.7 M rows against 0.5 ms of HBM time)
+            # the vectorised epilogue (27 columns would go through the much slower per-element path)
             ncol = round_up(taps * self.cout, 32)
             self.tap_out = PackedLinear.from_packed(repack(w, self.cout, cin, taps, None, ncol,
                                                            mode=_lib.REPACK_TAP_OUT, pitch=round_up(cin, 64)),
@@ -459,8 +458,7 @@ def _fill_segs(p: IgemmParams, segs) -> None:
 
 _SPLIT_K = os.environ.get("B200_SPLIT_K", "1") != "0"    # dev switch (tests compare split and one-pass reductions)
 # one launch (per-tile tickets, the CTAs of a tile reduce it cooperatively) instead of GEMM + reduce kernel.  Off by default:
-# the first form (the LAST CTA of a tile reduced all of it, one row per thread) measured 4x slower end to end (C2 UNet
-# step 1.79 -> 7.88 ms, brain-LDM 7.12 -> 11.29 ms); B200_SPLIT_FUSED=1 selects the cooperative form for A/B runs.
+# B200_SPLIT_FUSED=1 selects the cooperative form for A/B runs.
 _SPLIT_FUSED = os.environ.get("B200_SPLIT_FUSED", "0") != "0"
 _SPLIT_COUNTERS: dict = {}       # device index -> int32 [IGEMM_SPLIT_COUNTERS] zeros (self-resetting tickets)
 
@@ -714,9 +712,8 @@ def groupnorm_affine(srcs: CL | Sequence[CL], groups: int, eps: float, gamma: to
 
 
 # Single-launch GroupNorm for small tensors (b200_groupnorm_fused): one CTA per (sample, group) computes the statistics
-# and applies them — GroupNorm is 138 of the 309 launches of a C2 latent-UNet step as three kernels.  Verified on a B200
-# in round 2 (the full -m gpu suite with it on; C2 UNet step 2.28 -> 1.88 ms, brain-LDM UNet 7.65 -> 7.39 ms, graph
-# replayed).  B200_GN_SMALL=0 turns it off.
+# and applies them — GroupNorm is 138 of the 309 launches of a C2 latent-UNet step as three kernels (the -m gpu suite
+# runs with it on).  B200_GN_SMALL=0 turns it off.
 _GN_SMALL = os.environ.get("B200_GN_SMALL", "1") != "0"
 _GN_SMALL_MAX_ELEMS = 1 << 17           # spatial * channels-per-group handled by one CTA
 
@@ -920,9 +917,6 @@ def linear_geglu(x: CL, pl: PackedLinear) -> CL:
 _TC_ATTN_MIN_S = 64
 _FLASH_HEAD_DIMS = (64, 128, 256, 512)
 _FORCE_UNFUSED_ATTENTION = False      # tests flip this to cover the GEMM + softmax + GEMM path
-_LAST_FLASH_WS = None
-_KEEP_FLASH_WS = False
-_FLASH_REPLAY = True                  # tests flip this to compare the replay and recompute variants of head_dim 512
 _ATTN_CHUNK_BYTES = 6 << 30   # fp32 score slab per query chunk
 
 
@@ -932,7 +926,7 @@ def attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, heads: int, dh:
 
     Tensor-core paths (head_dim % 64 == 0, S >= 64; ``vt`` must hold V^T ``[B, H*dh, S_pitch]``, produced for free
     by swapping the operands of the V projection):
-      * head_dim in {64, 128, 256, 512}: the flash-style tcgen05 kernel — scores stay in TMEM, online softmax;
+      * head_dim in {64, 128, 256, 512}: the flash-style wgmma kernel — scores stay in registers, online softmax;
       * other multiples of 64 (e.g. 768): per (batch, head) QK^T -> fp32 scores (+ softmax partials from the GEMM
         epilogue), one-pass row softmax -> h16, PV, in query slabs so the score matrix never exceeds a few GB.
     Everything else runs on the CUDA-core online-softmax kernel.  ``residual`` ([B, T, pitch] h16) is added in
@@ -968,22 +962,13 @@ def attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, heads: int, dh:
         fp.scale = scale
         if out.shape[2] > heads * dh:
             out.zero_()
-        ws = None
-        if _FLASH_REPLAY:
-            need = int(lib.b200_attention_flash_workspace_bytes(C.byref(fp)))
-            if need:        # head_dim 512: probability tiles are written once and replayed for the second output half
-                ws = torch.empty(need, dtype=torch.uint8, device=q.device)
-                fp.workspace, fp.workspace_bytes = ws.data_ptr(), need
-                if _KEEP_FLASH_WS:            # dev probes (tools/attn_timing.py) read the kernel's counters from here
-                    global _LAST_FLASH_WS
-                    _LAST_FLASH_WS = ws
         check(lib.b200_attention_flash(C.byref(fp), _stream()), "b200_attention_flash")
         return out
     Sp = round_up(S, 8)
     chunk = max(128, min(T, (_ATTN_CHUNK_BYTES // (4 * Sp)) // 128 * 128))
     scores = torch.empty((min(chunk, T), Sp), dtype=torch.float32, device=q.device)
     probs = torch.empty((min(chunk, T), Sp), dtype=H16, device=q.device)
-    n_tiles = (Sp + 255) // 256
+    n_tiles = (Sp + 127) // 128
     partials = torch.empty((min(chunk, T), n_tiles, 2), dtype=torch.float32, device=q.device)
     nk = round_up(dh, 64) // 64
     ns = round_up(S, 64) // 64
@@ -1005,7 +990,7 @@ def attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, heads: int, dh:
                 p.cout, p.out_cols = S, Sp
                 p.out_sN, p.out_sD, p.out_sH, p.out_sW = tc * Sp, tc * Sp, tc * Sp, Sp
                 p.act1, p.scale, p.act2 = ACT_NONE, scale, ACT_NONE
-                p.stat_ptr = partials.data_ptr()     # epilogue leaves (max, sum exp) per 256-column tile
+                p.stat_ptr = partials.data_ptr()     # epilogue leaves (max, sum exp) per 128-column tile
                 igemm_raw(p)
                 check(lib.b200_softmax_rows_partials(scores.data_ptr(), tc, S, Sp, partials.data_ptr(), n_tiles,
                                                      probs.data_ptr(), Sp, _stream()), "b200_softmax_rows_partials")

@@ -1,5 +1,5 @@
 /*
- * b200gen.h — C-ABI of libb200gen.so: the sm_100a kernels behind the MONAI-GenerativeModels
+ * b200gen.h — C-ABI of libb200gen.so: the sm_90a kernels behind the MONAI-GenerativeModels
  * diffusion *sampling* hot path (SURVEY.md §8).  Plain pointers and sizes only; no torch types.
  *
  * Conventions (SURVEY.md §8(b), inner boundary)
@@ -25,7 +25,7 @@ extern "C" {
 #define B200_EINVAL   -1   /* bad shape / alignment / null pointer                    */
 #define B200_ENOTSUP  -2   /* valid request this build has no kernel for              */
 #define B200_ECUDA    -3   /* CUDA runtime / driver error, see b200_last_error_string */
-#define B200_ENODEV   -4   /* device is not compute capability 10.x                   */
+#define B200_ENODEV   -4   /* device is not compute capability 9.0                    */
 
 /* "h16" = the library's 16-bit storage type for activations and packed weights: IEEE fp16 in libb200gen.so (the
  * default: 11 significand bits, fp32 -> fp16 conversions saturate at +-65504), bfloat16 in the libb200gen_bf16.so
@@ -56,7 +56,7 @@ const char* b200_last_error_string(void);
 int b200_version(void);
 /* B200_H16_FP16 or B200_H16_BF16: the 16-bit format this build stores activations / weights in. */
 int b200_act_dtype(void);
-/* 0 iff the current CUDA device is sm_100-class (fails loudly elsewhere: there is no fallback). */
+/* 0 iff the current CUDA device is sm_90 (fails loudly elsewhere: there is no fallback). */
 int b200_device_check(void);
 int b200_sm_count(void);
 /* sizeof() of the parameter structs below, for binding-layer ABI checks:
@@ -65,7 +65,7 @@ int b200_sm_count(void);
 int b200_abi_sizeof(int which);
 
 /* ------------------------------------------------------------------------------------------------
- * Implicit-GEMM on tcgen05 tensor cores (TMA-staged NDHWC tiles, accumulators in TMEM).
+ * Implicit-GEMM on wgmma tensor cores (TMA-staged NDHWC tiles, accumulators in registers).
  * One kernel family serves every dense contraction on the path:
  *   - nn.Conv2d/3d k in {1,3,4}, stride {1,2}, symmetric or asymmetric zero padding
  *     (monai Convolution call sites: diffusion_model_unet.py:277,303,510,555,625,645,659,1748,1857;
@@ -121,9 +121,9 @@ typedef struct {
   int32_t res_dtype;
   int64_t res_sN, res_sD, res_sH, res_sW;
   int32_t act2;
-  float*  stat_ptr;     /* optional softmax partials: [out_W][ceil(out_cols/256)][2] = (max, sum exp(v - max)) of every
-                           256-column tile of every output row (GEMM-shaped calls only); NULL to skip            */
-  int32_t impl;         /* 0 = tcgen05 kernel, 1 = CUDA-core cross-check kernel  */
+  float*  stat_ptr;     /* optional softmax partials: [out_W][ceil(out_cols/128)][2] = (max, sum exp(v - max)) of every
+                           128-column tile of every output row (GEMM-shaped calls only); NULL to skip            */
+  int32_t impl;         /* 0 = wgmma kernel, 1 = CUDA-core cross-check kernel    */
   /* Optional GroupNorm partial sums for whoever normalises this output next (nn.GroupNorm after every conv of the
    * ResnetBlock, diffusion_model_unet.py:623-684): gn_partial[n][slot][cout/8][2] += (sum, sum of squares) of the
    * stored h16 values per 8-channel group; the kernel uses slots [gn_slot0, gn_slot0 + 4 * SM count) of the
@@ -158,8 +158,8 @@ typedef struct {
 
 int b200_igemm(const b200_igemm_params* p, void* stream);
 /* Host-only planning query, no CUDA call: what b200_igemm would choose for this call on a GPU with sm_count SMs —
- * out = {column tile (16..256), split factor (1 = one pass; > 1 only if with_workspace), output tiles, 1 if the CTA-pair
- * (cta_group::2) kernel would run}.  The rules (DESIGN.md section 2): an under-filled grid narrows its column tile while
+ * out = {column tile (16..128), split factor (1 = one pass; > 1 only if with_workspace), output tiles, 0 (reserved)}.
+ * The rules (DESIGN.md section 2): an under-filled grid narrows its column tile while
  * the tiles still fit one wave; a reduction is split only into >= 3 ranges of >= 32 chunks of 64. */
 int b200_igemm_plan(const b200_igemm_params* p, int32_t sm_count, int32_t with_workspace, int32_t out[4]);
 /* Bytes of split_ws with which b200_igemm would split the reduction of this call; 0 when it would not (enough tiles
@@ -275,11 +275,11 @@ int b200_geglu(const void* x, int64_t M, int32_t H, int32_t x_pitch, void* y, in
  * (attention_scores.softmax(dim=-1), diffusion_model_unet.py:150,412). Pad columns are zeroed. */
 int b200_softmax_rows(const float* s, int64_t M, int32_t S, int64_t s_pitch, void* p, int64_t p_pitch,
                       void* stream);
-/* Same result in ONE pass over the scores, given the per-(row, 256-column tile) partials b200_igemm wrote. */
+/* Same result in ONE pass over the scores, given the per-(row, 128-column tile) partials b200_igemm wrote. */
 int b200_softmax_rows_partials(const float* s, int64_t M, int32_t S, int64_t s_pitch, const float* partials,
                                int32_t n_tiles, void* p, int64_t p_pitch, void* stream);
 
-/* Flash-style attention on tcgen05 (scores stay in TMEM; online softmax; head_dim in {64,128,256,512}, any T, S).
+/* Flash-style attention on wgmma (scores stay in registers; online softmax; head_dim in {64,128,256,512}, any T, S).
  * q: [B][T][q_pitch], k: [B][S][k_pitch] h16 rows with heads as channel slices [h*dh, (h+1)*dh);
  * vt: V transposed, [B][heads*dh][vt_pitch] (key index contiguous); out / res: [B][T][pitch] h16; res may be NULL.
  * out[b,t,h*dh+c] = sum_s softmax_s(scale * q.k)[s] * v[s,c] (+ res).   (diffusion_model_unet.py:143-153, 406-416) */
@@ -288,10 +288,8 @@ typedef struct {
   int32_t B, T, S, heads, dh;
   int32_t q_pitch, k_pitch, vt_pitch, out_pitch, res_pitch;
   float scale;
-  /* Optional device scratch for head_dim 512 (whose 128 x 512 fp32 output tile does not fit tensor memory beside the
-   * scores): with at least b200_attention_flash_workspace_bytes() bytes the kernel computes every probability tile
-   * once and replays it for the second half of the output channels; with NULL it recomputes the scores instead
-   * (same result up to h16 rounding of identical P values, 1.5x the tensor work).  Other head dims ignore it. */
+  /* Reserved scratch: the kernel keeps every probability tile on chip and needs none
+   * (b200_attention_flash_workspace_bytes() returns 0); both fields are ignored. */
   void* workspace; int64_t workspace_bytes;
 } b200_flash_params;
 int b200_attention_flash(const b200_flash_params* p, void* stream);

@@ -5,6 +5,8 @@ from pathlib import Path
 
 import torch
 
+from tests import golden
+
 GOLD = Path(__file__).resolve().parent / "golden"
 
 
@@ -157,7 +159,7 @@ def check_c3_fixture(device, steps=True):
     from generativemodels_b200.networks.nets import DiffusionModelUNet
     from generativemodels_b200.networks.schedulers import DDIMScheduler
     from tests.golden import configs as G
-    fx = torch.load(GOLD / "g_c3.pt", weights_only=False)
+    fx = golden.load("g_c3")
     m = DiffusionModelUNet(**G.C3_UNET).eval()
     G.recipe_state_dict(m, 13)
     assert sum(p.numel() for p in m.parameters()) == fx["n_params"]
@@ -185,7 +187,7 @@ def check_c4_fixture(device):
     counted."""
     from generativemodels_b200.networks.nets import VQVAE
     from tests.golden import configs as G
-    fx = torch.load(GOLD / "g_c4.pt", weights_only=False)
+    fx = golden.load("g_c4")
     m = VQVAE(**G.C4_VQVAE).eval()
     G.recipe_state_dict(m, 14)
     assert sum(p.numel() for p in m.parameters()) == fx["n_params"]
@@ -229,7 +231,7 @@ def check_c5_fixture(device):
     from generativemodels_b200.networks.nets import ControlNet, DiffusionModelUNet
     from generativemodels_b200.networks.schedulers import DDIMScheduler
     from tests.golden import configs as G
-    fx = torch.load(GOLD / "g_c5.pt", weights_only=False)
+    fx = golden.load("g_c5")
     unet = DiffusionModelUNet(**G.C5_UNET).eval()
     cn = ControlNet(**G.C5_CONTROLNET).eval()
     G.recipe_state_dict(unet, 15)

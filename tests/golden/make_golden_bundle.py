@@ -11,6 +11,7 @@ from pathlib import Path
 
 import torch
 
+from tests import golden
 from tests.golden import configs as G      # before the reference import: /root/reference has its own `tests` package
 from oracle import ref_import
 
@@ -35,9 +36,9 @@ def main():
     noise = torch.randn(G.BUNDLE_NOISE)
     conditioning = torch.tensor([[0.0, 0.1, 0.2, 0.4]]).unsqueeze(1)        # inference.json: gender, age, vols
     sample = mod.Sampler().sampling_fn(noise, ae, unet, scheduler, conditioning)
-    torch.save(dict(aekl_kwargs=G.BUNDLE_AEKL, unet_kwargs=G.BUNDLE_UNET, aekl_state=ae.state_dict(),
+    golden.save(dict(aekl_kwargs=G.BUNDLE_AEKL, unet_kwargs=G.BUNDLE_UNET, aekl_state=ae.state_dict(),
                     unet_state=unet.state_dict(), noise=noise, conditioning=conditioning, sample=sample),
-               OUT / "g_bundle_brain_ldm.pt")
+               "g_bundle_brain_ldm")
     f = OUT / "g_bundle_brain_ldm.pt"
     print(f.name, f.stat().st_size, tuple(sample.shape), float(sample.abs().mean()))
 

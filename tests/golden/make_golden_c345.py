@@ -14,6 +14,7 @@ from pathlib import Path
 
 import torch
 
+from tests import golden
 from tests.golden import configs as G      # before the reference import: /root/reference has its own `tests` package
 from oracle import ref_import
 
@@ -34,8 +35,8 @@ def make_c3():
         y500 = m(noise, torch.Tensor((500,)))
         sample, inter = DiffusionInferer(s).sample(input_noise=noise, diffusion_model=m, scheduler=s, verbose=False,
                                                    save_intermediates=True, intermediate_steps=1)
-    torch.save(dict(noise=noise, y500=y500, sample=sample, intermediates=inter, timesteps=[int(t) for t in s.timesteps],
-                    n_params=sum(p.numel() for p in m.parameters())), OUT / "g_c3.pt")
+    golden.save(dict(noise=noise, y500=y500, sample=sample, intermediates=inter, timesteps=[int(t) for t in s.timesteps],
+                    n_params=sum(p.numel() for p in m.parameters())), "g_c3")
     print("g_c3.pt", (OUT / "g_c3.pt").stat().st_size, float(y500.abs().mean()), float(sample.abs().mean()))
 
 
@@ -56,8 +57,8 @@ def make_c4():
         margin = (two[:, 0] - two[:, 1]).reshape(idx.shape)          # >= 0: distance gap second-best minus best
         assert torch.equal(torch.max(-d, 1)[1].reshape(idx.shape), idx)
         recon_from_idx = m.decode_samples(idx)
-    torch.save(dict(x=x, z=z, indices=idx, margin=margin, recon=recon, loss=loss, recon_from_idx=recon_from_idx,
-                    n_params=sum(p.numel() for p in m.parameters())), OUT / "g_c4.pt")
+    golden.save(dict(x=x, z=z, indices=idx, margin=margin, recon=recon, loss=loss, recon_from_idx=recon_from_idx,
+                    n_params=sum(p.numel() for p in m.parameters())), "g_c4")
     print("g_c4.pt", (OUT / "g_c4.pt").stat().st_size, float(recon.abs().mean()), int(idx.unique().numel()),
           float(margin.min()), float(margin.median()))
 
@@ -85,9 +86,9 @@ def make_c5():
         eu, et = eps2.chunk(2)
         eps = eu + G.C5_GUIDANCE * (et - eu)
         nxt, _ = s.step(eps, t, x)
-    torch.save(dict(x=x, t=t, eps2=eps2, eps=eps, nxt=nxt, mid_mean=mid.mean((2, 3)), down_means=[d.mean((2, 3)) for d in down],
+    golden.save(dict(x=x, t=t, eps2=eps2, eps=eps, nxt=nxt, mid_mean=mid.mean((2, 3)), down_means=[d.mean((2, 3)) for d in down],
                     n_params=(sum(p.numel() for p in unet.parameters()), sum(p.numel() for p in cn.parameters()))),
-               OUT / "g_c5.pt")
+               "g_c5")
     print("g_c5.pt", (OUT / "g_c5.pt").stat().st_size, float(eps2.abs().mean()), float(nxt.abs().mean()))
 
 

@@ -127,12 +127,12 @@ def emulate(p: IgemmParams) -> None:
         valid = col < H
     else:
         v = _act(v, p.act1) * np.float32(p.scale)
-    if p.stat_ptr:       # softmax partials per 256-column tile (GEMM-shaped calls): (max, sum exp(v - max))
-        nt = (cols + 255) // 256
+    if p.stat_ptr:       # softmax partials per 128-column tile (GEMM-shaped calls): (max, sum exp(v - max))
+        nt = (cols + 127) // 128
         st = _f32_view(p.stat_ptr, OW * nt * 2).reshape(OW, nt, 2)
         rows2d = v.reshape(OW, cols)
         for t in range(nt):
-            seg = rows2d[:, t * 256:min((t + 1) * 256, p.cout)]
+            seg = rows2d[:, t * 128:min((t + 1) * 128, p.cout)]
             if seg.shape[1] == 0:
                 st[:, t, 0], st[:, t, 1] = -np.inf, 0.0
                 continue

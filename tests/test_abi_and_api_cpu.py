@@ -126,8 +126,9 @@ def test_inferer_error_conventions():
 
 
 def test_igemm_planner_rules():
-    """b200_igemm_plan (host-only, no CUDA call): the planner's column-tile / split-K / CTA-pair decisions for a 148-SM
-    part, pinned on the shapes DESIGN.md section 2 quotes (measured with tools/gemm_probe.py on the B200)."""
+    """b200_igemm_plan (host-only, no CUDA call): the planner's column-tile / split-K decisions for a 132-SM part (H100
+    SXM), pinned on shapes of the UNets DESIGN.md section 2 quotes.  Column tiles are at most 128 wide; out[3] is reserved
+    and always 0."""
     import ctypes as C
     lib = _lib.load()
 
@@ -141,24 +142,24 @@ def test_igemm_planner_rules():
         p.n_seg = 1
         p.seg[0].nchunks = K // 64
         out = (C.c_int32 * 4)()
-        assert lib.b200_igemm_plan(C.byref(p), 148, int(workspace), out) == 0
+        assert lib.b200_igemm_plan(C.byref(p), 132, int(workspace), out) == 0
         return tuple(out)          # (column tile, splits, tiles, pair kernel)
 
-    # machine-filling convolution-sized calls: widest tile, no split, CTA pairs
-    assert plan(5734400, 256, 6912) == (256, 1, 44800, 1)
-    assert plan(131072, 128, 1152) == (128, 1, 1024, 1)
-    # under-filled grids narrow the column tile only while the tiles still fit ONE wave (8192 x 256 x 2304: 24.8 -> 15.5 us)
-    assert plan(8192, 256, 2304)[:2] == (128, 1)          # 64 M tiles x 2 = 128 <= 148; x 4 would be a second wave
-    assert plan(8192, 512, 4608)[:2] == (256, 1)          # 128 tiles already; narrowing would need 256
+    # machine-filling convolution-sized calls: widest tile, no split
+    assert plan(5734400, 256, 6912) == (128, 1, 89600, 0)
+    assert plan(131072, 128, 1152) == (128, 1, 1024, 0)
+    # under-filled grids narrow the column tile only while the tiles still fit ONE wave
+    assert plan(8192, 256, 2304)[:2] == (128, 1)          # 64 M tiles x 2 = 128 <= 132; x 4 would be a second wave
+    assert plan(8192, 512, 4608)[:2] == (128, 1)          # 256 tiles already
     assert plan(1024, 256, 2304)[:2] == (64, 1)
     # short reductions (K = 256: the transformer linears) follow the same one-wave rule
     assert plan(8192, 256, 256)[:2] == (128, 1)
-    assert plan(8192, 512, 256)[:2] == (256, 1)
+    assert plan(4096, 256, 256)[:2] == (64, 1)            # 32 M tiles x 4 = 128 <= 132
     # a reduction is split only into >= 3 ranges of >= 32 chunks (and only with a workspace)
-    assert plan(8192, 256, 4608)[1] == 1                  # two ranges of 36 chunks: lost to the one-pass kernel
+    assert plan(8192, 256, 4608)[1] == 1                  # 128 wide tiles: no room for a second range
     assert plan(1024, 256, 2304)[1] == 1                  # 36 chunks: never
-    assert plan(1400, 512, 13824)[:2] == (256, 6)         # brain-LDM level 1: 22 wide tiles x 6 ranges of 36 chunks
+    assert plan(1400, 512, 13824)[:2] == (128, 3)         # brain-LDM level 1: 44 wide tiles x 3 ranges of 72 chunks
     assert plan(1400, 512, 13824, workspace=False)[1] == 1
-    assert plan(175, 768, 20736)[1] == 10                 # 6 wide tiles, 324 chunks -> 10 ranges of >= 32
+    assert plan(175, 768, 20736)[1] == 10                 # 12 wide tiles, 324 chunks -> 10 ranges of >= 32
     bad = (C.c_int32 * 4)()
-    assert lib.b200_igemm_plan(None, 148, 1, bad) != 0
+    assert lib.b200_igemm_plan(None, 132, 1, bad) != 0

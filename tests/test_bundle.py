@@ -12,7 +12,7 @@ import pytest
 import torch
 
 from oracle import torch_oracle as O
-from tests import cpu_backend
+from tests import cpu_backend, golden
 from tests.golden import configs as G
 
 GOLD = Path(__file__).resolve().parent / "golden"
@@ -25,7 +25,7 @@ def rel(a, b):
 def _bundle_models(device):
     from generativemodels_b200.networks.nets import AutoencoderKL, DiffusionModelUNet
     from generativemodels_b200.networks.schedulers import DDIMScheduler
-    fx = torch.load(GOLD / "g_bundle_brain_ldm.pt", weights_only=False)
+    fx = golden.load("g_bundle_brain_ldm")
     ae = AutoencoderKL(**fx["aekl_kwargs"]).eval()
     unet = DiffusionModelUNet(**fx["unet_kwargs"]).eval()
     ae.load_state_dict(fx["aekl_state"])
@@ -48,7 +48,7 @@ def _oracle_sample(fx):
 # oracle pinned to the reference's own bundle script
 # ------------------------------------------------------------------------------------------------------------------
 def test_oracle_bundle_sampler_matches_reference_fixture():
-    fx = torch.load(GOLD / "g_bundle_brain_ldm.pt", weights_only=False)
+    fx = golden.load("g_bundle_brain_ldm")
     got = _oracle_sample(fx)
     assert got.shape == fx["sample"].shape
     assert rel(got, fx["sample"]) < 1e-5, rel(got, fx["sample"])
@@ -149,11 +149,11 @@ _SMALL_CONFIG = {
 
 def test_bundle_config_runs_reference_syntax_cpu(monkeypatch, tmp_path):
     """Same item graph as the bundle's inference.json (targets in the reference's namespace, ``_requires_`` ordering,
-    ``@`` references inside ``$`` expressions), resolved onto the B200 classes."""
+    ``@`` references inside ``$`` expressions), resolved onto this package's classes."""
     cpu_backend.install(monkeypatch)
     from generativemodels_b200.bundle import BundleConfig, NiftiSaver, Sampler
     from generativemodels_b200.networks.nets import AutoencoderKL
-    fx = torch.load(GOLD / "g_bundle_brain_ldm.pt", weights_only=False)
+    fx = golden.load("g_bundle_brain_ldm")
     cfg = BundleConfig(json.loads(json.dumps(_SMALL_CONFIG)), {"bundle_root": str(tmp_path), "states": "$None"})
     cfg._resolved["states"] = fx                               # tensors cannot come through JSON
     cfg.run("save_nii")
@@ -172,10 +172,9 @@ def test_bundle_config_runs_reference_syntax_cpu(monkeypatch, tmp_path):
 
 
 def test_reference_inference_json_parses_when_present():
-    """The unmodified bundle config (only in the build container) resolves its network definitions on this package."""
-    path = Path("/root/reference/model-zoo/models/brain_image_synthesis_latent_diffusion_model/configs/inference.json")
-    if not path.exists():
-        pytest.skip("reference tree not present")
+    """The unmodified bundle config (the brain-LDM bundle's configs/inference.json, stored verbatim under tests/golden)
+    resolves its network definitions on this package."""
+    path = GOLD / "brain_ldm_inference.json"
     from generativemodels_b200.bundle import BundleConfig, Sampler
     from generativemodels_b200.networks.nets import AutoencoderKL, DiffusionModelUNet
     from generativemodels_b200.networks.schedulers import DDIMScheduler

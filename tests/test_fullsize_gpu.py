@@ -1,7 +1,7 @@
 """Checks at BASELINE.json's FULL sizes (config C3: 160 x 224 x 160, T = 89 600 tokens; config C4: 32 768 vectors),
 where the CPU oracle cannot run: size-independent properties and cross-implementation agreement on the GPU.
 
-* full-resolution 3x3x3 convolution: the tcgen05/TMA kernel against the independent CUDA-core cross-check kernel
+* full-resolution 3x3x3 convolution: the wgmma/TMA kernel against the independent CUDA-core cross-check kernel
   (same bf16 operands, fp32 accumulation) — they share only the parameter block, not the data path;
 * full-length attention (one head of 512, 89 600 keys): the flash kernel against the GEMM + softmax + GEMM path on a
   slab of query rows, plus the invariant that rows of softmax sum to one (constant V gives back the constant);

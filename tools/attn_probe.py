@@ -1,12 +1,8 @@
-"""Dev probe: one full-length attention call (T = S = 89 600, d = 512) for ncu / timing, replay vs recompute."""
+"""Dev probe: one full-length attention call (T = S = 89 600, d = 512), timed with CUDA events."""
 import math, sys
 from pathlib import Path
 sys.path.insert(0, str(Path(__file__).resolve().parents[1]))
-import os
 import torch
-from generativemodels_b200 import _lib
-if os.environ.get("B200_DEV_LIB", ""):            # dev ablation builds of the library (tools only)
-    _lib.LIB_PATH = Path(os.environ["B200_DEV_LIB"]).resolve()
 from generativemodels_b200 import ops
 T = S = 89600
 dh = 512
@@ -14,13 +10,10 @@ torch.manual_seed(0)
 q = (torch.randn(1, T, dh, device="cuda") * 0.5).to(ops.H16)
 k = (torch.randn(1, S, dh, device="cuda") * 0.5).to(ops.H16)
 vt = torch.randn(1, dh, S, device="cuda").to(ops.H16)
-modes = [("replay", True), ("recompute", False)] if len(sys.argv) < 2 else [(sys.argv[1], sys.argv[1] == "replay")]
-for name, flag in modes:
-    ops._FLASH_REPLAY = flag
-    for i in range(6):
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        o = ops.attention(q, k, None, 1, dh, 1 / math.sqrt(dh), vt=vt)
-        e1.record(); torch.cuda.synchronize()
-        ms = e0.elapsed_time(e1)
-        print(f"flash attention [{name}] T=S={T} d={dh}: {ms:.2f} ms, {4*T*S*dh/ms/1e9:.0f} TFLOP/s algorithmic")
+for i in range(6):
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    o = ops.attention(q, k, None, 1, dh, 1 / math.sqrt(dh), vt=vt)
+    e1.record(); torch.cuda.synchronize()
+    ms = e0.elapsed_time(e1)
+    print(f"flash attention T=S={T} d={dh}: {ms:.2f} ms, {4*T*S*dh/ms/1e9:.0f} TFLOP/s algorithmic")
