@@ -48,62 +48,6 @@ static constexpr int kThreads = 128;
 static constexpr int kBM = 64, kBKV = 64;
 static constexpr int kChunkBytes = 64 * 64 * 2;        // 8 KB: 64 rows x 64 channels
 
-__device__ __forceinline__ uint32_t smem_u32(const void* p) {
-  return static_cast<uint32_t>(__cvta_generic_to_shared(p));
-}
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
-}
-__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-  uint32_t done;
-  do {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(done)
-        : "r"(bar), "r"(parity)
-        : "memory");
-  } while (!done);
-}
-// arrive on the barrier at the same shared-memory offset in CTA `cta` of the cluster.  Default (.cta) release
-// semantics: the arrivals only announce that wgmma reads have retired, and a .cluster release would put a GPU-scope
-// memory barrier in front of every one of them
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t bar, uint32_t cta) {
-  uint32_t remote;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(bar), "r"(cta));
-  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(remote) : "memory");
-}
-__device__ __forceinline__ void tma_load_3d(const CUtensorMap* tm, uint32_t bar, uint32_t dst, int c0, int c1, int c2) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4, %5}], [%2];" ::"r"(dst),
-      "l"(reinterpret_cast<uint64_t>(tm)), "r"(bar), "r"(c0), "r"(c1), "r"(c2)
-      : "memory");
-}
-// the box lands at offset dst, and completes its bytes on the barrier at offset bar, in every CTA of cta_mask
-__device__ __forceinline__ void tma_load_3d_multicast(const CUtensorMap* tm, uint32_t bar, uint32_t dst, int c0, int c1,
-                                                      int c2, uint16_t cta_mask) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
-      " [%0], [%1, {%3, %4, %5}], [%2], %6;" ::"r"(dst),
-      "l"(reinterpret_cast<uint64_t>(tm)), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "h"(cta_mask)
-      : "memory");
-}
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void named_sync(uint32_t id, uint32_t threads) {
-  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
-}
 __device__ __forceinline__ float ex2_approx(float x) {
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
@@ -145,11 +89,11 @@ __global__ void __launch_bounds__(kThreads, 1) flash_attn_kernel(const __grid_co
   __syncthreads();
   pdl_wait();
   if (tid == 0) {
-    mbar_expect_tx(q_bar, DCH * kChunkBytes);
+    mbar_arrive_expect_tx(q_bar, DCH * kChunkBytes);
     for (int c = 0; c < DCH; ++c) tma_load_3d(&p.tmQ, q_bar, q_base + c * kChunkBytes, qc + 64 * c, q0, b);
-    mbar_expect_tx(k_bar, DCH * kChunkBytes);
+    mbar_arrive_expect_tx(k_bar, DCH * kChunkBytes);
     for (int c = 0; c < DCH; ++c) tma_load_3d(&p.tmK, k_bar, k_base + c * kChunkBytes, qc + 64 * c, 0, b);
-    mbar_expect_tx(v_bar, DV * kBKV * 2);
+    mbar_arrive_expect_tx(v_bar, DV * kBKV * 2);
     tma_load_3d(&p.tmVt, v_bar, v_base, 0, vc, b);
   }
 
@@ -177,7 +121,7 @@ __global__ void __launch_bounds__(kThreads, 1) flash_attn_kernel(const __grid_co
     wgmma_touch<32>(s);
     __syncthreads();                          // every warp's S is done with the K buffer
     if (tid == 0 && j + 1 < p.n_kv) {
-      mbar_expect_tx(k_bar, DCH * kChunkBytes);
+      mbar_arrive_expect_tx(k_bar, DCH * kChunkBytes);
       for (int c = 0; c < DCH; ++c) tma_load_3d(&p.tmK, k_bar, k_base + c * kChunkBytes, qc + 64 * c, (j + 1) * kBKV, b);
     }
 
@@ -235,7 +179,7 @@ __global__ void __launch_bounds__(kThreads, 1) flash_attn_kernel(const __grid_co
     wgmma_touch<DV / 2>(o);
     __syncthreads();                          // every warp's PV is done with the V^T buffer
     if (tid == 0 && j + 1 < p.n_kv) {
-      mbar_expect_tx(v_bar, DV * kBKV * 2);
+      mbar_arrive_expect_tx(v_bar, DV * kBKV * 2);
       tma_load_3d(&p.tmVt, v_bar, v_base, (j + 1) * kBKV, vc, b);
     }
   }
@@ -337,14 +281,14 @@ __global__ void __launch_bounds__(d512::kThreads, 1) flash_attn_d512_kernel(cons
     // ---------------------------------------------------------------- producer
     setmaxnreg_dec<kProducerRegs>();
     if (tid == 0) {
-      mbar_expect_tx(q_bar, 8 * kChunkBytes);
+      mbar_arrive_expect_tx(q_bar, 8 * kChunkBytes);
       for (int c = 0; c < 8; ++c) tma_load_3d(&p.tmQ, q_bar, q_base + c * kChunkBytes, qc + 64 * c, q0, b);
       for (int j = 0; j < p.n_kv; ++j) {
         for (int n = 0; n < kChunksPerBlock; ++n) {
           const int slot = n % kRing;
           // use 2j + n / 16 of the slot waits for the release of use 2j + n / 16 - 1 (the first wait passes)
           mbar_wait(empty0 + 8 * slot, ((n / kRing) & 1) ^ 1);
-          mbar_expect_tx(full0 + 8 * slot, kChunkBytes);
+          mbar_arrive_expect_tx(full0 + 8 * slot, kChunkBytes);
           if ((n & 1) != (int)rank) continue;
           const uint32_t dst = ring + slot * kChunkBytes, fb = full0 + 8 * slot;
           if (n < 16) {

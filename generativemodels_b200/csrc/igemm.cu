@@ -91,50 +91,12 @@ struct IgemmDev {
 // ------------------------------------------------------------------------------------------------
 // PTX wrappers
 // ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t smem_u32(const void* p) {
-  return static_cast<uint32_t>(__cvta_generic_to_shared(p));
-}
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
-}
-__device__ __forceinline__ void mbar_arrive_expect_tx(uint32_t bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-  uint32_t done;
-  do {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(done)
-        : "r"(bar), "r"(parity)
-        : "memory");
-  } while (!done);
-}
-// role warps (TMA / MMA): one lane polls, the warp re-converges — 32 lanes spinning on the same barrier word only
-// steal issue slots and shared-memory bandwidth from the epilogue / softmax warps
-__device__ __forceinline__ void mbar_wait_warp(uint32_t bar, uint32_t parity) {
-  if ((threadIdx.x & 31) == 0) mbar_wait(bar, parity);
-  __syncwarp();
-}
 __device__ __forceinline__ void tma_load_5d(const CUtensorMap* tm, uint32_t bar, uint32_t dst, int c0,
                                             int c1, int c2, int c3, int c4) {
   asm volatile(
       "cp.async.bulk.tensor.5d.shared::cluster.global.mbarrier::complete_tx::bytes"
       " [%0], [%1, {%3, %4, %5, %6, %7}], [%2];" ::"r"(dst),
       "l"(reinterpret_cast<uint64_t>(tm)), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_3d(const CUtensorMap* tm, uint32_t bar, uint32_t dst, int c0,
-                                            int c1, int c2) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4, %5}], [%2];" ::"r"(dst),
-      "l"(reinterpret_cast<uint64_t>(tm)), "r"(bar), "r"(c0), "r"(c1), "r"(c2)
       : "memory");
 }
 // CH consecutive fp32 accumulator values of one tile row from the shared-memory hand-off tile
@@ -337,26 +299,25 @@ __device__ __forceinline__ void epilogue_fast(const IgemmDev& p, const uint32_t*
 #pragma unroll
       for (int g = 0; g < CH / 8; ++g) *reinterpret_cast<uint4*>(o + g * 8) = pk[g];
     }
-    if constexpr (CH == 32) {
-      if (gs) {   // GroupNorm partials of the values as stored (16-bit-rounded)
-        if (p.gn_sh == 3) {          // one 8-channel group per 16-byte vector: gs[0..3] sums, gs[4..7] sums of squares
+    if (gs) {   // GroupNorm partials of the values as stored (16-bit-rounded)
+      constexpr int G8 = CH / 8, G4 = CH / 4;
+      if (p.gn_sh == 3) {          // one 8-channel group per 16-byte vector: gs[0, G8) sums, gs[G8, 2 G8) sums of squares
 #pragma unroll
-          for (int g = 0; g < 4; ++g) {
-            float f[8];
-            unpack8(pk[g], f);
+        for (int g = 0; g < G8; ++g) {
+          float f[8];
+          unpack8(pk[g], f);
 #pragma unroll
-            for (int j = 0; j < 8; ++j) { gs[g] += f[j]; gs[4 + g] = fmaf(f[j], f[j], gs[4 + g]); }
-          }
-        } else {                     // 4-channel groups (GroupNorm(32) over 128 channels): gs[0..7] sums, gs[8..15] squares
+          for (int j = 0; j < 8; ++j) { gs[g] += f[j]; gs[G8 + g] = fmaf(f[j], f[j], gs[G8 + g]); }
+        }
+      } else {                     // 4-channel groups (GroupNorm(32) over 128 channels): gs[0, G4) sums, gs[G4, 2 G4) squares
 #pragma unroll
-          for (int g = 0; g < 4; ++g) {
-            float f[8];
-            unpack8(pk[g], f);
+        for (int g = 0; g < G8; ++g) {
+          float f[8];
+          unpack8(pk[g], f);
 #pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              gs[2 * g + (j >> 2)] += f[j];
-              gs[8 + 2 * g + (j >> 2)] = fmaf(f[j], f[j], gs[8 + 2 * g + (j >> 2)]);
-            }
+          for (int j = 0; j < 8; ++j) {
+            gs[2 * g + (j >> 2)] += f[j];
+            gs[G4 + 2 * g + (j >> 2)] = fmaf(f[j], f[j], gs[G4 + 2 * g + (j >> 2)]);
           }
         }
       }
@@ -979,6 +940,258 @@ __global__ void __launch_bounds__(kThreads, 1) igemm_tc_kernel(const __grid_cons
 }
 
 // ------------------------------------------------------------------------------------------------
+// The wide kernel: 128 x 256 tiles in clusters of two CTAs that share the weight tile
+// ------------------------------------------------------------------------------------------------
+// 384 threads: warpgroup 0 is the producer (one TMA thread; setmaxnreg hands its registers to the consumers), warpgroups
+// 1 and 2 are consumers, each computing 64 rows x 256 columns with m64n256k16 (128 fp32 accumulators per thread) and
+// running its own epilogue.  A work unit is a pair of adjacent M tiles with one 256-column tile; the two CTAs of a
+// cluster take one M tile each.  Per 64-channel chunk a CTA loads its own 128 x 64 A box and one 128-row half of the
+// 256 x 64 weight tile, multicast to both CTAs: against the 128-column kernel this halves the operand bytes per FLOP
+// that leave L2 and the shared-memory bytes per FLOP that wgmma reads.  A ring slot's empty barrier takes one arrival
+// per consumer warp of BOTH CTAs, because the peer's multicast writes into it.  While the consumers run the epilogue
+// the producer already fills the ring with the next unit's chunks.
+namespace wide {
+static constexpr int kThreads = 384;
+static constexpr int kCluster = 2;
+static constexpr int kBN = 256;
+static constexpr int kStages = 4;
+static constexpr int kBHalfBytes = 128 * kBK * 2;                  // one CTA's share of the weight chunk: 16 KB
+static constexpr int kStageBytes = kABytes + 2 * kBHalfBytes;      // 48 KB
+static constexpr int kSliceLd = 36;                                // padded fp32 row of a 16 x 32 accumulator slice
+static constexpr int kOffSlice = kStages * kStageBytes;            // per consumer warp: [16][kSliceLd] fp32
+static constexpr int kOffAdd = kOffSlice + 8 * 16 * kSliceLd * 4;  // per consumer warp: bias + row vector [kBN] fp32
+static constexpr int kOffBar = kOffAdd + 8 * kBN * 4;              // full[kStages], empty[kStages]
+static constexpr int kSmem = 1024 + kOffBar + 2 * kStages * 8;
+static constexpr int kProducerRegs = 40, kConsumerRegs = 232;
+static_assert(kProducerRegs * 128 + kConsumerRegs * 256 <= 65536, "register budget of one CTA per SM");
+}  // namespace wide
+
+// GroupNorm partials of a 16-column chunk summed over the 16 lanes that share it (lane bits 0..3).  The lane then holds
+// statistic (lane >> 3) & 1 (0 sum, 1 sum of squares) of group (lane >> 2) & 1 of the chunk (8-channel groups: gs[0..1]
+// sums, gs[2..3] squares) or of group 2 ((lane >> 2) & 1) + ((lane >> 1) & 1) (4-channel groups: gs[0..3], gs[4..7]).
+__device__ __forceinline__ float gn_reduce16(const float* gs, int lane, int gn_sh) {
+  const bool h3 = (lane & 8) != 0, h2 = (lane & 4) != 0, h1 = (lane & 2) != 0;
+  if (gn_sh == 3) {
+    float a[2];
+#pragma unroll
+    for (int i = 0; i < 2; ++i) a[i] = (h3 ? gs[2 + i] : gs[i]) + __shfl_xor_sync(0xffffffffu, h3 ? gs[i] : gs[2 + i], 8);
+    float c = (h2 ? a[1] : a[0]) + __shfl_xor_sync(0xffffffffu, h2 ? a[0] : a[1], 4);
+    c += __shfl_xor_sync(0xffffffffu, c, 2);
+    c += __shfl_xor_sync(0xffffffffu, c, 1);
+    return c;
+  }
+  float a4[4], a2[2];
+#pragma unroll
+  for (int i = 0; i < 4; ++i) a4[i] = (h3 ? gs[4 + i] : gs[i]) + __shfl_xor_sync(0xffffffffu, h3 ? gs[i] : gs[4 + i], 8);
+#pragma unroll
+  for (int i = 0; i < 2; ++i) a2[i] = (h2 ? a4[2 + i] : a4[i]) + __shfl_xor_sync(0xffffffffu, h2 ? a4[i] : a4[2 + i], 4);
+  float c = (h1 ? a2[1] : a2[0]) + __shfl_xor_sync(0xffffffffu, h1 ? a2[0] : a2[1], 2);
+  c += __shfl_xor_sync(0xffffffffu, c, 1);
+  return c;
+}
+
+// Calls it takes (see wide_fits): h16 vector-aligned output with cout == out_cols a multiple of 256, h16 vector-aligned
+// residual or none, no softmax statistics / GEGLU / row bias / batched weights / broadcast A / split-K.
+// p.num_tiles is the number of units: ceil(M tiles / 2) x column tiles.
+__global__ void __launch_bounds__(wide::kThreads, 1) igemm_wide_kernel(const __grid_constant__ IgemmDev p) {
+  using namespace wide;
+  if (!p.pdl_late) pdl_launch_dependents();
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* sm = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+  const uint32_t ring = smem_u32(sm);
+  const uint32_t full0 = ring + kOffBar, empty0 = full0 + 8 * kStages;
+
+  const int tid = threadIdx.x;
+  // warp-uniform by construction (broadcast from lane 0): otherwise ptxas treats the role branches as divergent and
+  // serialises every wgmma behind them
+  const int wg = __shfl_sync(0xffffffffu, tid >> 7, 0);
+  const uint32_t rank = cluster_ctarank();
+  const int cid = (int)blockIdx.x / kCluster, n_clusters = (int)gridDim.x / kCluster;
+  const int m_tiles = p.tiles_w * p.tiles_h * p.tiles_d * p.N;
+  const int num_units = p.num_tiles;
+  const int num_k = p.num_k_chunks;
+
+  if (tid == 0) {
+    for (int s = 0; s < kStages; ++s) {
+      mbar_init(full0 + 8 * s, 1);
+      mbar_init(empty0 + 8 * s, 8 * kCluster);     // one arrival per consumer warp of each CTA
+    }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  cluster_sync();                   // both CTAs' barriers exist before any multicast or remote arrival
+  pdl_wait();
+
+  // unit u -> column tile u % tiles_n and M tile 2 (u / tiles_n) + rank (column tile fastest: neighbouring units share
+  // their A halos in L2).  The partner of an odd last M tile loads a valid tile, runs the whole protocol, stores nothing.
+  struct MTile { int nt, wt, ht, dt, nb; bool ok; };
+  auto unit_tile = [&](int u) {
+    MTile t;
+    t.nt = u % p.tiles_n;
+    int m = 2 * (u / p.tiles_n) + (int)rank;
+    t.ok = m < m_tiles;
+    if (!t.ok) m = m_tiles - 1;
+    t.wt = m % p.tiles_w; m /= p.tiles_w;
+    t.ht = m % p.tiles_h; m /= p.tiles_h;
+    t.dt = m % p.tiles_d;
+    t.nb = m / p.tiles_d;
+    return t;
+  };
+
+  if (wg == 0) {
+    // ============================== producer ==============================
+    setmaxnreg_dec<kProducerRegs>();
+    if (tid == 0) {
+      int stage = 0;
+      uint32_t phase = 0;
+      for (int u = cid; u < num_units; u += n_clusters) {
+        const MTile t = unit_tile(u);
+        const int iw0 = t.wt * p.BW * p.sw, ih0 = t.ht * p.BH * p.sh, id0 = t.dt * p.BD * p.sd;
+        const int wrow = t.nt * kBN + 128 * (int)rank;      // this CTA's half of the weight tile
+        int kglob = 0;
+        for (int s = 0; s < p.n_seg; ++s) {
+          const SegDev sg = p.seg[s];
+          const CUtensorMap* tm = &p.tmA[sg.src];
+          const int cw = iw0 + sg.dw, ch = ih0 + sg.dh, cd = id0 + sg.dd;
+          for (int c = 0; c < sg.nchunks; ++c, ++kglob) {
+            mbar_wait(empty0 + 8 * stage, phase ^ 1u);
+            const uint32_t dst = ring + stage * kStageBytes, fb = full0 + 8 * stage;
+            mbar_arrive_expect_tx(fb, kStageBytes);       // own A box + both halves of the weight chunk
+            tma_load_5d(tm, fb, dst, (sg.c0 + c) * kBK, cw, ch, cd, t.nb);
+            tma_load_3d_multicast(&p.tmB, fb, dst + kABytes + rank * kBHalfBytes, kglob * kBK, wrow, 0, 0x3);
+            if (++stage == kStages) { stage = 0; phase ^= 1u; }
+          }
+        }
+      }
+      if (p.pdl_late) pdl_launch_dependents();     // every operand load of this CTA is issued
+    }
+  } else {
+    // ============================== consumers ==============================
+    setmaxnreg_inc<kConsumerRegs>();
+    const int c = wg - 1;                          // rows 64c .. 64c + 63 of the tile
+    const int wq = (tid >> 5) & 3;                 // 16-row slice of those
+    const int lane = tid & 31;
+    float* slice = reinterpret_cast<float*>(sm + kOffSlice) + (4 * c + wq) * 16 * kSliceLd;
+    float* addv = reinterpret_cast<float*>(sm + kOffAdd) + (4 * c + wq) * kBN;
+    // epilogue: the lane owns row (lane & 15) of the warp's 16 rows and columns 16 (lane >> 4) .. + 15 of each
+    // 32-column slice
+    const int er = 64 * c + 16 * wq + (lane & 15);
+    const int eh = lane >> 4;
+    const int rw = er & (p.BW - 1), rh = (er >> p.bw_log2) & (p.BH - 1), rd = er >> (p.bw_log2 + p.bh_log2);
+    auto release = [&](int s) {
+      __syncwarp();
+      if (lane == 0) {
+        mbar_arrive_cluster(empty0 + 8 * s, 0);
+        mbar_arrive_cluster(empty0 + 8 * s, 1);
+      }
+    };
+
+    // GroupNorm partials: gacc[s] is this lane's statistic (see gn_reduce16) of slice s, summed over the units of one
+    // (sample, column tile); on a change it is added to slot gn_slot0 + 4 blockIdx.x + wq — the same slot for warp wq of
+    // both consumers, so consumer 0 adds first and consumer 1 after a barrier (deterministic, no atomics)
+    const bool gn_on = p.gn_partial != nullptr;
+    const int gsh = p.gn_sh;
+    float gacc[kBN / 32];
+#pragma unroll
+    for (int s = 0; s < kBN / 32; ++s) gacc[s] = 0.f;
+    int key = -1, gn_nb = 0, gn_n0 = 0;
+    auto gn_flush = [&]() {
+      const bool writer = (lane & (gsh == 3 ? 3 : 1)) == 0;
+      const int stat = (lane >> 3) & 1;
+      const int gl = gsh == 3 ? (lane >> 2) & 1 : ((lane >> 1) & 3);
+      float* dst = p.gn_partial +
+                   (((long long)gn_nb * p.gn_slots + p.gn_slot0 + 4 * blockIdx.x + wq) * (p.cout >> gsh)) * 2 + stat;
+      for (int pass = 0; pass < 2; ++pass) {
+        if (pass == c && writer) {
+#pragma unroll
+          for (int s = 0; s < kBN / 32; ++s) dst[(((gn_n0 + 32 * s + 16 * eh) >> gsh) + gl) * 2] += gacc[s];
+        }
+        if (pass == 0) named_sync(1, 256);
+      }
+#pragma unroll
+      for (int s = 0; s < kBN / 32; ++s) gacc[s] = 0.f;
+    };
+
+    float acc[kBN / 2];
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int u = cid; u < num_units; u += n_clusters) {
+      int prev = -1;
+      for (int k = 0; k < num_k; ++k) {
+        mbar_wait(full0 + 8 * stage, phase);
+        const uint32_t st = ring + stage * kStageBytes;
+        const uint64_t adesc = wgmma_desc(st + c * (64 * kBK * 2));
+        const uint64_t bdesc = wgmma_desc(st + kABytes);
+        wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < kBK / 16; ++kk)
+          wgmma_ss<kBN>(acc, adesc + 2u * kk, bdesc + 2u * kk, (k | kk) != 0 ? 1u : 0u);
+        wgmma_commit();
+        wgmma_wait<1>();            // the group of the previous chunk has finished reading its stage
+        if (prev >= 0) release(prev);
+        prev = stage;
+        if (++stage == kStages) { stage = 0; phase ^= 1u; }
+      }
+      wgmma_wait<0>();
+      wgmma_touch<kBN / 2>(acc);
+      release(prev);
+
+      // ---- epilogue: the same arithmetic, in the same order, as the 128-column kernel's fast epilogue ----
+      const MTile t = unit_tile(u);
+      const int n0 = t.nt * kBN;
+      const int ow = t.wt * p.BW + rw, oh = t.ht * p.BH + rh, od = t.dt * p.BD + rd;
+      const bool row_ok = t.ok && ow < p.OW && oh < p.OH && od < p.OD;
+      const long long out_off = t.nb * p.out_sN + od * p.out_sD + oh * p.out_sH + ow * p.out_sW;
+      const long long res_off = t.nb * p.res_sN + od * p.res_sD + oh * p.res_sH + ow * p.res_sW;
+      if (t.nb * p.tiles_n + t.nt != key) {
+        if (gn_on && key >= 0) gn_flush();
+        key = t.nb * p.tiles_n + t.nt;
+        gn_nb = t.nb;
+        gn_n0 = n0;
+        // bias + per-sample row vector of this (sample, column tile), shared by all rows
+        float bv[kBN / 32], rv[kBN / 32];
+#pragma unroll
+        for (int i = 0; i < kBN / 32; ++i) {
+          const int col = n0 + lane + 32 * i;
+          bv[i] = p.bias ? __ldg(p.bias + col) : 0.f;
+          rv[i] = p.rowvec ? __ldg(p.rowvec + (long long)t.nb * p.rowvec_bstride + col) : 0.f;
+        }
+        __syncwarp();
+#pragma unroll
+        for (int i = 0; i < kBN / 32; ++i) addv[lane + 32 * i] = bv[i] + rv[i];
+        __syncwarp();
+      }
+      const bool res_on = p.res_ptr && row_ok;
+      uint4 rv_next[2] = {make_uint4(0u, 0u, 0u, 0u), make_uint4(0u, 0u, 0u, 0u)};
+      if (res_on) load_res_fast<16>(p, rv_next, res_off, n0 + 16 * eh);
+#pragma unroll
+      for (int s = 0; s < kBN / 32; ++s) {
+        // the warp's 16 x 32 accumulator slice s through shared memory, so that a lane holds 16 columns of one row
+        __syncwarp();
+#pragma unroll
+        for (int j = 4 * s; j < 4 * s + 4; ++j) {
+          const int col = 8 * (j - 4 * s) + 2 * (lane & 3);
+          *reinterpret_cast<float2*>(slice + (lane >> 2) * kSliceLd + col) = make_float2(acc[4 * j], acc[4 * j + 1]);
+          *reinterpret_cast<float2*>(slice + ((lane >> 2) + 8) * kSliceLd + col) =
+              make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+        }
+        __syncwarp();
+        uint32_t raw[16];
+        acc_ld<16>(slice + (lane & 15) * kSliceLd + 16 * eh, raw);
+        const uint4 rv[2] = {rv_next[0], rv_next[1]};
+        if (res_on && s + 1 < kBN / 32) load_res_fast<16>(p, rv_next, res_off, n0 + 32 * (s + 1) + 16 * eh);
+        const int cc = 32 * s + 16 * eh;
+        // (gs is always passed: a pointer select would keep it in local memory)
+        float gs[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+        if (row_ok) epilogue_fast<16>(p, raw, addv + cc, rv, out_off, n0 + cc, gs);
+        if (gn_on) gacc[s] += gn_reduce16(gs, lane, gsh);
+      }
+    }
+    if (gn_on && key >= 0) gn_flush();
+  }
+  cluster_sync();                   // no CTA leaves while its partner may still multicast into it or arrive on its barriers
+}
+
+// ------------------------------------------------------------------------------------------------
 // CUDA-core cross-check kernel: same parameters, same zero-fill semantics, same epilogue.
 // One thread per (output voxel, 16-column group).  Used by tests and for debugging only.
 // ------------------------------------------------------------------------------------------------
@@ -1166,11 +1379,34 @@ __global__ void __launch_bounds__(256) igemm_split_reduce_kernel(const IgemmDev 
 // Launch geometry shared by b200_igemm and b200_igemm_split_workspace_bytes (host only, no CUDA calls but sm_count()).
 struct Plan {
   TileShape ts;
-  long long m_tiles, ntiles, rows;
+  long long m_tiles, ntiles, rows;   // ntiles: work items of the launch (units of two M tiles for the wide kernel)
   int kchunks, BN, tiles_n;
   int splits, ws_cols;
   long long ws_bytes;
+  bool wide;                         // igemm_wide_kernel (BN = 256)
 };
+
+static int env_impl() {
+  static int v = -1;
+  if (v < 0) {
+    const char* e = getenv("B200_IGEMM_IMPL");
+    v = (e && strcmp(e, "check") == 0) ? 1 : 0;
+  }
+  return v;
+}
+
+// The calls igemm_wide_kernel can compute: its epilogue is the vectorised 16-bit one with every column real.
+static bool wide_fits(const b200_igemm_params* p) {
+  auto v8 = [](long long a, long long b, long long c, long long d) { return a % 8 == 0 && b % 8 == 0 && c % 8 == 0 && d % 8 == 0; };
+  const bool out_vec = v8(p->out_sN, p->out_sD, p->out_sH, p->out_sW) && ((uintptr_t)p->out_ptr % 16) == 0;
+  const bool res_ok = !p->res_ptr || (p->res_dtype == B200_DT_H16 && v8(p->res_sN, p->res_sD, p->res_sH, p->res_sW) &&
+                                      ((uintptr_t)p->res_ptr % 16) == 0);
+  return p->out_dtype == B200_DT_H16 && p->cout == p->out_cols && p->cout % wide::kBN == 0 && out_vec && res_ok &&
+         !p->stat_ptr && p->act1 != B200_ACT_GEGLU && !p->row_bias && !p->w_batched && !p->a_broadcast;
+}
+// Reductions shorter than this many 64-channel chunks stay on the 128-column kernel, whose epilogue overlaps the next
+// tile's main loop (the wide kernel's consumers run their own epilogue).
+static constexpr int kWideMinChunks = 32;
 // dev knobs (read once): the shortest reduction, in 64-element chunks, for which an under-filled grid narrows its
 // column tile within one wave (B200_NARROW_MIN_CHUNKS, default 4), and the fewest ranges a split reduction must have to be worth its
 // fp32 partials + second kernel (B200_SPLIT_MIN, default 3), and the shortest range, in chunks, a split may leave each
@@ -1199,6 +1435,17 @@ static Plan make_plan(const b200_igemm_params* p, bool allow_split, int nsm = 0)
   pl.splits = 1;
   pl.ws_cols = ((p->out_cols + 7) / 8) * 8;
   pl.ws_bytes = 0;
+  // 128 x 256 tiles in clusters of two (impl 3 forces them, impl 2 forbids them): convolutions (>= 8 taps) with a long
+  // reduction whose units fill at least one wave of clusters.  GEMM-shaped calls keep the 128-column kernel.
+  const int impl = p->impl ? p->impl : env_impl();
+  pl.wide = wide_fits(p) && (impl == 3 || (impl == 0 && p->n_seg >= 8 && pl.kchunks >= kWideMinChunks &&
+                                            ((pl.m_tiles + 1) / 2) * (p->cout / wide::kBN) >= nsm / wide::kCluster));
+  if (pl.wide) {
+    pl.BN = wide::kBN;
+    pl.tiles_n = p->cout / wide::kBN;
+    pl.ntiles = ((pl.m_tiles + 1) / 2) * pl.tiles_n;
+    return pl;
+  }
   // N tile: as wide as the output needs, up to 128 columns (the widest tile whose fp32 hand-off buffer and a 4-deep
   // operand ring fit the 227 KB of shared memory a block may use)
   const int cols16 = (((p->act1 == B200_ACT_GEGLU ? p->cout : p->out_cols) + 15) / 16) * 16;   // GEGLU: tile the GEMM's columns
@@ -1253,13 +1500,35 @@ static int launch_tc(const IgemmDev& d, cudaStream_t stream) {
   return B200_OK;
 }
 
-static int env_impl() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("B200_IGEMM_IMPL");
-    v = (e && strcmp(e, "check") == 0) ? 1 : 0;
-  }
-  return v;
+// persistent: at most as many clusters as can be co-resident, each walking units cid, cid + clusters, ...
+static int launch_wide(const IgemmDev& d, cudaStream_t stream) {
+  static_assert(wide::kSmem <= 227 * 1024, "igemm: shared memory over the 227 KB a block may use");
+  static std::once_flag once;
+  static cudaError_t rc = cudaSuccess;
+  static int max_clusters = 0;
+  std::call_once(once, [] {
+    rc = cudaFuncSetAttribute(igemm_wide_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, wide::kSmem);
+    if (rc != cudaSuccess) return;
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(wide::kCluster);
+    cfg.blockDim = dim3(wide::kThreads);
+    cfg.dynamicSmemBytes = wide::kSmem;
+    cudaLaunchAttribute attr;
+    attr.id = cudaLaunchAttributeClusterDimension;
+    attr.val.clusterDim.x = wide::kCluster;
+    attr.val.clusterDim.y = 1;
+    attr.val.clusterDim.z = 1;
+    cfg.attrs = &attr;
+    cfg.numAttrs = 1;
+    rc = cudaOccupancyMaxActiveClusters(&max_clusters, igemm_wide_kernel, &cfg);
+  });
+  B200_CUDA(rc);
+  if (max_clusters < 1) { set_error("igemm: no cluster of igemm_wide_kernel fits on this device"); return B200_ECUDA; }
+  const int clusters = d.num_tiles < max_clusters ? d.num_tiles : max_clusters;
+  B200_CUDA(b200::launch_cluster(igemm_wide_kernel, wide::kCluster, clusters * wide::kCluster, wide::kThreads,
+                                 wide::kSmem, stream, d));
+  B200_LAUNCH_CHECK("igemm_wide_kernel");
+  return B200_OK;
 }
 
 }  // namespace b200
@@ -1275,8 +1544,8 @@ extern "C" int64_t b200_igemm_split_workspace_bytes(const b200_igemm_params* p) 
 }
 
 // Host-only planning query (no CUDA call): the column tile, the split factor and the tile count b200_igemm would use
-// for this call on a GPU with `sm_count` SMs — lets the binding layer's CPU tests pin the planner's rules.  out[3] is
-// always 0 (reserved: the kernel has a single-CTA variant only).
+// for this call on a GPU with `sm_count` SMs — lets the binding layer's CPU tests pin the planner's rules.  For calls
+// of the wide kernel out[0] is 256 and out[2] the number of units (pairs of M tiles x column tiles).  out[3] is always 0.
 extern "C" int b200_igemm_plan(const b200_igemm_params* p, int32_t sm_count_, int32_t with_workspace, int32_t out[4]) {
   if (!p || !out || sm_count_ < 1 || p->n_seg < 1 || p->n_seg > B200_IGEMM_MAX_SEG || p->out_N < 1 || p->out_D < 1 ||
       p->out_H < 1 || p->out_W < 1 || p->out_cols < 1)
@@ -1394,6 +1663,11 @@ extern "C" int b200_igemm(const b200_igemm_params* p, void* stream_v) {
   }
 
   const int impl = p->impl ? p->impl : env_impl();
+  B200_CHECK_ARG(impl >= 0 && impl <= 3, "igemm: impl %d not in 0..3", impl);
+  B200_CHECK_ARG(impl != 3 || wide_fits(p),
+                 "igemm: impl 3 (128 x 256 tiles) needs a vector-aligned h16 output with cout == out_cols a multiple of "
+                 "256, a vector-aligned h16 residual or none, and no stat_ptr / GEGLU / row_bias / batched weights / "
+                 "broadcast A");
   if (impl == 1) {
     const long long rows = (long long)d.N * d.OD * d.OH * d.OW;
     const long long total = rows * ((d.out_cols + 15) / 16);
@@ -1460,7 +1734,8 @@ extern "C" int b200_igemm(const b200_igemm_params* p, void* stream_v) {
     cuuint64_t bs = p->w_bstride ? (cuuint64_t)p->w_bstride * 2 : (cuuint64_t)p->w_rows * p->w_pitch * 2;
     cuuint64_t strides[2] = {(cuuint64_t)p->w_pitch * 2, bs};
     B200_CHECK_ARG(bs % 16 == 0, "igemm: weight batch stride not 16-byte aligned");
-    cuuint32_t box[3] = {(cuuint32_t)kBK, (cuuint32_t)BN, 1};
+    // the wide kernel loads its 256-row weight tile as two 128-row halves, one per CTA of the cluster
+    cuuint32_t box[3] = {(cuuint32_t)kBK, (cuuint32_t)(pl.wide ? 128 : BN), 1};
     cuuint32_t estr[3] = {1, 1, 1};
     CUresult r = g_encode(&d.tmB, B200_H16_TMAP, 3, const_cast<void*>(p->w_ptr), dims,
                           strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
@@ -1472,6 +1747,7 @@ extern "C" int b200_igemm(const b200_igemm_params* p, void* stream_v) {
     }
   }
 
+  if (pl.wide) return launch_wide(d, stream);
   auto launch = [&](const IgemmDev& dev) {
     switch (BN) {
       case 16:  return launch_tc<16, 8>(dev, stream);

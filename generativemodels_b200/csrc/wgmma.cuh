@@ -5,8 +5,10 @@
 // advances the descriptor's start address by 32 bytes.  Accumulators are fp32 registers of the issuing warpgroup:
 // for m64nN, thread t (warp w = t / 32 of the warpgroup, lane l) holds d[4j + {0,1,2,3}] = rows 16w + l/4 (+8 for
 // {2,3}), columns 8j + 2 (l % 4) (+1 for {1,3}).
+// Also the mbarrier / TMA / cluster PTX wrappers both files' warp-specialised kernels use.
 #pragma once
 #include "common.cuh"
+#include <cuda.h>
 
 #ifdef B200_H16_IS_BF16
 #define B200_WGMMA_AB "bf16"
@@ -148,6 +150,69 @@ __device__ __forceinline__ void wgmma_rs(float* d, const uint32_t* a, uint64_t b
   if constexpr (N == 64) wgmma_rs_n64(d, a, bdesc, accumulate);
   else if constexpr (N == 128) wgmma_rs_n128(d, a, bdesc, accumulate);
   else wgmma_rs_n256(d, a, bdesc, accumulate);
+}
+
+// ------------------------------------------------------------------------------------------------
+// mbarrier, TMA and cluster helpers of the warp-specialised kernels
+// ------------------------------------------------------------------------------------------------
+__device__ __forceinline__ uint32_t smem_u32(const void* p) {
+  return static_cast<uint32_t>(__cvta_generic_to_shared(p));
+}
+__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
+  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
+}
+__device__ __forceinline__ void mbar_arrive_expect_tx(uint32_t bar, uint32_t bytes) {
+  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
+}
+__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
+  uint32_t done;
+  do {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
+        "selp.u32 %0, 1, 0, p;\n\t}"
+        : "=r"(done)
+        : "r"(bar), "r"(parity)
+        : "memory");
+  } while (!done);
+}
+// arrive on the barrier at the same shared-memory offset in CTA `cta` of the cluster.  Default (.cta) release
+// semantics: the arrivals only announce that wgmma reads have retired, and a .cluster release would put a GPU-scope
+// memory barrier in front of every one of them
+__device__ __forceinline__ void mbar_arrive_cluster(uint32_t bar, uint32_t cta) {
+  uint32_t remote;
+  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(bar), "r"(cta));
+  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(remote) : "memory");
+}
+__device__ __forceinline__ void tma_load_3d(const CUtensorMap* tm, uint32_t bar, uint32_t dst, int c0, int c1, int c2) {
+  asm volatile(
+      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes"
+      " [%0], [%1, {%3, %4, %5}], [%2];" ::"r"(dst),
+      "l"(reinterpret_cast<uint64_t>(tm)), "r"(bar), "r"(c0), "r"(c1), "r"(c2)
+      : "memory");
+}
+// the box lands at offset dst, and completes its bytes on the barrier at offset bar, in every CTA of cta_mask
+__device__ __forceinline__ void tma_load_3d_multicast(const CUtensorMap* tm, uint32_t bar, uint32_t dst, int c0, int c1,
+                                                      int c2, uint16_t cta_mask) {
+  asm volatile(
+      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
+      " [%0], [%1, {%3, %4, %5}], [%2], %6;" ::"r"(dst),
+      "l"(reinterpret_cast<uint64_t>(tm)), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "h"(cta_mask)
+      : "memory");
+}
+__device__ __forceinline__ uint32_t cluster_ctarank() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+  return r;
+}
+__device__ __forceinline__ void cluster_sync() {
+  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
+}
+__device__ __forceinline__ void named_sync(uint32_t id, uint32_t threads) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
 }
 
 }  // namespace b200

@@ -123,7 +123,9 @@ typedef struct {
   int32_t act2;
   float*  stat_ptr;     /* optional softmax partials: [out_W][ceil(out_cols/128)][2] = (max, sum exp(v - max)) of every
                            128-column tile of every output row (GEMM-shaped calls only); NULL to skip            */
-  int32_t impl;         /* 0 = wgmma kernel, 1 = CUDA-core cross-check kernel    */
+  int32_t impl;         /* 0 = wgmma kernels (the planner picks one), 1 = CUDA-core cross-check kernel,
+                           2 = the 128-column wgmma kernel only, 3 = the 128 x 256 two-CTA wgmma kernel
+                           (B200_EINVAL for a call outside its envelope)                               */
   /* Optional GroupNorm partial sums for whoever normalises this output next (nn.GroupNorm after every conv of the
    * ResnetBlock, diffusion_model_unet.py:623-684): gn_partial[n][slot][cout/8][2] += (sum, sum of squares) of the
    * stored h16 values per 8-channel group; the kernel uses slots [gn_slot0, gn_slot0 + 4 * SM count) of the
@@ -158,8 +160,10 @@ typedef struct {
 
 int b200_igemm(const b200_igemm_params* p, void* stream);
 /* Host-only planning query, no CUDA call: what b200_igemm would choose for this call on a GPU with sm_count SMs —
- * out = {column tile (16..128), split factor (1 = one pass; > 1 only if with_workspace), output tiles, 0 (reserved)}.
- * The rules (DESIGN.md section 2): an under-filled grid narrows its column tile while
+ * out = {column tile (16..256), split factor (1 = one pass; > 1 only if with_workspace), work items, 0 (reserved)}.
+ * The rules (DESIGN.md section 2): a convolution of >= 8 taps with a long reduction, 16-bit output and cout a multiple
+ * of 256 whose units fill one wave of two-CTA clusters takes the 256-column kernel (work items = units of two M tiles);
+ * otherwise an under-filled grid narrows its column tile while
  * the tiles still fit one wave; a reduction is split only into >= 3 ranges of >= 32 chunks of 64. */
 int b200_igemm_plan(const b200_igemm_params* p, int32_t sm_count, int32_t with_workspace, int32_t out[4]);
 /* Bytes of split_ws with which b200_igemm would split the reduction of this call; 0 when it would not (enough tiles
