@@ -1568,11 +1568,11 @@ extern "C" int b200_igemm(const b200_igemm_params* p, void* stream_v) {
   const bool geglu = p->act1 == B200_ACT_GEGLU;
   B200_CHECK_ARG(p->cout >= 1 && p->out_cols >= (geglu ? p->cout / 2 : p->cout), "igemm: bad cout/out_cols");
   if (geglu) {
-    B200_CHECK_ARG(p->cout % 64 == 0 && p->out_dtype == B200_DT_H16 && !p->res_ptr && p->scale == 1.0f &&
-                   p->act2 == B200_ACT_NONE && !p->stat_ptr && !p->gn_partial && !p->row_bias && p->impl != 1 &&
-                   env_impl() != 1,
-                   "igemm: B200_ACT_GEGLU needs cout %% 64 == 0, a h16 output and no residual / scale / act2 / "
-                   "statistics / row bias (and has no cross-check kernel)");
+    B200_CHECK_ARG(p->cout % 64 == 0 && p->out_cols == p->cout / 2 && p->out_dtype == B200_DT_H16 && !p->res_ptr &&
+                   p->scale == 1.0f && p->act2 == B200_ACT_NONE && !p->stat_ptr && !p->gn_partial && !p->row_bias &&
+                   p->impl != 1 && env_impl() != 1,
+                   "igemm: B200_ACT_GEGLU needs cout %% 64 == 0, out_cols == cout / 2, a h16 output and no residual / "
+                   "scale / act2 / statistics / row bias (and has no cross-check kernel)");
   }
   B200_CHECK_ARG(p->w_pitch % 8 == 0 && p->w_rows >= 1, "igemm: weight pitch must be a multiple of 8");
   B200_CHECK_ARG(((uintptr_t)p->w_ptr & 15) == 0, "igemm: weight pointer not 16-byte aligned");
@@ -1664,6 +1664,7 @@ extern "C" int b200_igemm(const b200_igemm_params* p, void* stream_v) {
 
   const int impl = p->impl ? p->impl : env_impl();
   B200_CHECK_ARG(impl >= 0 && impl <= 3, "igemm: impl %d not in 0..3", impl);
+  B200_CHECK_ARG(impl != 1 || !p->stat_ptr, "igemm: stat_ptr has no cross-check kernel (impl 1)");
   B200_CHECK_ARG(impl != 3 || wide_fits(p),
                  "igemm: impl 3 (128 x 256 tiles) needs a vector-aligned h16 output with cout == out_cols a multiple of "
                  "256, a vector-aligned h16 residual or none, and no stat_ptr / GEGLU / row_bias / batched weights / "

@@ -46,8 +46,8 @@ extern "C" {
  * diffusion_model_unet.py:211: linear1 -> a * gelu(gate) with a, gate = chunk(2, -1)) fused into linear1's epilogue.
  * The GEMM's `cout` columns come in 64-column groups [32 x a | 32 x gate] (the caller interleaves the weight rows and
  * the bias that way); output channel (col / 64) * 32 + col % 32 = (acc_a + bias_a) * gelu(acc_gate + bias_gate), so
- * the stored row has cout / 2 channels (out_cols >= cout / 2).  Needs cout % 64 == 0, a h16 16-byte-aligned output,
- * no residual / scale / act2 / statistics / split. */
+ * the stored row has cout / 2 channels and no padding columns (out_cols == cout / 2).  Needs cout % 64 == 0, a h16
+ * 16-byte-aligned output, no residual / scale / act2 / statistics / split. */
 #define B200_ACT_GEGLU 7
 
 #define B200_IGEMM_MAX_SEG 128
@@ -121,8 +121,11 @@ typedef struct {
   int32_t res_dtype;
   int64_t res_sN, res_sD, res_sH, res_sW;
   int32_t act2;
-  float*  stat_ptr;     /* optional softmax partials: [out_W][ceil(out_cols/128)][2] = (max, sum exp(v - max)) of every
-                           128-column tile of every output row (GEMM-shaped calls only); NULL to skip            */
+  float*  stat_ptr;     /* optional softmax partials: [out_W][ceil(out_cols/128)][2] = (max, sum exp(v - max)) over the
+                           columns < cout of every 128-column tile of every output row, v = the fp32 value of `out`
+                           above (after the residual and act2, before any 16-bit rounding); (-inf, 0) for a tile
+                           with no such column.  GEMM-shaped calls only (out_N == out_D == out_H == 1), not with
+                           impl = 1; NULL to skip                                                          */
   int32_t impl;         /* 0 = wgmma kernels (the planner picks one), 1 = CUDA-core cross-check kernel,
                            2 = the 128-column wgmma kernel only, 3 = the 128 x 256 two-CTA wgmma kernel
                            (B200_EINVAL for a call outside its envelope)                               */

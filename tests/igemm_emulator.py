@@ -49,8 +49,8 @@ def _act(x, a):
     if a == ACT_SIGMOID:
         return (1 / (1 + np.exp(-x))).astype(np.float32)
     if a == ACT_GELU:
-        from math import erf
-        return (0.5 * x * (1.0 + np.vectorize(erf)(x * 0.7071067811865476))).astype(np.float32)
+        from scipy.special import erf      # float64 erf of the float32 argument, as math.erf would give
+        return (0.5 * x * (1.0 + erf(np.asarray(x * 0.7071067811865476).astype(np.float64)))).astype(np.float32)
     return x
 
 
@@ -73,7 +73,7 @@ def emulate(p: IgemmParams) -> None:
     OD, OH, OW = p.out_D, p.out_H, p.out_W
     geglu = p.act1 == ACT_GEGLU          # [32 a | 32 gate] column groups of the GEMM -> a * gelu(gate), cout / 2 channels
     if geglu:
-        assert p.cout % 64 == 0 and p.out_cols >= p.cout // 2 and not p.res_ptr and p.scale == 1.0 and not p.row_bias
+        assert p.cout % 64 == 0 and p.out_cols == p.cout // 2 and not p.res_ptr and p.scale == 1.0 and not p.row_bias
     cols = p.cout if geglu else p.out_cols
     acc = np.zeros((N, OD, OH, OW, cols), dtype=np.float64)
     od = np.arange(OD)[:, None, None]
@@ -127,18 +127,6 @@ def emulate(p: IgemmParams) -> None:
         valid = col < H
     else:
         v = _act(v, p.act1) * np.float32(p.scale)
-    if p.stat_ptr:       # softmax partials per 128-column tile (GEMM-shaped calls): (max, sum exp(v - max))
-        nt = (cols + 127) // 128
-        st = _f32_view(p.stat_ptr, OW * nt * 2).reshape(OW, nt, 2)
-        rows2d = v.reshape(OW, cols)
-        for t in range(nt):
-            seg = rows2d[:, t * 128:min((t + 1) * 128, p.cout)]
-            if seg.shape[1] == 0:
-                st[:, t, 0], st[:, t, 1] = -np.inf, 0.0
-                continue
-            mx = seg.max(1)
-            st[:, t, 0] = mx
-            st[:, t, 1] = np.exp(seg - mx[:, None]).sum(1)
 
     def strided_index(sN, sD, sH, sW):
         n = np.arange(N)[:, None, None, None, None]
@@ -153,6 +141,19 @@ def emulate(p: IgemmParams) -> None:
             r = _f32_view(p.res_ptr, int(idx.max()) + 1)[idx]
         v = v + r
     v = _act(v, p.act2)
+    if p.stat_ptr:       # softmax partials per 128-column tile (GEMM-shaped calls) of the fp32 output: (max, sum exp(v - max))
+        assert N == OD == OH == 1
+        nt = (cols + 127) // 128
+        st = _f32_view(p.stat_ptr, OW * nt * 2).reshape(OW, nt, 2)
+        rows2d = v.reshape(OW, cols)
+        for t in range(nt):
+            seg = rows2d[:, t * 128:min((t + 1) * 128, p.cout)]
+            if seg.shape[1] == 0:
+                st[:, t, 0], st[:, t, 1] = -np.inf, 0.0
+                continue
+            mx = seg.max(1)
+            st[:, t, 0] = mx
+            st[:, t, 1] = np.exp(seg - mx[:, None]).sum(1)
     v[..., ~valid] = 0
     idx = strided_index(p.out_sN, p.out_sD, p.out_sH, p.out_sW)
     if p.out_dtype == DT_H16:

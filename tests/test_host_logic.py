@@ -1,7 +1,8 @@
 """CPU tests of the host-side logic in generativemodels_b200.ops: weight packing, tap tables, asymmetric padding,
 stride, transposed-conv phases, virtual concat, GEMM/attention parameter blocks.  The C-ABI call is replaced by
 tests/igemm_emulator.py (a literal reading of include/b200gen.h), so what is verified here is exactly the struct the
-GPU kernel receives.  Kernel arithmetic itself is covered by the -m gpu tests."""
+GPU kernel receives.  That the kernels compute what the emulator computes, on every store path and kernel of b200_igemm,
+is checked on the GPU by tests/test_igemm_contract_gpu.py."""
 import math
 
 import pytest
