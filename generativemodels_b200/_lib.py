@@ -27,6 +27,8 @@ DT_H16, DT_F32 = 0, 1
 H16_FP16, H16_BF16 = 0, 1
 ACT_NONE, ACT_RELU, ACT_SILU, ACT_LEAKYRELU, ACT_GELU, ACT_TANH, ACT_SIGMOID = 0, 1, 2, 3, 4, 5, 6
 ACT_GEGLU = 7        # b200_igemm act1 only: [32 a | 32 gate] column groups -> a * gelu(gate), half as many output channels
+ACT_LEAKYRELU02 = 8  # nn.LeakyReLU(0.2)
+INTERP_BILINEAR, INTERP_BICUBIC = 0, 1
 PRED_EPSILON, PRED_SAMPLE, PRED_V = 0, 1, 2
 IGEMM_MAX_SEG = 128
 IGEMM_SPLIT_COUNTERS = 256
@@ -139,6 +141,7 @@ SIGNATURES = {
     "b200_nchw_to_nhwc": [_P, _I32, _I32, _I64, _P, _I32, _P],
     "b200_nhwc_to_nchw": [_P, _I32, _I32, _I32, _I64, _I32, _P, _P],
     "b200_upsample_nearest2x": [_P, _I32, _I32, _I32, _I32, _I32, _I32, _P, _P],
+    "b200_upsample2x_interp": [_P, _I32, _I32, _I32, _I32, _I32, _P, _P],
     "b200_avgpool2": [_P, _I32, _I32, _I32, _I32, _I32, _I32, _P, _P],
     "b200_axpy_h16": [_P, _P, _F, _P, _I64, _P],
     "b200_copy_channels": [_P, _I32, _I32, _P, _I32, _I32, _I64, _P],
@@ -166,6 +169,7 @@ SIGNATURES = {
     "b200_ddpm_kl": [_P, _P, _P, C.POINTER(KlCoef), _P, _P, _I32, _I64, _P],
     "b200_pndm_step": [C.POINTER(_P), _P, C.POINTER(PndmCoef), _P, _P, _I64, _P],
     "b200_exp_half_clamped": [_P, _F, _F, _P, _I64, _P],
+    "b200_vae_reparam_kld": [_P, _P, _P, _P, _P, _I64, _P],
     "b200_scale_f32": [_P, _F, _F, _P, _I64, _P],
     "b200_fma_f32": [_P, _P, _P, _P, _I64, _P],
     "b200_add_noise": [_P, _P, _P, _P, _F, _I32, _I64, _P, _P],

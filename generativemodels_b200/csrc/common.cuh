@@ -107,6 +107,7 @@ __device__ __forceinline__ float apply_act(float x, int act) {
   if (act == B200_ACT_RELU) return fmaxf(x, 0.0f);
   if (act == B200_ACT_SILU) return silu_f(x);
   if (act == B200_ACT_LEAKYRELU) return x > 0.0f ? x : 0.01f * x;
+  if (act == B200_ACT_LEAKYRELU02) return x > 0.0f ? x : 0.2f * x;
   if (act == B200_ACT_GELU) return 0.5f * x * (1.0f + erff(x * 0.70710678118654752f));
   if (act == B200_ACT_TANH) return tanhf(x);
   if (act == B200_ACT_SIGMOID) return 1.0f / (1.0f + __expf(-x));

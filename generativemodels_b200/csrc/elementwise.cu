@@ -80,6 +80,79 @@ __global__ void upsample2x_kernel(const uint4* __restrict__ x, int N, int D, int
   }
 }
 
+// ------------------------------------------------------------------------------------------------
+// x2 bilinear / bicubic upsample of a 2-D channels-last tensor (align_corners=False); one thread per (output pixel,
+// 8 channels).  Output o = 2i + parity reads source coordinate s = i - 0.25 (even) or i + 0.25 (odd), so each axis has
+// two sets of taps and weights, picked by parity.
+// ------------------------------------------------------------------------------------------------
+// bilinear: s clamped at 0 (only the first even output is affected: it copies row 0)
+__device__ __forceinline__ void interp_taps_linear(int o, int n, int* idx, float* w) {
+  const int i = o >> 1;
+  if (o & 1)       { idx[0] = i;     idx[1] = min(i + 1, n - 1); w[0] = 0.75f; w[1] = 0.25f; }
+  else if (i == 0) { idx[0] = 0;     idx[1] = 0;                 w[0] = 1.0f;  w[1] = 0.0f;  }
+  else             { idx[0] = i - 1; idx[1] = i;                 w[0] = 0.25f; w[1] = 0.75f; }
+}
+// bicubic: upsample_bicubic2d's cubic convolution (A = -0.75) at fraction t = 0.75 (even) or 0.25 (odd), taps
+// floor(s) - 1 .. floor(s) + 2 clamped to the border
+__device__ __forceinline__ void interp_taps_cubic(int o, int n, int* idx, float* w) {
+  const float A = -0.75f;
+  const int f = (o & 1) ? (o >> 1) : (o >> 1) - 1;
+  const float t = (o & 1) ? 0.25f : 0.75f;
+  const float x0 = t + 1.0f, x1 = t, x2 = 1.0f - t, x3 = 2.0f - t;
+  w[0] = ((A * x0 - 5.0f * A) * x0 + 8.0f * A) * x0 - 4.0f * A;
+  w[1] = ((A + 2.0f) * x1 - (A + 3.0f)) * x1 * x1 + 1.0f;
+  w[2] = ((A + 2.0f) * x2 - (A + 3.0f)) * x2 * x2 + 1.0f;
+  w[3] = ((A * x3 - 5.0f * A) * x3 + 8.0f * A) * x3 - 4.0f * A;
+#pragma unroll
+  for (int k = 0; k < 4; ++k) idx[k] = min(max(f - 1 + k, 0), n - 1);
+}
+
+template <int MODE>
+__global__ void upsample2x_interp_kernel(const uint4* __restrict__ x, int N, int H, int W, int pv,
+                                         uint4* __restrict__ y) {
+  pdl_entry();
+  constexpr int T = MODE == B200_INTERP_BICUBIC ? 4 : 2;
+  const int OH = 2 * H, OW = 2 * W;
+  const long long total = (long long)N * OH * OW * pv;
+  for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < total;
+       idx += (long long)gridDim.x * blockDim.x) {
+    long long t = idx;
+    const int v = (int)(t % pv); t /= pv;
+    const int ow = (int)(t % OW); t /= OW;
+    const int oh = (int)(t % OH); t /= OH;
+    const int n = (int)t;
+    int hi[T], wi[T];
+    float hw[T], ww[T];
+    if constexpr (MODE == B200_INTERP_BICUBIC) {
+      interp_taps_cubic(oh, H, hi, hw);
+      interp_taps_cubic(ow, W, wi, ww);
+    } else {
+      interp_taps_linear(oh, H, hi, hw);
+      interp_taps_linear(ow, W, wi, ww);
+    }
+    const uint4* img = x + (long long)n * H * W * pv + v;
+    float out[8];
+#pragma unroll
+    for (int c = 0; c < 8; ++c) out[c] = 0.f;
+#pragma unroll
+    for (int a = 0; a < T; ++a) {            // interpolate along W within each source row, then along H
+      float row[8];
+#pragma unroll
+      for (int c = 0; c < 8; ++c) row[c] = 0.f;
+#pragma unroll
+      for (int b = 0; b < T; ++b) {
+        float f[8];
+        unpack8(__ldg(img + ((long long)hi[a] * W + wi[b]) * pv), f);
+#pragma unroll
+        for (int c = 0; c < 8; ++c) row[c] = fmaf(f[c], ww[b], row[c]);
+      }
+#pragma unroll
+      for (int c = 0; c < 8; ++c) out[c] = fmaf(row[c], hw[a], out[c]);
+    }
+    y[idx] = pack8(out);
+  }
+}
+
 __global__ void avgpool2_kernel(const uint4* __restrict__ x, int N, int D, int H, int W, int pv, int dims,
                                 uint4* __restrict__ y) {
   pdl_entry();
@@ -520,6 +593,30 @@ __global__ void fma_f32_kernel(const float* __restrict__ a, const float* __restr
     y[i] = a[i] + b[i] * c[i];
 }
 
+// one CTA: z elementwise, the KL sum in fp64 in a fixed order (strided per thread, then a fixed shuffle / shared tree)
+__global__ void __launch_bounds__(256) vae_reparam_kld_kernel(const float* __restrict__ mu,
+                                                              const float* __restrict__ logvar,
+                                                              const float* __restrict__ eps, float* __restrict__ z,
+                                                              float* __restrict__ kld, long long n) {
+  pdl_entry();
+  double s = 0.0;
+  for (long long i = threadIdx.x; i < n; i += blockDim.x) {
+    const float m = mu[i], lv = logvar[i];
+    z[i] = fmaf(eps[i], expf(0.5f * lv), m);
+    s += 1.0 + (double)lv - (double)m * (double)m - exp((double)lv);
+  }
+  for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+  __shared__ double red[8];
+  const int w = threadIdx.x >> 5, l = threadIdx.x & 31;
+  if (l == 0) red[w] = s;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double t = 0.0;
+    for (int k = 0; k < (int)(blockDim.x >> 5); ++k) t += red[k];
+    kld[0] = (float)(-0.5 * t);
+  }
+}
+
 __global__ void scale_f32_kernel(const float* __restrict__ x, float mul, float div, float* __restrict__ y, long long n) {
   pdl_entry();
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
@@ -677,6 +774,32 @@ extern "C" int b200_upsample_nearest2x(const void* x, int32_t N, int32_t D, int3
   B200_CUDA(b200::launch_pdl(upsample2x_kernel, grid_for(total), 256, 0, stream, reinterpret_cast<const uint4*>(x), N, D, H, W, pitch / 8, dims,
                                                         reinterpret_cast<uint4*>(y)));
   B200_LAUNCH_CHECK("upsample2x_kernel");
+  return B200_OK;
+}
+
+extern "C" int b200_upsample2x_interp(const void* x, int32_t N, int32_t H, int32_t W, int32_t pitch, int32_t mode,
+                                      void* y, void* stream_v) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
+  B200_CHECK_ARG(x && y && N >= 1 && H >= 1 && W >= 1 && pitch >= 8 && pitch % 8 == 0 &&
+                 (uintptr_t)x % 16 == 0 && (uintptr_t)y % 16 == 0, "upsample2x_interp: bad arguments");
+  B200_CHECK_ARG(mode == B200_INTERP_BILINEAR || mode == B200_INTERP_BICUBIC, "upsample2x_interp: unknown mode %d", mode);
+  const long long total = (long long)N * 2 * H * 2 * W * (pitch / 8);
+  if (mode == B200_INTERP_BICUBIC)
+    B200_CUDA(b200::launch_pdl(upsample2x_interp_kernel<B200_INTERP_BICUBIC>, grid_for(total), 256, 0, stream,
+                               reinterpret_cast<const uint4*>(x), N, H, W, pitch / 8, reinterpret_cast<uint4*>(y)));
+  else
+    B200_CUDA(b200::launch_pdl(upsample2x_interp_kernel<B200_INTERP_BILINEAR>, grid_for(total), 256, 0, stream,
+                               reinterpret_cast<const uint4*>(x), N, H, W, pitch / 8, reinterpret_cast<uint4*>(y)));
+  B200_LAUNCH_CHECK("upsample2x_interp_kernel");
+  return B200_OK;
+}
+
+extern "C" int b200_vae_reparam_kld(const float* mu, const float* logvar, const float* eps, float* z, float* kld,
+                                    int64_t n, void* stream_v) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
+  B200_CHECK_ARG(mu && logvar && eps && z && kld && n >= 1, "vae_reparam_kld: bad arguments");
+  B200_CUDA(b200::launch_pdl(vae_reparam_kld_kernel, 1, 256, 0, stream, mu, logvar, eps, z, kld, (long long)n));
+  B200_LAUNCH_CHECK("vae_reparam_kld_kernel");
   return B200_OK;
 }
 

@@ -234,9 +234,10 @@ __device__ __forceinline__ void act_inplace(float* v, int act) {
   if (act == B200_ACT_SILU) {
 #pragma unroll
     for (int j = 0; j < CH; ++j) v[j] = silu_f(v[j]);
-  } else if (act == B200_ACT_LEAKYRELU) {
+  } else if (act == B200_ACT_LEAKYRELU || act == B200_ACT_LEAKYRELU02) {
+    const float slope = act == B200_ACT_LEAKYRELU ? 0.01f : 0.2f;
 #pragma unroll
-    for (int j = 0; j < CH; ++j) v[j] = v[j] > 0.0f ? v[j] : 0.01f * v[j];
+    for (int j = 0; j < CH; ++j) v[j] = v[j] > 0.0f ? v[j] : slope * v[j];
   } else if (act == B200_ACT_GELU) {
 #pragma unroll
     for (int j = 0; j < CH; ++j) v[j] = 0.5f * v[j] * (1.0f + erff(v[j] * 0.70710678118654752f));

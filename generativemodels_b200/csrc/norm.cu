@@ -222,6 +222,16 @@ __device__ __forceinline__ float silu_fast(float x) {
   // costs ~10 ALU instructions per element and made this HBM-bound pass instruction-bound.
   return __fdividef(x, 1.0f + __expf(-x));
 }
+// the activations the GroupNorm apply passes take: none, SiLU, LeakyReLU(0.01), LeakyReLU(0.2)
+__device__ __forceinline__ float gn_act(float t, int act) {
+  if (act == B200_ACT_SILU) return silu_fast(t);
+  if (act == B200_ACT_LEAKYRELU) return t > 0.0f ? t : 0.01f * t;
+  if (act == B200_ACT_LEAKYRELU02) return t > 0.0f ? t : 0.2f * t;
+  return t;
+}
+__host__ __forceinline__ bool gn_act_ok(int act) {
+  return act == B200_ACT_NONE || act == B200_ACT_SILU || act == B200_ACT_LEAKYRELU || act == B200_ACT_LEAKYRELU02;
+}
 
 template <int VEC>
 __global__ void gn_apply_kernel(const h16* __restrict__ x0, const h16* __restrict__ x1,
@@ -265,7 +275,7 @@ __global__ void gn_apply_kernel(const h16* __restrict__ x0, const h16* __restric
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
           const float t = fmaf(f[j], a[j], b[j]);
-          f[j] = (act == B200_ACT_SILU) ? silu_fast(t) : t;
+          f[j] = gn_act(t, act);
         }
         *reinterpret_cast<uint4*>(dst + (s + (long long)u * rows) * y_pitch) = pack8(f);
       }
@@ -282,7 +292,7 @@ __global__ void gn_apply_kernel(const h16* __restrict__ x0, const h16* __restric
 #pragma unroll
     for (int j = 0; j < VEC; ++j) {
       const float t = fmaf(f[j], a[j], b[j]);
-      f[j] = (act == B200_ACT_SILU) ? silu_fast(t) : t;
+      f[j] = gn_act(t, act);
     }
     if constexpr (VEC == 8) {
       *reinterpret_cast<uint4*>(dst + s * y_pitch) = pack8(f);
@@ -432,7 +442,7 @@ __global__ void __launch_bounds__(512) gn_fused_small_kernel(const h16* __restri
 #pragma unroll
           for (int j = 0; j < 8; ++j) {
             const float t = fmaf(f[j], a[j], b[j]);
-            f[j] = (act == B200_ACT_SILU) ? silu_fast(t) : t;
+            f[j] = gn_act(t, act);
           }
           gn_store_vec<8>(dst + (long long)r * y_pitch + c_off, f);
         }
@@ -445,7 +455,7 @@ __global__ void __launch_bounds__(512) gn_fused_small_kernel(const h16* __restri
 #pragma unroll
         for (int j = 0; j < VEC; ++j) {
           const float t = fmaf(f[j], a[j], b[j]);
-          f[j] = (act == B200_ACT_SILU) ? silu_fast(t) : t;
+          f[j] = gn_act(t, act);
         }
         gn_store_vec<VEC>(dst + (long long)r * y_pitch + c_off, f);
       }
@@ -710,6 +720,7 @@ extern "C" int b200_groupnorm_apply(const b200_gn_apply_params* p, void* stream_
   const int C0 = p->x_C[0], C1 = p->x_ptr[1] ? p->x_C[1] : 0;
   const int C = C0 + C1;
   B200_CHECK_ARG(p->y_pitch >= C, "gn_apply: y_pitch %d < C %d", p->y_pitch, C);
+  B200_CHECK_ARG(gn_act_ok(p->act), "gn_apply: unsupported activation %d", p->act);
   const int vec = (C0 % 8 == 0 && C1 % 8 == 0 && p->x_pitch[0] % 8 == 0 && (C1 == 0 || p->x_pitch[1] % 8 == 0) &&
                    p->y_pitch % 8 == 0 && ((uintptr_t)p->x_ptr[0] % 16 == 0) &&
                    (C1 == 0 || (uintptr_t)p->x_ptr[1] % 16 == 0) && ((uintptr_t)p->y_ptr % 16 == 0)) ? 8 : 1;
@@ -753,7 +764,7 @@ extern "C" int b200_groupnorm_fused(const b200_gn_stats_params* sp, const b200_g
   B200_CHECK_ARG(sp->N >= 1 && sp->N <= 65535 && sp->spatial >= 1 && sp->spatial < (1ll << 24),
                  "groupnorm_fused: batch / spatial extent out of range");
   B200_CHECK_ARG(ap->y_pitch >= C, "groupnorm_fused: y_pitch %d < C %d", ap->y_pitch, C);
-  B200_CHECK_ARG(ap->act == B200_ACT_NONE || ap->act == B200_ACT_SILU, "groupnorm_fused: unsupported activation %d", ap->act);
+  B200_CHECK_ARG(gn_act_ok(ap->act), "groupnorm_fused: unsupported activation %d", ap->act);
   const int cpg = C / sp->groups;
   B200_CHECK_ARG(C1 == 0 || C0 % cpg == 0, "groupnorm_fused: a group of %d channels straddles the two sources", cpg);
   // widest vector every access of every group can use: channel offsets, row pitches and base addresses

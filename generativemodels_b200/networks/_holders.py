@@ -38,10 +38,14 @@ _ACT_CODES = {"RELU": ops.ACT_RELU, "SILU": ops.ACT_SILU, "SWISH": ops.ACT_SILU,
 
 
 def act_code(act) -> int:
-    """monai ``Act[...]`` name (or (name, kwargs) tuple with default kwargs) -> epilogue activation code."""
+    """monai ``Act[...]`` name (or (name, kwargs) tuple with default kwargs) -> epilogue activation code.  The one
+    non-default argument set with a code of its own is ``("LEAKYRELU", {"negative_slope": 0.2})`` (SPADENet)."""
     name = act[0] if isinstance(act, (tuple, list)) else act
     if isinstance(act, (tuple, list)) and len(act) > 1 and act[1]:
-        raise NotImplementedError(f"activation {act!r} with non-default arguments is not supported")
+        if str(name).upper() == "LEAKYRELU" and dict(act[1]) == {"negative_slope": 0.2}:
+            return ops.ACT_LEAKYRELU02
+        raise NotImplementedError(f"activation {act!r} with non-default arguments is not supported "
+                                  "(the only one is ('LEAKYRELU', {'negative_slope': 0.2}))")
     code = _ACT_CODES.get(str(name).upper())
     if code is None:
         raise NotImplementedError(f"activation {name!r} is not supported on the CUDA path ({sorted(_ACT_CODES)})")
@@ -55,11 +59,14 @@ def _same_padding(kernel_size: int, dilation: int = 1) -> int:
 class Convolution(nn.Module, _Cached):
     """Holder with the key layout of ``monai.networks.blocks.Convolution``: child ``conv`` is the nn.Conv /
     nn.ConvTranspose whose parameters are used (monai semantics restated in SURVEY.md §8c: padding=None -> same
-    padding, output_padding=None -> stride - 1).  ``act`` is the ADN activation ("RELU") applied in the epilogue."""
+    padding, output_padding=None -> stride - 1).  ``act`` is the ADN activation ("RELU") applied in the epilogue.
+    ``norm="INSTANCE"`` (with ``conv_only=False``) is monai's ADN order "NDA": conv, then InstanceNorm (eps 1e-5, no
+    affine, child ``adn.N`` without parameters), then ``act`` applied by the normalisation pass."""
 
     def __init__(self, spatial_dims: int, in_channels: int, out_channels: int, strides: int = 1, kernel_size: int = 3,
                  padding: int | None = None, dilation: int = 1, bias: bool = True, conv_only: bool = True,
-                 is_transposed: bool = False, output_padding: int | None = None, act: str | None = None, **_ignored):
+                 is_transposed: bool = False, output_padding: int | None = None, act: str | None = None,
+                 norm: str | None = None, **_ignored):
         super().__init__()
         self.spatial_dims, self.in_channels, self.out_channels = spatial_dims, in_channels, out_channels
         self.strides, self.kernel_size, self.dilation = strides, kernel_size, dilation
@@ -76,6 +83,12 @@ class Convolution(nn.Module, _Cached):
             ctor = nn.Conv2d if spatial_dims == 2 else nn.Conv3d
             self.conv = ctor(in_channels, out_channels, kernel_size, stride=strides, padding=self.padding, bias=bias)
         self.act = ops.ACT_NONE if (conv_only or act is None) else act_code(act)
+        self.instance_norm = not conv_only and norm is not None
+        if self.instance_norm:
+            if str(norm).upper() != "INSTANCE" or is_transposed:
+                raise NotImplementedError(f"Convolution norm {norm!r} is not supported (INSTANCE after a convolution)")
+            self.adn = nn.Sequential()
+            self.adn.add_module("N", (nn.InstanceNorm2d if spatial_dims == 2 else nn.InstanceNorm3d)(out_channels))
 
     def packed(self, splits: Sequence[int] | None = None, padding=None):
         pad = self.padding if padding is None else padding
@@ -100,6 +113,11 @@ class Convolution(nn.Module, _Cached):
         if self.is_transposed:
             return ops.conv_transpose(x, self.packed(), act1=self.act)
         srcs = [x] if isinstance(x, CL) else list(x)
+        if self.instance_norm:
+            y = ops.conv(srcs, self.packed([a.C for a in srcs]), **epilogue)
+            dev = y.t.device
+            return ops.groupnorm(y, y.C, self.adn.N.eps, ops._const_vec(y.C, 1.0, dev), ops._const_vec(y.C, 0.0, dev),
+                                 act=self.act)
         if self.act != ops.ACT_NONE:
             epilogue.setdefault("act1", self.act)
         return ops.conv(srcs, self.packed([a.C for a in srcs]), **epilogue)

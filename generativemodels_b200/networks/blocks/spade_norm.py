@@ -1,5 +1,6 @@
 """SPADE normalisation (Park et al. 2019) with the module tree of ``generative/networks/blocks/spade_norm.py``:
-``param_free_norm.N`` (GroupNorm for the diffusion / autoencoder blocks), ``mlp_shared.conv`` (+LeakyReLU),
+``param_free_norm.N`` (GroupNorm for the diffusion / autoencoder blocks, parameter-free InstanceNorm for SPADENet),
+``mlp_shared.conv`` (+LeakyReLU),
 ``mlp_gamma.conv`` and ``mlp_beta.conv``.
 
 Reference forward (spade_norm.py:78-96):  ``norm(x) * (1 + gamma(seg)) + beta(seg)`` with the segmentation map resized
@@ -42,11 +43,18 @@ class SPADE(nn.Module, _Cached):
                  hidden_channels: int = 64, norm: str | tuple = "INSTANCE", norm_params: dict | None = None) -> None:
         super().__init__()
         norm_params = dict(norm_params or {})
-        if str(norm).upper() != "GROUP":
-            raise NotImplementedError("SPADE is built with a GROUP base norm by the diffusion and autoencoder blocks; "
-                                      f"{norm!r} is not on that path")
+        kind = str(norm).upper()
+        if kind == "INSTANCE" and norm_params:
+            raise NotImplementedError(f"SPADE with an INSTANCE base norm takes no norm_params (got {norm_params!r})")
+        if kind not in ("GROUP", "INSTANCE"):
+            raise NotImplementedError(f"SPADE base norm {norm!r} is not supported: GROUP (with its norm_params) or "
+                                      "INSTANCE (default parameters)")
         self.param_free_norm = nn.Sequential()
-        self.param_free_norm.add_module("N", nn.GroupNorm(num_channels=norm_nc, **norm_params))
+        if kind == "GROUP":
+            self.param_free_norm.add_module("N", nn.GroupNorm(num_channels=norm_nc, **norm_params))
+        else:
+            inorm = nn.InstanceNorm2d if spatial_dims == 2 else nn.InstanceNorm3d
+            self.param_free_norm.add_module("N", inorm(norm_nc))
         self.mlp_shared = Convolution(spatial_dims, label_nc, hidden_channels, kernel_size=kernel_size,
                                       padding=kernel_size // 2, conv_only=False, act="LEAKYRELU")
         self.mlp_gamma = Convolution(spatial_dims, hidden_channels, norm_nc, kernel_size=kernel_size,
@@ -68,7 +76,10 @@ class SPADE(nn.Module, _Cached):
             raise RuntimeError(f"segmentation map has {seg.base.C} channels but this SPADE block was built for "
                                f"label_nc = {self.mlp_shared.in_channels}")
         gn = self.param_free_norm.N
-        affine = ops.groupnorm_affine(srcs, gn.num_groups, gn.eps, gn.weight, gn.bias)
+        if isinstance(gn, nn.GroupNorm):
+            affine = ops.groupnorm_affine(srcs, gn.num_groups, gn.eps, gn.weight, gn.bias)
+        else:       # InstanceNorm without affine: GroupNorm with one channel per group
+            affine = ops.groupnorm_affine(srcs, sum(a.C for a in srcs), gn.eps, None, None)
         dims = (a0.H, a0.W) if a0.spatial_dims == 2 else (a0.D, a0.H, a0.W)
         actv = self.mlp_shared(seg.at(dims), act1=ACT_LEAKYRELU)
         gb = ops.conv(actv, self._packed_gamma_beta())

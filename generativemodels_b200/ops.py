@@ -15,7 +15,7 @@ from typing import Sequence
 import torch
 
 from . import _lib
-from ._lib import (ACT_GEGLU, ACT_GELU, ACT_LEAKYRELU, ACT_NONE, ACT_RELU, ACT_SIGMOID, ACT_SILU, ACT_TANH, DT_H16, DT_F32, DdimCoef, DdpmCoef, GnApplyParams, GnStatsParams,
+from ._lib import (ACT_GEGLU, ACT_GELU, ACT_LEAKYRELU, ACT_LEAKYRELU02, ACT_NONE, ACT_RELU, ACT_SIGMOID, ACT_SILU, ACT_TANH, DT_H16, DT_F32, DdimCoef, DdpmCoef, GnApplyParams, GnStatsParams,
                    IgemmParams, PndmCoef, check)
 
 # torch dtype of the library's 16-bit storage type (fp16 unless B200_ACT_DTYPE=h16; see _lib.ACT_DTYPE)
@@ -23,7 +23,8 @@ H16 = torch.float16 if _lib.ACT_DTYPE == "fp16" else torch.bfloat16
 
 __all__ = ["CL", "to_cl", "from_cl", "PackedConv", "PackedConvTranspose", "PackedLinear", "conv", "conv_transpose",
            "linear", "linear_geglu", "fork", "groupnorm", "layernorm", "upsample_nearest2x", "avgpool2", "axpy", "geglu", "attention",
-           "timestep_embedding", "small_linear", "ACT_NONE", "ACT_RELU", "ACT_SILU", "ACT_LEAKYRELU", "ACT_GELU", "ACT_TANH", "ACT_SIGMOID"]
+           "timestep_embedding", "small_linear", "ACT_NONE", "ACT_RELU", "ACT_SILU", "ACT_LEAKYRELU", "ACT_GELU", "ACT_TANH", "ACT_SIGMOID",
+           "ACT_LEAKYRELU02", "upsample2x_interp", "vae_reparam_kld"]
 
 
 def _stream() -> int:
@@ -720,13 +721,13 @@ _GN_SMALL_MAX_ELEMS = 1 << 17           # spatial * channels-per-group handled b
 
 def groupnorm(srcs: CL | Sequence[CL], groups: int, eps: float, gamma: torch.Tensor, beta: torch.Tensor,
               act: int = ACT_NONE) -> CL:
-    """GroupNorm (+SiLU) over the virtual channel-concat of ``srcs``; returns one dense CL."""
+    """GroupNorm (+SiLU / LeakyReLU) over the virtual channel-concat of ``srcs``; returns one dense CL."""
     lib = _lib.require_device()
     if isinstance(srcs, CL):
         srcs = [srcs]
     a0 = srcs[0]
     Ct = sum(a.C for a in srcs)
-    if _GN_SMALL and Ct % groups == 0 and act in (ACT_NONE, ACT_SILU):
+    if _GN_SMALL and Ct % groups == 0 and act in (ACT_NONE, ACT_SILU, ACT_LEAKYRELU, ACT_LEAKYRELU02):
         cpg = Ct // groups
         if a0.spatial * cpg <= _GN_SMALL_MAX_ELEMS and cpg <= 4096 and (len(srcs) == 1 or a0.C % cpg == 0) \
                 and not (_GN_FUSE and all(a.gn is not None for a in srcs)):
@@ -802,6 +803,36 @@ def upsample_nearest2x(x: CL) -> CL:
     check(lib.b200_upsample_nearest2x(x.t.data_ptr(), x.N, x.D, x.H, x.W, x.pitch, sd, out.t.data_ptr(), _stream()),
           "b200_upsample_nearest2x")
     return out
+
+
+_INTERP_MODES = {"bilinear": _lib.INTERP_BILINEAR, "bicubic": _lib.INTERP_BICUBIC}
+
+
+def upsample2x_interp(x: CL, mode: str) -> CL:
+    """F.interpolate(scale_factor=2, mode="bilinear" | "bicubic", align_corners=False) of a 2-D channels-last tensor."""
+    if x.spatial_dims != 2 or x.D != 1:
+        raise NotImplementedError(f"{mode} x2 upsampling is 2-D only (3-D tensors take nearest)")
+    if mode not in _INTERP_MODES:
+        raise ValueError(f"unknown interpolation mode {mode!r}; expected one of {sorted(_INTERP_MODES)}")
+    lib = _lib.require_device()
+    out = x.like(dims=(1, x.H * 2, x.W * 2))
+    check(lib.b200_upsample2x_interp(x.t.data_ptr(), x.N, x.H, x.W, x.pitch, _INTERP_MODES[mode], out.t.data_ptr(),
+                                     _stream()), "b200_upsample2x_interp")
+    return out
+
+
+def vae_reparam_kld(mu: torch.Tensor, logvar: torch.Tensor, eps: torch.Tensor) -> tuple[torch.Tensor, torch.Tensor]:
+    """(eps * exp(0.5 * logvar) + mu, -0.5 * sum(1 + logvar - mu^2 - exp(logvar))) as fp32 tensors; the KL term is a
+    0-dim tensor summed in a fixed order."""
+    if mu.shape != logvar.shape or mu.shape != eps.shape:
+        raise ValueError(f"mu {tuple(mu.shape)}, logvar {tuple(logvar.shape)} and eps {tuple(eps.shape)} must match")
+    lib = _lib.require_device()
+    mu, logvar, eps = (t.contiguous().float() for t in (mu, logvar, eps))
+    z = torch.empty_like(mu)
+    kld = torch.empty((), dtype=torch.float32, device=mu.device)
+    check(lib.b200_vae_reparam_kld(mu.data_ptr(), logvar.data_ptr(), eps.data_ptr(), z.data_ptr(), kld.data_ptr(),
+                                   mu.numel(), _stream()), "b200_vae_reparam_kld")
+    return z, kld
 
 
 def avgpool2(x: CL) -> CL:

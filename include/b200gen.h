@@ -49,6 +49,10 @@ extern "C" {
  * the stored row has cout / 2 channels and no padding columns (out_cols == cout / 2).  Needs cout % 64 == 0, a h16
  * 16-byte-aligned output, no residual / scale / act2 / statistics / split. */
 #define B200_ACT_GEGLU 7
+/* nn.LeakyReLU(0.2): monai (act="LEAKYRELU", {"negative_slope": 0.2}), the default activation of SPADENet's encoder,
+ * decoder output and residual blocks (nets/spade_network.py:82,158,245-246).  A code of its own rather than a slope
+ * field, so that no parameter struct changes. */
+#define B200_ACT_LEAKYRELU02 8
 
 #define B200_IGEMM_MAX_SEG 128
 
@@ -213,7 +217,7 @@ typedef struct {
   int32_t N;
   int64_t spatial;
   const float* affine;    /* [N][C][2] from b200_groupnorm_stats          */
-  int32_t act;            /* B200_ACT_NONE / B200_ACT_SILU                */
+  int32_t act;            /* B200_ACT_NONE / SILU / LEAKYRELU / LEAKYRELU02 */
   void*   y_ptr;          /* h16 NDHWC, channel pitch y_pitch            */
   int32_t y_pitch;
 } b200_gn_apply_params;
@@ -253,6 +257,18 @@ int b200_nhwc_to_nchw(const void* x, int32_t x_dtype, int32_t N, int32_t C, int6
 /* F.interpolate(scale_factor=2, mode="nearest") (diffusion_model_unet.py:578; autoencoderkl.py:84). */
 int b200_upsample_nearest2x(const void* x, int32_t N, int32_t D, int32_t H, int32_t W, int32_t pitch,
                             int32_t dims /*2 or 3*/, void* y, void* stream);
+/* nn.Upsample(scale_factor=2, mode="bilinear" | "bicubic") on a 2-D NHWC h16 tensor [N][H][W][pitch] -> [N][2H][2W][pitch]
+ * (SPADEDecoder's upsampling_mode, nets/spade_network.py:280,317), PyTorch's align_corners=False semantics: source
+ * coordinate s = (dst + 0.5) / 2 - 0.5 per axis;
+ *   B200_INTERP_BILINEAR: s clamped at 0, taps floor(s) and min(floor(s) + 1, in - 1);
+ *   B200_INTERP_BICUBIC : s not clamped, taps floor(s) - 1 .. floor(s) + 2 each clamped to [0, in - 1], Keys cubic
+ *                         convolution weights with A = -0.75 (upsample_bicubic2d), rows interpolated first.
+ * At the fixed x2 scale the weights depend only on the output parity.  fp32 arithmetic, one rounding on the store;
+ * pad channels are interpolated like the others (zeros stay zeros).  pitch % 8 == 0. */
+#define B200_INTERP_BILINEAR 0
+#define B200_INTERP_BICUBIC  1
+int b200_upsample2x_interp(const void* x, int32_t N, int32_t H, int32_t W, int32_t pitch, int32_t mode, void* y,
+                           void* stream);
 /* nn.AvgPool{2,3}d(kernel=2, stride=2) (diffusion_model_unet.py:522). */
 int b200_avgpool2(const void* x, int32_t N, int32_t D, int32_t H, int32_t W, int32_t pitch,
                   int32_t dims, void* y, void* stream);
@@ -412,6 +428,11 @@ int b200_pndm_step(const float* const* hist, const float* sample, const b200_pnd
                    float* prev_sample, float* eps_out, int64_t n, void* stream);
 /* AutoencoderKL.encode tail (autoencoderkl.py:731-734): sigma = exp(clamp(log_var, lo, hi) / 2), fp32. */
 int b200_exp_half_clamped(const float* log_var, float lo, float hi, float* sigma, int64_t n, void* stream);
+/* SPADENet's VAE step (nets/spade_network.py:214-217, 33-34) over n fp32 elements:
+ *   z[i] = eps[i] * exp(0.5 * logvar[i]) + mu[i],   kld[0] = -0.5 * sum_i (1 + logvar[i] - mu[i]^2 - exp(logvar[i])).
+ * eps is drawn by the caller.  One CTA sums in a fixed order (fp64), so kld is the same on every call. */
+int b200_vae_reparam_kld(const float* mu, const float* logvar, const float* eps, float* z, float* kld, int64_t n,
+                         void* stream);
 /* out = x * mul / div, fp32 (latent scale_factor handling, inferer.py:385, 472-475). */
 int b200_scale_f32(const float* x, float mul, float div, float* out, int64_t n, void* stream);
 /* AutoencoderKL.sampling (autoencoderkl.py:751-752): out = a + b * c elementwise, fp32. */
