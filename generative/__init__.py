@@ -8,9 +8,10 @@ on ``sys.path`` those imports resolve here, and every ``generative.<x>`` module 
 module of the same relative name (one module object under two names, so classes, ``isinstance`` checks and pickles
 agree) — a tutorial's sampling cell or a reference test runs with only ``sys.path`` changed.
 
-The parts of the reference outside the sampling path (``generative.losses``, ``generative.metrics``,
-``generative.engines``, the GAN / encoder networks) are not provided: importing them raises ``ModuleNotFoundError``
-naming this scope (SURVEY.md section 8, out of scope), rather than silently resolving to something else.
+The discriminators (``PatchDiscriminator``, ``MultiScalePatchDiscriminator``) are provided as forward-only,
+inference-mode networks.  The training-side parts of the reference (``generative.losses``, ``generative.metrics``,
+``generative.engines``) are not provided: importing them raises ``ModuleNotFoundError`` naming this scope
+(SURVEY.md section 8, out of scope), rather than silently resolving to something else.
 """
 from __future__ import annotations
 

@@ -29,6 +29,7 @@ ACT_NONE, ACT_RELU, ACT_SILU, ACT_LEAKYRELU, ACT_GELU, ACT_TANH, ACT_SIGMOID = 0
 ACT_GEGLU = 7        # b200_igemm act1 only: [32 a | 32 gate] column groups -> a * gelu(gate), half as many output channels
 ACT_LEAKYRELU02 = 8  # nn.LeakyReLU(0.2)
 INTERP_BILINEAR, INTERP_BICUBIC = 0, 1
+POOL_AVG, POOL_MAX = 0, 1
 PRED_EPSILON, PRED_SAMPLE, PRED_V = 0, 1, 2
 IGEMM_MAX_SEG = 128
 IGEMM_SPLIT_COUNTERS = 256
@@ -143,6 +144,7 @@ SIGNATURES = {
     "b200_upsample_nearest2x": [_P, _I32, _I32, _I32, _I32, _I32, _I32, _P, _P],
     "b200_upsample2x_interp": [_P, _I32, _I32, _I32, _I32, _I32, _P, _P],
     "b200_avgpool2": [_P, _I32, _I32, _I32, _I32, _I32, _I32, _P, _P],
+    "b200_pool_s2": [_P, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _P, _P],
     "b200_axpy_h16": [_P, _P, _F, _P, _I64, _P],
     "b200_copy_channels": [_P, _I32, _I32, _P, _I32, _I32, _I64, _P],
     "b200_geglu": [_P, _I64, _I32, _I32, _P, _I32, _P],
@@ -176,6 +178,7 @@ SIGNATURES = {
     "b200_vq_argmin_gather": [_P, _I64, _I32, _I32, _P, _I32, _P, _P, _I32, _P, _I32, _P, _P, _P],
     "b200_vq_gather": [_P, _I64, _P, _I32, _I32, _P, _I32, _P],
     "b200_repack_weight": [_P, _I32, _I32, _I32, _I32, _I32, C.POINTER(RepackBlock), _I32, _P, _I32, _I32, _P],
+    "b200_batchnorm_fold": [_P, _P, _P, _P, _P, _P, _F, _I32, _I64, _P, _P, _P],
 }
 _RESTYPES = {"b200_last_error_string": C.c_char_p, "b200_groupnorm_workspace_bytes": C.c_int64,
              "b200_attention_flash_workspace_bytes": C.c_int64, "b200_igemm_split_workspace_bytes": C.c_int64}

@@ -187,6 +187,58 @@ __global__ void avgpool2_kernel(const uint4* __restrict__ x, int N, int D, int H
   }
 }
 
+// ------------------------------------------------------------------------------------------------
+// k^dims window, stride 2, padding p on channels-last h16 (PatchGAN pyramid pooling); one thread per (output voxel,
+// 8 channels).  Avg counts the padding (count_include_pad=True: with floor-mode output sizes every window lies inside
+// the padded extent, so the divisor is k^dims); max skips it (-inf) and keeps the first NaN it meets, like PyTorch.
+// ------------------------------------------------------------------------------------------------
+template <int MODE>
+__global__ void pool_s2_kernel(const uint4* __restrict__ x, int N, int D, int H, int W, int pv, int dims, int k,
+                               int pad, int OD, int OH, int OW, uint4* __restrict__ y) {
+  pdl_entry();
+  const int kd = dims == 3 ? k : 1;
+  const float div = (float)(kd * k * k);
+  const long long total = (long long)N * OD * OH * OW * pv;
+  for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < total;
+       idx += (long long)gridDim.x * blockDim.x) {
+    long long t = idx;
+    const int v = (int)(t % pv); t /= pv;
+    const int ow = (int)(t % OW); t /= OW;
+    const int oh = (int)(t % OH); t /= OH;
+    const int od = (int)(t % OD); t /= OD;
+    const int n = (int)t;
+    const int d0 = dims == 3 ? od * 2 - pad : od, h0 = oh * 2 - pad, w0 = ow * 2 - pad;
+    float acc[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) acc[j] = MODE == B200_POOL_MAX ? -INFINITY : 0.f;
+    for (int a = 0; a < kd; ++a) {
+      const int id = d0 + a;
+      if (id < 0 || id >= D) continue;
+      for (int b = 0; b < k; ++b) {
+        const int ih = h0 + b;
+        if (ih < 0 || ih >= H) continue;
+        const uint4* row = x + (((long long)n * D + id) * H + ih) * W * pv + v;
+        for (int c = 0; c < k; ++c) {
+          const int iw = w0 + c;
+          if (iw < 0 || iw >= W) continue;
+          float f[8];
+          unpack8(__ldg(row + (long long)iw * pv), f);
+#pragma unroll
+          for (int j = 0; j < 8; ++j) {
+            if constexpr (MODE == B200_POOL_MAX) acc[j] = (f[j] > acc[j] || isnan(f[j])) ? f[j] : acc[j];
+            else acc[j] += f[j];
+          }
+        }
+      }
+    }
+    if constexpr (MODE == B200_POOL_AVG) {
+#pragma unroll
+      for (int j = 0; j < 8; ++j) acc[j] /= div;
+    }
+    y[idx] = pack8(acc);
+  }
+}
+
 __global__ void axpy_h16_kernel(const uint4* __restrict__ a, const uint4* __restrict__ b, float alpha,
                                  uint4* __restrict__ y, long long nvec) {
   pdl_entry();
@@ -812,6 +864,32 @@ extern "C" int b200_avgpool2(const void* x, int32_t N, int32_t D, int32_t H, int
   B200_CUDA(b200::launch_pdl(avgpool2_kernel, grid_for(total), 256, 0, stream, reinterpret_cast<const uint4*>(x), N, D, H, W, pitch / 8, dims,
                                                       reinterpret_cast<uint4*>(y)));
   B200_LAUNCH_CHECK("avgpool2_kernel");
+  return B200_OK;
+}
+
+extern "C" int b200_pool_s2(const void* x, int32_t N, int32_t D, int32_t H, int32_t W, int32_t pitch, int32_t dims,
+                            int32_t kernel, int32_t padding, int32_t mode, void* y, void* stream_v) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
+  B200_CHECK_ARG(x && y && N >= 1 && D >= 1 && H >= 1 && W >= 1 && pitch >= 8 && pitch % 8 == 0 &&
+                 (dims == 2 || dims == 3) && (uintptr_t)x % 16 == 0 && (uintptr_t)y % 16 == 0,
+                 "pool_s2: bad arguments");
+  B200_CHECK_ARG(mode == B200_POOL_AVG || mode == B200_POOL_MAX, "pool_s2: unknown mode %d", mode);
+  B200_CHECK_ARG(kernel >= 1 && kernel <= 64 && padding >= 0 && 2 * padding <= kernel,
+                 "pool_s2: kernel %d / padding %d (padding must be at most half the kernel)", kernel, padding);
+  B200_CHECK_ARG(H + 2 * padding >= kernel && W + 2 * padding >= kernel && (dims == 2 || D + 2 * padding >= kernel),
+                 "pool_s2: input %d x %d x %d smaller than the kernel %d with padding %d", D, H, W, kernel, padding);
+  const int OD = dims == 3 ? (D + 2 * padding - kernel) / 2 + 1 : D;
+  const int OH = (H + 2 * padding - kernel) / 2 + 1, OW = (W + 2 * padding - kernel) / 2 + 1;
+  const long long total = (long long)N * OD * OH * OW * (pitch / 8);
+  if (mode == B200_POOL_MAX)
+    B200_CUDA(b200::launch_pdl(pool_s2_kernel<B200_POOL_MAX>, grid_for(total), 256, 0, stream,
+                               reinterpret_cast<const uint4*>(x), N, D, H, W, pitch / 8, dims, kernel, padding, OD, OH,
+                               OW, reinterpret_cast<uint4*>(y)));
+  else
+    B200_CUDA(b200::launch_pdl(pool_s2_kernel<B200_POOL_AVG>, grid_for(total), 256, 0, stream,
+                               reinterpret_cast<const uint4*>(x), N, D, H, W, pitch / 8, dims, kernel, padding, OD, OH,
+                               OW, reinterpret_cast<uint4*>(y)));
+  B200_LAUNCH_CHECK("pool_s2_kernel");
   return B200_OK;
 }
 

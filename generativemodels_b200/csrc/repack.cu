@@ -69,6 +69,30 @@ __global__ void __launch_bounds__(256) repack_kernel(const __grid_constant__ Rep
   *reinterpret_cast<uint4*>(p.dst + (long long)row * p.pitch + col0) = pack8(v);
 }
 
+// eval-mode BatchNorm folded into the convolution before it: s = gamma / sqrt(var + eps), w' = w * s[co],
+// b' = beta + (b - mean) * s.  fp64 arithmetic, one rounding to fp32 per output.
+__device__ __forceinline__ double bn_scale(const float* gamma, const float* var, float eps, int co) {
+  return (double)__ldg(gamma + co) / sqrt((double)__ldg(var + co) + (double)eps);
+}
+
+__global__ void __launch_bounds__(256) batchnorm_fold_kernel(const float* __restrict__ w, const float* __restrict__ b,
+                                                             const float* __restrict__ gamma,
+                                                             const float* __restrict__ beta,
+                                                             const float* __restrict__ mean,
+                                                             const float* __restrict__ var, float eps, int cout,
+                                                             long long per_out, float* __restrict__ w_out,
+                                                             float* __restrict__ b_out) {
+  pdl_entry();
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  const long long i0 = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  for (long long i = i0; i < (long long)cout * per_out; i += stride)
+    w_out[i] = (float)((double)__ldg(w + i) * bn_scale(gamma, var, eps, (int)(i / per_out)));
+  for (long long co = i0; co < cout; co += stride) {
+    const double bias = b ? (double)__ldg(b + co) : 0.0;
+    b_out[co] = (float)((double)__ldg(beta + co) + (bias - (double)__ldg(mean + co)) * bn_scale(gamma, var, eps, (int)co));
+  }
+}
+
 }  // namespace b200
 
 using namespace b200;
@@ -109,5 +133,20 @@ extern "C" int b200_repack_weight(const float* src, int32_t cout, int32_t cin, i
   B200_CHECK_ARG((total + 255) / 256 < (1ll << 31), "repack_weight: weight too large");
   B200_CUDA(b200::launch_pdl(repack_kernel, (unsigned)((total + 255) / 256), 256, 0, stream, d));
   B200_LAUNCH_CHECK("repack_kernel");
+  return B200_OK;
+}
+
+extern "C" int b200_batchnorm_fold(const float* w, const float* b, const float* gamma, const float* beta,
+                                   const float* mean, const float* var, float eps, int32_t cout, int64_t per_out,
+                                   float* w_out, float* b_out, void* stream_v) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
+  B200_CHECK_ARG(w && gamma && beta && mean && var && w_out && b_out, "batchnorm_fold: null pointer");
+  B200_CHECK_ARG(cout >= 1 && per_out >= 1 && eps >= 0.f, "batchnorm_fold: bad extent %d x %lld or eps", cout,
+                 (long long)per_out);
+  const long long blocks = ((long long)cout * per_out + 255) / 256;
+  B200_CHECK_ARG(blocks < (1ll << 31), "batchnorm_fold: weight too large");
+  B200_CUDA(b200::launch_pdl(batchnorm_fold_kernel, (unsigned)blocks, 256, 0, stream, w, b, gamma, beta, mean, var, eps,
+                             (int)cout, (long long)per_out, w_out, b_out));
+  B200_LAUNCH_CHECK("batchnorm_fold_kernel");
   return B200_OK;
 }

@@ -61,7 +61,10 @@ class Convolution(nn.Module, _Cached):
     nn.ConvTranspose whose parameters are used (monai semantics restated in SURVEY.md §8c: padding=None -> same
     padding, output_padding=None -> stride - 1).  ``act`` is the ADN activation ("RELU") applied in the epilogue.
     ``norm="INSTANCE"`` (with ``conv_only=False``) is monai's ADN order "NDA": conv, then InstanceNorm (eps 1e-5, no
-    affine, child ``adn.N`` without parameters), then ``act`` applied by the normalisation pass."""
+    affine, child ``adn.N`` without parameters), then ``act`` applied by the normalisation pass.
+    ``norm="BATCH"`` is the same order with an ``nn.BatchNorm{2,3}d`` child ``adn.N``; in eval mode it is folded into the
+    packed weights (b200_batchnorm_fold: w * s, beta + (b - mean) * s with s = gamma / sqrt(var + eps)) and ``act``
+    runs in the convolution's epilogue.  Its batch statistics are not computed: forward in train mode raises."""
 
     def __init__(self, spatial_dims: int, in_channels: int, out_channels: int, strides: int = 1, kernel_size: int = 3,
                  padding: int | None = None, dilation: int = 1, bias: bool = True, conv_only: bool = True,
@@ -83,12 +86,15 @@ class Convolution(nn.Module, _Cached):
             ctor = nn.Conv2d if spatial_dims == 2 else nn.Conv3d
             self.conv = ctor(in_channels, out_channels, kernel_size, stride=strides, padding=self.padding, bias=bias)
         self.act = ops.ACT_NONE if (conv_only or act is None) else act_code(act)
-        self.instance_norm = not conv_only and norm is not None
-        if self.instance_norm:
-            if str(norm).upper() != "INSTANCE" or is_transposed:
-                raise NotImplementedError(f"Convolution norm {norm!r} is not supported (INSTANCE after a convolution)")
+        self.norm = None if (conv_only or norm is None) else str(norm).upper()
+        self.instance_norm = self.norm == "INSTANCE"
+        if self.norm is not None:
+            if self.norm not in ("INSTANCE", "BATCH") or is_transposed:
+                raise NotImplementedError(f"Convolution norm {norm!r} is not supported (INSTANCE or BATCH after a "
+                                          "convolution)")
+            norms = {"INSTANCE": (nn.InstanceNorm2d, nn.InstanceNorm3d), "BATCH": (nn.BatchNorm2d, nn.BatchNorm3d)}
             self.adn = nn.Sequential()
-            self.adn.add_module("N", (nn.InstanceNorm2d if spatial_dims == 2 else nn.InstanceNorm3d)(out_channels))
+            self.adn.add_module("N", norms[self.norm][spatial_dims == 3](out_channels))
 
     def packed(self, splits: Sequence[int] | None = None, padding=None):
         pad = self.padding if padding is None else padding
@@ -96,6 +102,12 @@ class Convolution(nn.Module, _Cached):
         if self.is_transposed:
             return self._cached(extra, (self.conv.weight, self.conv.bias), lambda: ops.PackedConvTranspose(
                 self.conv.weight, self.conv.bias, self.strides, self.padding, self.output_padding))
+        if self.norm == "BATCH":
+            bn = self.adn.N
+            stats = (bn.weight, bn.bias, bn.running_mean, bn.running_var)
+            return self._cached(extra + ("bn", bn.eps), (self.conv.weight, self.conv.bias, *stats),
+                                lambda: ops.PackedConv(*ops.batchnorm_fold(self.conv.weight, self.conv.bias, *stats,
+                                                                           bn.eps), self.strides, pad, splits=splits))
         return self._cached(extra, (self.conv.weight, self.conv.bias), lambda: ops.PackedConv(
             self.conv.weight, self.conv.bias, self.strides, pad, splits=splits))
 
@@ -113,6 +125,9 @@ class Convolution(nn.Module, _Cached):
         if self.is_transposed:
             return ops.conv_transpose(x, self.packed(), act1=self.act)
         srcs = [x] if isinstance(x, CL) else list(x)
+        if self.norm == "BATCH" and self.training:
+            raise RuntimeError("Convolution with norm='BATCH' runs the eval-mode BatchNorm (running statistics) only; "
+                               "call .eval()")
         if self.instance_norm:
             y = ops.conv(srcs, self.packed([a.C for a in srcs]), **epilogue)
             dev = y.t.device

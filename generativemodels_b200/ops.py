@@ -24,7 +24,7 @@ H16 = torch.float16 if _lib.ACT_DTYPE == "fp16" else torch.bfloat16
 __all__ = ["CL", "to_cl", "from_cl", "PackedConv", "PackedConvTranspose", "PackedLinear", "conv", "conv_transpose",
            "linear", "linear_geglu", "fork", "groupnorm", "layernorm", "upsample_nearest2x", "avgpool2", "axpy", "geglu", "attention",
            "timestep_embedding", "small_linear", "ACT_NONE", "ACT_RELU", "ACT_SILU", "ACT_LEAKYRELU", "ACT_GELU", "ACT_TANH", "ACT_SIGMOID",
-           "ACT_LEAKYRELU02", "upsample2x_interp", "vae_reparam_kld"]
+           "ACT_LEAKYRELU02", "upsample2x_interp", "vae_reparam_kld", "pool_s2", "batchnorm_fold"]
 
 
 def _stream() -> int:
@@ -843,6 +843,43 @@ def avgpool2(x: CL) -> CL:
     check(lib.b200_avgpool2(x.t.data_ptr(), x.N, x.D, x.H, x.W, x.pitch, sd, out.t.data_ptr(), _stream()),
           "b200_avgpool2")
     return out
+
+
+_POOL_MODES = {"avg": _lib.POOL_AVG, "max": _lib.POOL_MAX}
+
+
+def pool_s2(x: CL, kernel: int, padding: int, mode: str) -> CL:
+    """nn.AvgPool{2,3}d (count_include_pad=True) / nn.MaxPool{2,3}d with the given kernel, stride 2 and padding."""
+    if mode not in _POOL_MODES:
+        raise ValueError(f"unknown pooling mode {mode!r}; expected one of {sorted(_POOL_MODES)}")
+    lib = _lib.require_device()
+    sd = x.spatial_dims
+    o = lambda i: (i + 2 * padding - kernel) // 2 + 1
+    dims = (o(x.D) if sd == 3 else x.D, o(x.H), o(x.W))
+    if min(dims) < 1 or 2 * padding > kernel:
+        raise ValueError(f"pooling kernel {kernel} / padding {padding} does not fit input {(x.D, x.H, x.W)}")
+    out = x.like(dims=dims)
+    check(lib.b200_pool_s2(x.t.data_ptr(), x.N, x.D, x.H, x.W, x.pitch, sd, kernel, padding, _POOL_MODES[mode],
+                           out.t.data_ptr(), _stream()), "b200_pool_s2")
+    return out
+
+
+def batchnorm_fold(weight: torch.Tensor, bias: torch.Tensor | None, gamma: torch.Tensor, beta: torch.Tensor,
+                   mean: torch.Tensor, var: torch.Tensor, eps: float) -> tuple[torch.Tensor, torch.Tensor]:
+    """(w * s, beta + (b - mean) * s) with s = gamma / sqrt(var + eps) per output channel: an eval-mode BatchNorm folded
+    into the convolution before it, as fp32 tensors ready for PackedConv."""
+    lib = _lib.require_device()
+    w = _src_f32(weight)
+    b, g, bt, m, v = (None if t is None else _src_f32(t) for t in (bias, gamma, beta, mean, var))
+    cout = w.shape[0]
+    if any(t.numel() != cout for t in (g, bt, m, v)) or (b is not None and b.numel() != cout):
+        raise ValueError(f"BatchNorm parameters do not match the convolution's {cout} output channels")
+    w_out = torch.empty_like(w)
+    b_out = torch.empty(cout, dtype=torch.float32, device=w.device)
+    check(lib.b200_batchnorm_fold(w.data_ptr(), _ptr(b), g.data_ptr(), bt.data_ptr(), m.data_ptr(), v.data_ptr(), eps,
+                                  cout, w.numel() // cout, w_out.data_ptr(), b_out.data_ptr(), _stream()),
+          "b200_batchnorm_fold")
+    return w_out, b_out
 
 
 def axpy(a: CL, b: CL, alpha: float = 1.0, inplace: bool = False) -> CL:

@@ -272,6 +272,18 @@ int b200_upsample2x_interp(const void* x, int32_t N, int32_t H, int32_t W, int32
 /* nn.AvgPool{2,3}d(kernel=2, stride=2) (diffusion_model_unet.py:522). */
 int b200_avgpool2(const void* x, int32_t N, int32_t D, int32_t H, int32_t W, int32_t pitch,
                   int32_t dims, void* y, void* stream);
+/* nn.AvgPool{2,3}d / nn.MaxPool{2,3}d(kernel_size=kernel, stride=2, padding=padding) on NDHWC h16 [N][D][H][W][pitch]
+ * (MultiScalePatchDiscriminator's input pyramid, nets/patchgan_discriminator.py:89-92): dims == 2 pools H and W of
+ * every D slice, dims == 3 all three.  Output extent per pooled axis floor((in + 2 * padding - kernel) / 2) + 1
+ * (ceil_mode=False); requires 2 * padding <= kernel and in + 2 * padding >= kernel.
+ *   B200_POOL_AVG: count_include_pad=True, i.e. the sum of the in-bounds taps divided by kernel^dims;
+ *   B200_POOL_MAX: padding taps are -inf; a NaN tap makes the result NaN (PyTorch's max_pool semantics).
+ * fp32 arithmetic, one rounding on the store (max is exact); pad channels stay zero.  pitch % 8 == 0, x and y
+ * 16-byte aligned. */
+#define B200_POOL_AVG 0
+#define B200_POOL_MAX 1
+int b200_pool_s2(const void* x, int32_t N, int32_t D, int32_t H, int32_t W, int32_t pitch, int32_t dims,
+                 int32_t kernel, int32_t padding, int32_t mode, void* y, void* stream);
 /* y = a + alpha * b on h16 buffers of n elements (ControlNet residual adds,
  * diffusion_model_unet.py:1917-1925,1931-1932; controlnet.py:405-407,433-434). */
 int b200_axpy_h16(const void* a, const void* b, float alpha, void* y, int64_t n, void* stream);
@@ -482,6 +494,16 @@ typedef struct {
 int b200_repack_weight(const float* src, int32_t cout, int32_t cin, int32_t taps, int32_t transposed, int32_t mode,
                        const b200_repack_block* blocks, int32_t n_blocks, void* dst, int32_t rows_pad,
                        int32_t dst_pitch, void* stream);
+/* Eval-mode nn.BatchNorm{2,3}d folded into the convolution that feeds it (monai Convolution with ADN order "NDA" and
+ * norm="BATCH", PatchDiscriminator's hidden layers, nets/patchgan_discriminator.py:229-240), before
+ * b200_repack_weight rounds the result to h16 once:
+ *   s[co] = gamma[co] / sqrt(var[co] + eps)
+ *   w_out[co][j] = w[co][j] * s[co]                       for j < per_out (= cin * taps, the parameter's layout)
+ *   b_out[co]    = beta[co] + (b[co] - mean[co]) * s[co]  (b == NULL: a convolution without bias, b = 0)
+ * fp64 arithmetic, one rounding to fp32 per output.  All arrays fp32 device memory. */
+int b200_batchnorm_fold(const float* w, const float* b, const float* gamma, const float* beta, const float* mean,
+                        const float* var, float eps, int32_t cout, int64_t per_out, float* w_out, float* b_out,
+                        void* stream);
 
 #ifdef __cplusplus
 }
