@@ -30,6 +30,8 @@ ACT_GEGLU = 7        # b200_igemm act1 only: [32 a | 32 gate] column groups -> a
 ACT_LEAKYRELU02 = 8  # nn.LeakyReLU(0.2)
 INTERP_BILINEAR, INTERP_BICUBIC = 0, 1
 POOL_AVG, POOL_MAX = 0, 1
+(INTERPOLATE_NEAREST, INTERPOLATE_LINEAR, INTERPOLATE_BILINEAR, INTERPOLATE_BICUBIC, INTERPOLATE_TRILINEAR,
+ INTERPOLATE_AREA) = 0, 1, 2, 3, 4, 5
 PRED_EPSILON, PRED_SAMPLE, PRED_V = 0, 1, 2
 IGEMM_MAX_SEG = 128
 IGEMM_SPLIT_COUNTERS = 256
@@ -145,6 +147,8 @@ SIGNATURES = {
     "b200_upsample2x_interp": [_P, _I32, _I32, _I32, _I32, _I32, _P, _P],
     "b200_avgpool2": [_P, _I32, _I32, _I32, _I32, _I32, _I32, _P, _P],
     "b200_pool_s2": [_P, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _P, _P],
+    "b200_interpolate": [_P, _I32, _P, _P, _I32, _P, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _F, _F,
+                         _F, _P],
     "b200_axpy_h16": [_P, _P, _F, _P, _I64, _P],
     "b200_copy_channels": [_P, _I32, _I32, _P, _I32, _I32, _I64, _P],
     "b200_geglu": [_P, _I64, _I32, _I32, _P, _I32, _P],

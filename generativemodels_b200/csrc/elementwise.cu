@@ -239,6 +239,196 @@ __global__ void pool_s2_kernel(const uint4* __restrict__ x, int N, int D, int H,
   }
 }
 
+// ------------------------------------------------------------------------------------------------
+// F.interpolate(size | scale_factor, mode, align_corners=False) at any size, on any strided layout; the coordinate
+// rules are ATen's (include/b200gen.h, b200_interpolate).  FAM picks the kernel family, V the thread mapping:
+//   V = 8: one thread per (output voxel, 8 channels), 16-byte vectors across channels (channel stride 1);
+//   V = 1: one thread per output element, W fastest, so that planar reads and writes coalesce.
+// The coordinate arithmetic spells out every rounding with _rn intrinsics (nearest indices depend on the exact
+// rounding of dst * ratio).  Interpolation sums are separately rounded products and sums, left to right.
+// ------------------------------------------------------------------------------------------------
+enum { INTERP_FAM_NEAREST = 0, INTERP_FAM_LINEAR = 1, INTERP_FAM_CUBIC = 2, INTERP_FAM_AREA = 3 };
+
+struct InterpArgs {
+  const void* x;
+  void* y;
+  long long xs[5], ys[5];  // element strides n, c, d, h, w
+  int x_dt, y_dt;
+  int N, C, D, H, W, OD, OH, OW, dims;
+  float rd, rh, rw;        // per-axis ratio (see the header)
+};
+
+template <int V>
+__device__ __forceinline__ void interp_load(const void* x, int dt, long long off, float* f) {
+  if constexpr (V == 8) {
+    if (dt == B200_DT_H16) {
+      unpack8(__ldg(reinterpret_cast<const uint4*>(reinterpret_cast<const h16*>(x) + off)), f);
+    } else {
+      const float4* p = reinterpret_cast<const float4*>(reinterpret_cast<const float*>(x) + off);
+      const float4 a = __ldg(p), b = __ldg(p + 1);
+      f[0] = a.x; f[1] = a.y; f[2] = a.z; f[3] = a.w;
+      f[4] = b.x; f[5] = b.y; f[6] = b.z; f[7] = b.w;
+    }
+  } else {
+    f[0] = dt == B200_DT_H16 ? h2f(reinterpret_cast<const h16*>(x)[off]) : __ldg(reinterpret_cast<const float*>(x) + off);
+  }
+}
+
+template <int V>
+__device__ __forceinline__ void interp_store(void* y, int dt, long long off, const float* f) {
+  if constexpr (V == 8) {
+    if (dt == B200_DT_H16) {
+      *reinterpret_cast<uint4*>(reinterpret_cast<h16*>(y) + off) = pack8(f);
+    } else {
+      float4* p = reinterpret_cast<float4*>(reinterpret_cast<float*>(y) + off);
+      p[0] = make_float4(f[0], f[1], f[2], f[3]);
+      p[1] = make_float4(f[4], f[5], f[6], f[7]);
+    }
+  } else {
+    if (dt == B200_DT_H16) reinterpret_cast<h16*>(y)[off] = f2h(f[0]);
+    else reinterpret_cast<float*>(y)[off] = f[0];
+  }
+}
+
+// nearest: min(floor(dst * ratio), in - 1), the product rounded once
+__device__ __forceinline__ int interp_nearest(int o, int in, float r) {
+  return min((int)floorf(__fmul_rn((float)o, r)), in - 1);
+}
+
+// source coordinate ratio * (dst + 0.5) - 0.5, one rounding (ATen's expression as compilers contract it)
+__device__ __forceinline__ float interp_src(int o, float r) {
+  return __fmaf_rn(r, __fadd_rn((float)o, 0.5f), -0.5f);
+}
+
+// linear: source clamped at 0; i0 = min(floor(s), in - 1), i1 = i0 + (i0 < in - 1), weights (1 - l, l) with
+// l = clamp(s - i0, 0, 1); an axis whose extent does not change is copied (i0 = i1 = dst, weights (1, 0))
+__device__ __forceinline__ void interp_taps_linear_any(int o, int in, int out, float r, int* i, float* w) {
+  if (in == out) {
+    i[0] = i[1] = o;
+    w[0] = 1.f;
+    w[1] = 0.f;
+    return;
+  }
+  const float s = fmaxf(interp_src(o, r), 0.f);
+  i[0] = min((int)floorf(s), in - 1);
+  i[1] = i[0] + (i[0] < in - 1 ? 1 : 0);
+  const float l = fminf(fmaxf(__fsub_rn(s, (float)i[0]), 0.f), 1.f);
+  w[0] = __fsub_rn(1.f, l);
+  w[1] = l;
+}
+
+// cubic (A = -0.75): source not clamped; f = min(floor(s), in - 1), t = clamp(s - f, 0, 1); taps f - 1 .. f + 2 each
+// clamped to [0, in - 1]; weights cc2(t + 1), cc1(t), cc1(1 - t), cc2(2 - t) with
+// cc1(x) = ((A + 2) x - (A + 3)) x x + 1 and cc2(x) = ((A x - 5A) x + 8A) x - 4A
+// (Horner steps fused like the contracted ATen expressions)
+__device__ __forceinline__ float interp_cc1(float x) {
+  return __fmaf_rn(__fmul_rn(__fmaf_rn(1.25f, x, -2.25f), x), x, 1.f);
+}
+__device__ __forceinline__ float interp_cc2(float x) {
+  return __fmaf_rn(__fmaf_rn(__fmaf_rn(-0.75f, x, 3.75f), x, -6.f), x, 3.f);
+}
+__device__ __forceinline__ void interp_taps_cubic_any(int o, int in, float r, int* i, float* w) {
+  const float s = interp_src(o, r);
+  const int f = min((int)floorf(s), in - 1);
+  const float t = fminf(fmaxf(__fsub_rn(s, (float)f), 0.f), 1.f);
+  const float u = __fsub_rn(1.f, t);
+  w[0] = interp_cc2(__fadd_rn(t, 1.f));
+  w[1] = interp_cc1(t);
+  w[2] = interp_cc1(u);
+  w[3] = interp_cc2(__fadd_rn(u, 1.f));
+#pragma unroll
+  for (int k = 0; k < 4; ++k) i[k] = min(max(f - 1 + k, 0), in - 1);
+}
+
+template <int FAM, int V>
+__global__ void __launch_bounds__(256) interpolate_kernel(const InterpArgs a) {
+  pdl_entry();
+  const int CG = V == 8 ? (a.C + 7) >> 3 : a.C;
+  const long long total = (long long)a.N * CG * a.OD * a.OH * a.OW;
+  for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < total;
+       idx += (long long)gridDim.x * blockDim.x) {
+    long long t = idx;
+    int cg = 0;
+    if constexpr (V == 8) { cg = (int)(t % CG); t /= CG; }
+    const int ow = (int)(t % a.OW); t /= a.OW;
+    const int oh = (int)(t % a.OH); t /= a.OH;
+    const int od = (int)(t % a.OD); t /= a.OD;
+    if constexpr (V == 1) { cg = (int)(t % CG); t /= CG; }
+    const long long n = t;
+    const int c = V == 8 ? cg * 8 : cg;
+    const long long xb = n * a.xs[0] + (long long)c * a.xs[1];
+    float out[V];
+    if constexpr (FAM == INTERP_FAM_NEAREST) {
+      const int id = interp_nearest(od, a.D, a.rd), ih = interp_nearest(oh, a.H, a.rh),
+                iw = interp_nearest(ow, a.W, a.rw);
+      interp_load<V>(a.x, a.x_dt, xb + id * a.xs[2] + ih * a.xs[3] + iw * a.xs[4], out);
+    } else if constexpr (FAM == INTERP_FAM_AREA) {
+      // adaptive average: window [floor(o * in / out), ceil((o + 1) * in / out)) per axis, summed d, h, w
+      // (innermost last), then divided by the three window extents in turn.  32-bit unsigned bounds (the entry point
+      // checks in * out + out <= 2^32): a 64-bit division is a subroutine call the 8-channel kernel would spill around
+      const unsigned D = a.D, H = a.H, W = a.W, OD = a.OD, OH = a.OH, OW = a.OW;
+      const int d0 = (int)(od * D / OD), d1 = (int)(((od + 1) * D + OD - 1) / OD);
+      const int h0 = (int)(oh * H / OH), h1 = (int)(((oh + 1) * H + OH - 1) / OH);
+      const int w0 = (int)(ow * W / OW), w1 = (int)(((ow + 1) * W + OW - 1) / OW);
+#pragma unroll
+      for (int j = 0; j < V; ++j) out[j] = 0.f;
+      for (int id = d0; id < d1; ++id)
+        for (int ih = h0; ih < h1; ++ih) {
+          const long long row = xb + id * a.xs[2] + ih * a.xs[3];
+          for (int iw = w0; iw < w1; ++iw) {
+            float f[V];
+            interp_load<V>(a.x, a.x_dt, row + iw * a.xs[4], f);
+#pragma unroll
+            for (int j = 0; j < V; ++j) out[j] = __fadd_rn(out[j], f[j]);
+          }
+        }
+#pragma unroll
+      for (int j = 0; j < V; ++j)
+        out[j] = __fdiv_rn(__fdiv_rn(__fdiv_rn(out[j], (float)(d1 - d0)), (float)(h1 - h0)), (float)(w1 - w0));
+    } else {
+      // separable: interpolate along W within each source row, then along H, then along D (dims 2 and 3)
+      constexpr int T = FAM == INTERP_FAM_CUBIC ? 4 : 2;
+      int wi[T], hi[T], di[2] = {od, od};
+      float ww[T], hw[T], dw[2] = {1.f, 0.f};
+#pragma unroll
+      for (int k = 0; k < T; ++k) { hi[k] = oh; hw[k] = 0.f; }
+      if constexpr (FAM == INTERP_FAM_CUBIC) {
+        interp_taps_cubic_any(ow, a.W, a.rw, wi, ww);
+        interp_taps_cubic_any(oh, a.H, a.rh, hi, hw);
+      } else {
+        interp_taps_linear_any(ow, a.W, a.OW, a.rw, wi, ww);
+        if (a.dims >= 2) interp_taps_linear_any(oh, a.H, a.OH, a.rh, hi, hw);
+        if (a.dims == 3) interp_taps_linear_any(od, a.D, a.OD, a.rd, di, dw);
+      }
+      const int TH = a.dims >= 2 ? T : 1, TD = a.dims == 3 ? 2 : 1;
+#pragma unroll
+      for (int p = 0; p < 2; ++p) {
+        if (p >= TD) break;
+        float plane[V];
+#pragma unroll
+        for (int q = 0; q < T; ++q) {
+          if (q >= TH) break;
+          float row[V];
+#pragma unroll
+          for (int k = 0; k < T; ++k) {
+            float f[V];
+            interp_load<V>(a.x, a.x_dt, xb + di[p] * a.xs[2] + hi[q] * a.xs[3] + wi[k] * a.xs[4], f);
+#pragma unroll
+            for (int j = 0; j < V; ++j) row[j] = k == 0 ? __fmul_rn(f[j], ww[0]) : __fadd_rn(row[j], __fmul_rn(f[j], ww[k]));
+          }
+#pragma unroll
+          for (int j = 0; j < V; ++j)
+            plane[j] = TH == 1 ? row[j] : q == 0 ? __fmul_rn(row[j], hw[0]) : __fadd_rn(plane[j], __fmul_rn(row[j], hw[q]));
+        }
+#pragma unroll
+        for (int j = 0; j < V; ++j)
+          out[j] = TD == 1 ? plane[j] : p == 0 ? __fmul_rn(plane[j], dw[0]) : __fadd_rn(out[j], __fmul_rn(plane[j], dw[p]));
+      }
+    }
+    interp_store<V>(a.y, a.y_dt, n * a.ys[0] + (long long)c * a.ys[1] + od * a.ys[2] + oh * a.ys[3] + ow * a.ys[4], out);
+  }
+}
+
 __global__ void axpy_h16_kernel(const uint4* __restrict__ a, const uint4* __restrict__ b, float alpha,
                                  uint4* __restrict__ y, long long nvec) {
   pdl_entry();
@@ -890,6 +1080,75 @@ extern "C" int b200_pool_s2(const void* x, int32_t N, int32_t D, int32_t H, int3
                                reinterpret_cast<const uint4*>(x), N, D, H, W, pitch / 8, dims, kernel, padding, OD, OH,
                                OW, reinterpret_cast<uint4*>(y)));
   B200_LAUNCH_CHECK("pool_s2_kernel");
+  return B200_OK;
+}
+
+template <int FAM>
+static cudaError_t launch_interpolate(const b200::InterpArgs& a, bool vec, cudaStream_t stream) {
+  const long long total = (long long)a.N * (vec ? (a.C + 7) / 8 : a.C) * a.OD * a.OH * a.OW;
+  if (vec) return b200::launch_pdl(interpolate_kernel<FAM, 8>, grid_for(total), 256, 0, stream, a);
+  return b200::launch_pdl(interpolate_kernel<FAM, 1>, grid_for(total), 256, 0, stream, a);
+}
+
+extern "C" int b200_interpolate(const void* x, int32_t x_dtype, const int64_t* x_strides, void* y, int32_t y_dtype,
+                                const int64_t* y_strides, int32_t N, int32_t C, int32_t D, int32_t H, int32_t W,
+                                int32_t OD, int32_t OH, int32_t OW, int32_t dims, int32_t mode, float ratio_d,
+                                float ratio_h, float ratio_w, void* stream_v) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
+  B200_CHECK_ARG(x && y && x_strides && y_strides, "interpolate: null pointer");
+  B200_CHECK_ARG((x_dtype == B200_DT_H16 || x_dtype == B200_DT_F32) && (y_dtype == B200_DT_H16 || y_dtype == B200_DT_F32),
+                 "interpolate: unknown dtype %d / %d", x_dtype, y_dtype);
+  const bool dims_ok = (mode == B200_INTERPOLATE_NEAREST || mode == B200_INTERPOLATE_AREA) ? (dims >= 1 && dims <= 3)
+                       : mode == B200_INTERPOLATE_LINEAR                                 ? dims == 1
+                       : (mode == B200_INTERPOLATE_BILINEAR || mode == B200_INTERPOLATE_BICUBIC) ? dims == 2
+                       : mode == B200_INTERPOLATE_TRILINEAR                              ? dims == 3
+                                                                                         : false;
+  B200_CHECK_ARG(dims_ok, "interpolate: mode %d does not take %d spatial dims", mode, dims);
+  constexpr int kMaxExtent = 1 << 24;  // coordinates are exact in fp32 below this
+  B200_CHECK_ARG(N >= 1 && C >= 1 && D >= 1 && H >= 1 && W >= 1 && OD >= 1 && OH >= 1 && OW >= 1 && D <= kMaxExtent &&
+                 H <= kMaxExtent && W <= kMaxExtent && OD <= kMaxExtent && OH <= kMaxExtent && OW <= kMaxExtent,
+                 "interpolate: bad extents %d x %d x %d x %d x %d -> %d x %d x %d", N, C, D, H, W, OD, OH, OW);
+  B200_CHECK_ARG((dims == 3 || (D == 1 && OD == 1)) && (dims >= 2 || (H == 1 && OH == 1)),
+                 "interpolate: an axis outside the %d resampled ones must have extent 1", dims);
+  for (int i = 0; i < 5; ++i) B200_CHECK_ARG(x_strides[i] >= 0 && y_strides[i] >= 0, "interpolate: negative stride");
+  if (mode == B200_INTERPOLATE_AREA) {
+    const long long lim = 1ll << 32;
+    B200_CHECK_ARG((long long)D * OD + OD <= lim && (long long)H * OH + OH <= lim && (long long)W * OW + OW <= lim,
+                   "interpolate: area window arithmetic needs in * out + out <= 2^32 per axis");
+  } else {
+    const float r[3] = {ratio_d, ratio_h, ratio_w};
+    for (int i = 3 - dims; i < 3; ++i)
+      B200_CHECK_ARG(r[i] > 0.f && r[i] <= 3.0e38f, "interpolate: ratio %g of axis %d must be positive and finite",
+                     (double)r[i], i);
+  }
+  b200::InterpArgs a;
+  a.x = x;
+  a.y = y;
+  for (int i = 0; i < 5; ++i) {
+    a.xs[i] = x_strides[i];
+    a.ys[i] = y_strides[i];
+  }
+  a.x_dt = x_dtype;
+  a.y_dt = y_dtype;
+  a.N = N; a.C = C; a.D = D; a.H = H; a.W = W; a.OD = OD; a.OH = OH; a.OW = OW; a.dims = dims;
+  a.rd = dims == 3 ? ratio_d : 1.f;
+  a.rh = dims >= 2 ? ratio_h : 1.f;
+  a.rw = ratio_w;
+  // 16-byte vectors across channels: channel stride 1 and every other stride a multiple of 8 elements on both sides,
+  // 16-byte aligned pointers, and a voxel stride that leaves room for round_up(C, 8) channels
+  const long long c8 = (C + 7) / 8 * 8;
+  bool vec = x_strides[1] == 1 && y_strides[1] == 1 && (uintptr_t)x % 16 == 0 && (uintptr_t)y % 16 == 0 &&
+             x_strides[4] >= c8 && y_strides[4] >= c8;
+  for (int i : {0, 2, 3, 4}) vec = vec && x_strides[i] % 8 == 0 && y_strides[i] % 8 == 0;
+  cudaError_t e;
+  switch (mode) {
+    case B200_INTERPOLATE_NEAREST: e = launch_interpolate<INTERP_FAM_NEAREST>(a, vec, stream); break;
+    case B200_INTERPOLATE_BICUBIC: e = launch_interpolate<INTERP_FAM_CUBIC>(a, vec, stream); break;
+    case B200_INTERPOLATE_AREA: e = launch_interpolate<INTERP_FAM_AREA>(a, vec, stream); break;
+    default: e = launch_interpolate<INTERP_FAM_LINEAR>(a, vec, stream); break;
+  }
+  B200_CUDA(e);
+  B200_LAUNCH_CHECK("interpolate_kernel");
   return B200_OK;
 }
 

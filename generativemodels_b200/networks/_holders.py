@@ -83,7 +83,7 @@ class Convolution(nn.Module, _Cached):
             self.conv = ctor(in_channels, out_channels, kernel_size, stride=strides, padding=self.padding,
                              output_padding=self.output_padding, bias=bias)
         else:
-            ctor = nn.Conv2d if spatial_dims == 2 else nn.Conv3d
+            ctor = nn.Conv1d if spatial_dims == 1 else nn.Conv2d if spatial_dims == 2 else nn.Conv3d
             self.conv = ctor(in_channels, out_channels, kernel_size, stride=strides, padding=self.padding, bias=bias)
         self.act = ops.ACT_NONE if (conv_only or act is None) else act_code(act)
         self.norm = None if (conv_only or norm is None) else str(norm).upper()

@@ -7,7 +7,9 @@ Internal activation format: :class:`CL` — channels-last h16 ``[N, D, H, W, pit
 from __future__ import annotations
 
 import ctypes as C
+import numbers
 import os
+import struct
 import weakref
 from dataclasses import dataclass
 from typing import Sequence
@@ -24,7 +26,8 @@ H16 = torch.float16 if _lib.ACT_DTYPE == "fp16" else torch.bfloat16
 __all__ = ["CL", "to_cl", "from_cl", "PackedConv", "PackedConvTranspose", "PackedLinear", "conv", "conv_transpose",
            "linear", "linear_geglu", "fork", "groupnorm", "layernorm", "upsample_nearest2x", "avgpool2", "axpy", "geglu", "attention",
            "timestep_embedding", "small_linear", "ACT_NONE", "ACT_RELU", "ACT_SILU", "ACT_LEAKYRELU", "ACT_GELU", "ACT_TANH", "ACT_SIGMOID",
-           "ACT_LEAKYRELU02", "upsample2x_interp", "vae_reparam_kld", "pool_s2", "batchnorm_fold"]
+           "ACT_LEAKYRELU02", "upsample2x_interp", "vae_reparam_kld", "pool_s2", "batchnorm_fold", "interpolate",
+           "interpolate_plan"]
 
 
 def _stream() -> int:
@@ -862,6 +865,106 @@ def pool_s2(x: CL, kernel: int, padding: int, mode: str) -> CL:
     check(lib.b200_pool_s2(x.t.data_ptr(), x.N, x.D, x.H, x.W, x.pitch, sd, kernel, padding, _POOL_MODES[mode],
                            out.t.data_ptr(), _stream()), "b200_pool_s2")
     return out
+
+
+# F.interpolate mode -> (b200_interpolate mode, the numbers of spatial dims it takes)
+_INTERPOLATE_MODES = {"nearest": (_lib.INTERPOLATE_NEAREST, (1, 2, 3)), "linear": (_lib.INTERPOLATE_LINEAR, (1,)),
+                      "bilinear": (_lib.INTERPOLATE_BILINEAR, (2,)), "bicubic": (_lib.INTERPOLATE_BICUBIC, (2,)),
+                      "trilinear": (_lib.INTERPOLATE_TRILINEAR, (3,)), "area": (_lib.INTERPOLATE_AREA, (1, 2, 3))}
+
+
+def _f32(v: float) -> float:
+    """v rounded to the nearest fp32 value (C's static_cast<float> of a double)."""
+    return struct.unpack("f", struct.pack("f", v))[0]
+
+
+def interpolate_plan(in_sizes: Sequence[int], size=None, scale_factor=None,
+                     mode: str = "nearest") -> tuple[list[int], list[float]]:
+    """F.interpolate's argument rules (align_corners=False, antialias=False, recompute_scale_factor=None) for an input
+    with spatial extents ``in_sizes``: the output extents and the per-axis fp32 ratios b200_interpolate takes.
+
+    Raises what F.interpolate raises for the same arguments, in the same order: ``ValueError`` for both or neither of
+    size / scale_factor and for a sequence of the wrong length, ``TypeError`` for a non-integer size, then
+    ``NotImplementedError`` for a mode the input's rank does not take.  With a scale factor s the output extent is
+    int(in * s) in double precision (ATen's compute_output_size) and the ratio float(1.0 / s); with a size the ratio is
+    float(in) / out (ATen's compute_scales_value).  With an odd extent the two differ: 17 -> 8 is ratio 2 with
+    scale_factor=0.5 but 2.125 with size=8."""
+    dim = len(in_sizes)
+    if size is not None and scale_factor is not None:
+        raise ValueError("only one of size or scale_factor should be defined")
+    if size is not None:
+        sizes = list(size) if isinstance(size, (list, tuple)) else [size] * dim
+        if len(sizes) != dim:
+            raise ValueError(f"Input and output must have the same number of spatial dimensions, but got input "
+                             f"with spatial dimensions of {list(in_sizes)} and output size of {size}.")
+        if not all(isinstance(v, numbers.Integral) or (torch.is_tensor(v) and not v.is_floating_point()) for v in sizes):
+            raise TypeError(f"expected size to be one of int or Tuple[int] or Tuple[int, int] or Tuple[int, int, "
+                            f"int], but got size with types {[type(v) for v in sizes]}")
+        out = [int(v) for v in sizes]
+        scales = [None] * dim
+    elif scale_factor is not None:
+        if isinstance(scale_factor, (list, tuple)):
+            if len(scale_factor) != dim:
+                raise ValueError(f"Input and scale_factor must have the same number of spatial dimensions, but got "
+                                 f"input with spatial dimensions of {list(in_sizes)} and scale_factor of shape "
+                                 f"{scale_factor}.")
+            scales = [float(s) for s in scale_factor]
+        else:
+            scales = [float(scale_factor)] * dim
+        out = [int(i * s) for i, s in zip(in_sizes, scales)]
+    else:
+        raise ValueError("either size or scale_factor should be defined")
+    if mode not in _INTERPOLATE_MODES or dim not in _INTERPOLATE_MODES[mode][1]:
+        if 1 <= dim <= 3 and mode in ("linear", "bilinear", "trilinear"):
+            need = {"linear": 3, "bilinear": 4, "trilinear": 5}[mode]
+            raise NotImplementedError(f"Got {dim + 2}D input, but {mode} mode needs {need}D input")
+        raise NotImplementedError(f"Input Error: Only 3D, 4D and 5D input Tensors supported (got {dim + 2}D) for the "
+                                  f"modes: nearest | linear | bilinear | bicubic | trilinear | area | nearest-exact (got {mode})")
+    if min(out) < 1:
+        raise RuntimeError(f"Input and output sizes should be greater than 0, but got input {list(in_sizes)} and "
+                           f"output {out}")
+    ratios = [_f32(1.0 / s) if s is not None and s > 0 else _f32(float(i) / o) for i, o, s in zip(in_sizes, out, scales)]
+    return out, ratios
+
+
+def interpolate(x: torch.Tensor | CL, size=None, scale_factor=None, mode: str = "nearest", *,
+                planar_out: bool = False) -> torch.Tensor | CL:
+    """F.interpolate(x, size=... | scale_factor=..., mode=mode, align_corners=False) in one b200_interpolate launch.
+
+    ``x`` is either a planar fp32 NC[D]HW tensor (3-, 4- or 5-D, any strides), giving a planar fp32 tensor, or a
+    :class:`CL` whose storage ``t`` is h16 or fp32 (``spatial_dims`` 1, 2 or 3; a 1-D CL has D == H == 1), giving a
+    CL of the same storage type and pitch, or with ``planar_out`` an NC[D]HW fp32 tensor.  Argument rules and
+    exceptions: :func:`interpolate_plan`."""
+    dts = {H16: DT_H16, torch.float32: DT_F32}
+    cl = isinstance(x, CL)
+    t = x.t if cl else x
+    sd = x.spatial_dims if cl else x.dim() - 2
+    in_sizes = (x.D, x.H, x.W)[3 - sd:] if cl else tuple(x.shape[2:])
+    out_sizes, ratios = interpolate_plan(in_sizes, size, scale_factor, mode)
+    if t.dtype not in (dts if cl else (torch.float32,)):
+        raise TypeError(f"interpolate reads fp32 planar or h16 / fp32 channels-last tensors, got {t.dtype}")
+    if cl:
+        N, C_ = x.N, x.C
+        x_strides = (t.stride(0), 1, t.stride(1), t.stride(2), t.stride(3))
+    else:
+        N, C_ = x.shape[:2]
+        s = x.stride()
+        x_strides = (s[0], s[1], *(0,) * (3 - sd), *s[2:])
+    lib = _lib.require_device()
+    pad = (1,) * (3 - sd)
+    if cl and not planar_out:
+        y = torch.empty((N, *pad, *out_sizes, x.pitch), dtype=t.dtype, device=t.device)
+        res = CL(y, C_, sd)
+        y_strides, y_dt = (y.stride(0), 1, y.stride(1), y.stride(2), y.stride(3)), dts[t.dtype]
+    else:
+        y = res = torch.empty((N, C_, *out_sizes), dtype=torch.float32, device=t.device)
+        s = y.stride()
+        y_strides, y_dt = (s[0], s[1], *(0,) * (3 - sd), *s[2:]), DT_F32
+    r = [1.0] * (3 - sd) + ratios
+    check(lib.b200_interpolate(t.data_ptr(), dts[t.dtype], (C.c_int64 * 5)(*x_strides), y.data_ptr(), y_dt,
+                               (C.c_int64 * 5)(*y_strides), N, C_, *pad, *in_sizes, *pad, *out_sizes, sd,
+                               _INTERPOLATE_MODES[mode][0], *r, _stream()), "b200_interpolate")
+    return res
 
 
 def batchnorm_fold(weight: torch.Tensor, bias: torch.Tensor | None, gamma: torch.Tensor, beta: torch.Tensor,

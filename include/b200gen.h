@@ -284,6 +284,47 @@ int b200_avgpool2(const void* x, int32_t N, int32_t D, int32_t H, int32_t W, int
 #define B200_POOL_MAX 1
 int b200_pool_s2(const void* x, int32_t N, int32_t D, int32_t H, int32_t W, int32_t pitch, int32_t dims,
                  int32_t kernel, int32_t padding, int32_t mode, void* y, void* stream);
+/* F.interpolate(x, size=... | scale_factor=..., mode=..., align_corners=False, antialias=False) at any size or scale
+ * (SpatialRescaler, blocks/encoder_modules.py:60,78).  x is [N][C][D][H][W] and y [N][C][OD][OH][OW] with arbitrary
+ * element strides {n, c, d, h, w} (host arrays x_strides / y_strides) and their own dtypes (B200_DT_H16 / B200_DT_F32),
+ * so one entry point reads and writes planar NC[D]HW fp32, channels-last fp32 and channels-last h16.  `dims` is the
+ * number of resampled axes, the last ones: dims == 2 needs D == OD == 1, dims == 1 also H == OH == 1.
+ * Modes and the dims they take (anything else is B200_EINVAL):
+ *   B200_INTERPOLATE_NEAREST 1, 2, 3 | _LINEAR 1 | _BILINEAR 2 | _BICUBIC 2 | _TRILINEAR 3 | _AREA 1, 2, 3.
+ * Coordinates follow ATen (ATen/native/UpSample.h and AdaptivePooling.h) per resampled axis, with the fp32 ratio r the
+ * caller passes: r = float(1.0 / scale_factor) where F.interpolate was given a scale factor, else float(in) / out
+ * (ATen's compute_scales_value: with an odd extent the two differ, e.g. 17 -> 8 samples 0.5, 2.5, ... with
+ * scale_factor=0.5 but 0.5625, 2.6875, ... with size=8).  s = fma(r, dst + 0.5, -0.5) in fp32, one rounding, which is
+ * ATen's r * (dst + 0.5) - 0.5 as its compilers contract it.
+ *   NEAREST  : src = min(floor(dst * r), in - 1) (no identity shortcut: scale_factor=1.1 on 5 samples 0,0,1,2,3);
+ *   linear family (LINEAR / BILINEAR / TRILINEAR): an axis with out == in is copied (taps dst, dst; weights 1, 0);
+ *              otherwise s is clamped at 0, i0 = min(floor(s), in - 1), i1 = i0 + (i0 < in - 1),
+ *              l = clamp(s - i0, 0, 1), weights (1 - l, l);
+ *   BICUBIC  : s not clamped, f = min(floor(s), in - 1), t = clamp(s - f, 0, 1), taps f - 1 .. f + 2 each clamped to
+ *              [0, in - 1], Keys weights with A = -0.75: cc2(t + 1), cc1(t), cc1(1 - t), cc2(2 - t) where
+ *              cc1(x) = ((A + 2) x - (A + 3)) x x + 1 and cc2(x) = ((A x - 5 A) x + 8 A) x - 4 A, each Horner step
+ *              a fused multiply-add;
+ *   AREA     : adaptive average pooling, window [floor(o * in / out), ceil((o + 1) * in / out)) per axis in integer
+ *              arithmetic (the ratios are ignored).
+ * Numerics: fp32 arithmetic, one rounding on the store (fp16 stores saturate).  NEAREST is a copy (bit-exact when the
+ * dtypes match).  The separable modes interpolate along W within each source row first, then along H, then along D;
+ * each 1-D step is sum_k x_k * w_k over its taps in order, products and sums rounded separately.  AREA sums the window
+ * in d, h, w order (w innermost) and divides by the window's D, H and W extents in turn.
+ * Threads: with channel stride 1 on both sides, every other stride a multiple of 8 elements, x and y 16-byte aligned
+ * and w strides >= round_up(C, 8), one thread moves 8 channels as 16-byte vectors; these also write channels
+ * [C, round_up(C, 8)) of every output voxel (a channels-last buffer's pad channels, interpolated from the input's
+ * own: zeros stay zeros).  Otherwise one thread per output element, W fastest, so planar reads coalesce.
+ * Extents up to 2^24 per axis (AREA: in * out + out <= 2^32); ratios of resampled axes positive and finite. */
+#define B200_INTERPOLATE_NEAREST   0
+#define B200_INTERPOLATE_LINEAR    1
+#define B200_INTERPOLATE_BILINEAR  2
+#define B200_INTERPOLATE_BICUBIC   3
+#define B200_INTERPOLATE_TRILINEAR 4
+#define B200_INTERPOLATE_AREA      5
+int b200_interpolate(const void* x, int32_t x_dtype, const int64_t* x_strides, void* y, int32_t y_dtype,
+                     const int64_t* y_strides, int32_t N, int32_t C, int32_t D, int32_t H, int32_t W, int32_t OD,
+                     int32_t OH, int32_t OW, int32_t dims, int32_t mode, float ratio_d, float ratio_h, float ratio_w,
+                     void* stream);
 /* y = a + alpha * b on h16 buffers of n elements (ControlNet residual adds,
  * diffusion_model_unet.py:1917-1925,1931-1932; controlnet.py:405-407,433-434). */
 int b200_axpy_h16(const void* a, const void* b, float alpha, void* y, int64_t n, void* stream);
