@@ -348,7 +348,8 @@ int b200_tap_sum(const float* y, int32_t y_pitch, const int32_t* geom, int32_t c
 int b200_geglu(const void* x, int64_t M, int32_t H, int32_t x_pitch, void* y, int32_t y_pitch,
                void* stream);
 /* softmax over rows of an fp32 [M, S] score matrix -> h16 probabilities [M, p_pitch]
- * (attention_scores.softmax(dim=-1), diffusion_model_unet.py:150,412). Pad columns are zeroed. */
+ * (attention_scores.softmax(dim=-1), diffusion_model_unet.py:150,412): p = h16(exp(s - max) * (1 / sum)), normalised
+ * in fp32 before the one rounding.  Pad columns [S, p_pitch) are written +0; rows past M are not written. */
 int b200_softmax_rows(const float* s, int64_t M, int32_t S, int64_t s_pitch, void* p, int64_t p_pitch,
                       void* stream);
 /* Same result in ONE pass over the scores, given the per-(row, 128-column tile) partials b200_igemm wrote. */
@@ -358,7 +359,15 @@ int b200_softmax_rows_partials(const float* s, int64_t M, int32_t S, int64_t s_p
 /* Flash-style attention on wgmma (scores stay in registers; online softmax; head_dim in {64,128,256,512}, any T, S).
  * q: [B][T][q_pitch], k: [B][S][k_pitch] h16 rows with heads as channel slices [h*dh, (h+1)*dh);
  * vt: V transposed, [B][heads*dh][vt_pitch] (key index contiguous); out / res: [B][T][pitch] h16; res may be NULL.
- * out[b,t,h*dh+c] = sum_s softmax_s(scale * q.k)[s] * v[s,c] (+ res).   (diffusion_model_unet.py:143-153, 406-416) */
+ * out[b,t,h*dh+c] = sum_s softmax_s(scale * q.k)[s] * v[s,c] (+ res).   (diffusion_model_unet.py:143-153, 406-416)
+ * Numerics: sigma_s = fp32(scale * log2 e) * q.k in fp32; the running row maximum m advances once per key block (64
+ * keys; 128 for head_dim 512); each probability is rounded to h16 from fp32 as P~_s = h16(2^(sigma_s - m_block(s)))
+ * (ex2.approx.ftz), the denominator l = sum_s 2^(sigma_s - m) is accumulated in fp32 from the unrounded values, and
+ * out = h16(sum_s P~_s 2^(m_block(s) - m) v_s / l + res) with the residual added in fp32 before the one rounding.
+ * Only [B][T][heads*dh] of out is written: not the pad columns [heads*dh, out_pitch), not rows past T.  Not read:
+ * q / k columns past heads*dh, V^T columns [S, vt_pitch), residual columns past heads*dh.
+ * B200_EINVAL for another head_dim, a pitch (res_pitch with res) not a multiple of 8, a pointer not 16-byte aligned,
+ * or B, T, S, heads < 1.  (tests/test_attention_contract_gpu.py checks all of this against tests/attention_emulator.py.) */
 typedef struct {
   const void* q; const void* k; const void* vt; void* out; const void* res;
   int32_t B, T, S, heads, dh;
@@ -372,9 +381,10 @@ int b200_attention_flash(const b200_flash_params* p, void* stream);
 /* bytes of scratch the call described by p can use (0 when none is needed); pointer fields are not read */
 int64_t b200_attention_flash_workspace_bytes(const b200_flash_params* p);
 
-/* Small-shape attention on CUDA cores (any head_dim <= 256, any S); used for the test-suite
- * head dims (2..8) and for cross-attention with a handful of context tokens.
- * q: [B, T, H*dh] h16 pitch q_pitch; k, v: [B, S, H*dh]; out: [B, T, H*dh].
+/* Small-shape attention on CUDA cores (any head_dim <= 1024, any S); used for the test-suite
+ * head dims (2..8), for head dims that are not multiples of 64 and for cross-attention with a handful of context tokens.
+ * q: [B, T, H*dh] h16 pitch q_pitch; k, v: [B, S, H*dh]; out: [B, T, H*dh].  Pitches need no alignment.
+ * fp32 scores, online softmax and accumulation; only the output is rounded, and only its [B][T][H*dh] is written.
  * (CrossAttention._attention, diffusion_model_unet.py:136-153; AttentionBlock 406-416.) */
 int b200_attention_small(const void* q, const void* k, const void* v, void* out, int32_t B, int32_t T,
                          int32_t S, int32_t heads, int32_t dh, int32_t q_pitch, int32_t k_pitch,
@@ -408,7 +418,8 @@ int b200_rows_linear(const void* x, int32_t x_pitch, int32_t M, int32_t K, const
                      int32_t act, const void* res, int32_t r_pitch, void* out, int32_t o_pitch, int32_t out_dtype,
                      void* stream);
 /* One query row per (batch, head) against S cached keys / values ([B, kv_rows, pitch] h16; S = *pos_dev + 1 when
- * pos_dev != NULL): the keys are split over the warps of a block and the online-softmax states merged. */
+ * pos_dev != NULL): the keys are split over the warps of a block and the online-softmax states merged (warps without
+ * a key count nothing).  head_dim <= 256; fp32 throughout, only the output [B][heads*dh] rounded and written. */
 int b200_attention_decode(const void* q, const void* k, const void* v, void* out, int32_t B, int32_t S,
                           int32_t heads, int32_t dh, int32_t q_pitch, int32_t k_pitch, int32_t v_pitch,
                           int32_t o_pitch, float scale, int32_t kv_rows, const int32_t* pos_dev, void* stream);
