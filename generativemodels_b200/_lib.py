@@ -34,7 +34,6 @@ POOL_AVG, POOL_MAX = 0, 1
  INTERPOLATE_AREA) = 0, 1, 2, 3, 4, 5
 PRED_EPSILON, PRED_SAMPLE, PRED_V = 0, 1, 2
 IGEMM_MAX_SEG = 128
-IGEMM_SPLIT_COUNTERS = 256
 
 
 class B200Error(RuntimeError):
@@ -64,7 +63,7 @@ class IgemmParams(C.Structure):
         ("res_sN", C.c_int64), ("res_sD", C.c_int64), ("res_sH", C.c_int64), ("res_sW", C.c_int64),
         ("act2", C.c_int32), ("stat_ptr", C.c_void_p), ("impl", C.c_int32),
         ("gn_partial", C.c_void_p), ("gn_slots", C.c_int32), ("gn_slot0", C.c_int32),
-        ("split_ws", C.c_void_p), ("split_ws_bytes", C.c_int64), ("split_counters", C.c_void_p),
+        ("split_ws", C.c_void_p), ("split_ws_bytes", C.c_int64),
         ("a_broadcast", C.c_int32), ("gn_group", C.c_int32),
     ]
 

@@ -16,7 +16,6 @@ __global__ void attention_small_kernel(const h16* __restrict__ q, const h16* __r
                                        int T, int S, int heads, int dh, int q_pitch, int k_pitch, int v_pitch,
                                        int o_pitch, float scale, int kv_rows, int causal, int q_pos0,
                                        const int* __restrict__ pos_dev) {
-  pdl_entry();
   if (pos_dev) {                 // decode step captured in a CUDA graph: the prefix length lives in device memory
     q_pos0 = *pos_dev;
     S = q_pos0 + T;
@@ -101,7 +100,7 @@ extern "C" int b200_attention_small_ex(const void* q, const void* k, const void*
   const h16* kk = reinterpret_cast<const h16*>(k);
   const h16* vv = reinterpret_cast<const h16*>(v);
   h16* oo = reinterpret_cast<h16*>(out);
-#define LAUNCH(R) B200_CUDA(b200::launch_pdl(attention_small_kernel<R>, (unsigned)blocks, wpb * 32, 0, stream,  \
+#define LAUNCH(R) B200_CUDA(b200::launch_kernel(attention_small_kernel<R>, (unsigned)blocks, wpb * 32, 0, stream,  \
       qq, kk, vv, oo, B, T, S, heads, dh, q_pitch, k_pitch, v_pitch, o_pitch, scale, kv_rows, causal, q_pos0, pos_dev))
   if (dh <= 32) LAUNCH(1);
   else if (dh <= 64) LAUNCH(2);

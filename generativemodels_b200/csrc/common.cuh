@@ -38,67 +38,26 @@ int cuda_fail(cudaError_t e, const char* what);
 
 int sm_count();
 
-// ------------------------------------------------------------------------------------------------
-// Programmatic dependent launch.  Every kernel of this library is launched with
-// cudaLaunchAttributeProgrammaticStreamSerialization and starts with pdl_launch_dependents() (the next kernel in the
-// stream may be scheduled as soon as every CTA of this one is resident) and pdl_wait() before its first global-memory
-// access (blocks until the preceding grid has COMPLETED and its writes are visible — so the data dependencies are
-// exactly those of plain stream order).  What overlaps is the next kernel's launch latency and prologue (barrier
-// initialisation, tensor-map fetch) with this kernel's execution: a latent-UNet step is 150-300 dependent kernels of
-// a few microseconds each.  The persistent tensor-core kernels hold ~200 KB of shared memory per CTA, so a dependent
-// grid can only start on SMs the running grid left idle and its early-resident CTAs then spin in griddepcontrol.wait.
-// The launches therefore go out WITHOUT the attribute by default (the device-side instructions are no-ops then);
-// B200_PDL=1 turns it on for experiments.
-// ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
-__device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
-__device__ __forceinline__ void pdl_entry() { pdl_launch_dependents(); pdl_wait(); }
-
-// B200_PDL: 0 (default) = plain stream order; 1 = attribute on, every kernel triggers its dependents at entry (the whole
-// remainder of a captured graph piles onto the idle SMs and spins); 2 = attribute on, the tensor-core GEMM kernel
-// triggers only after its producer warp has issued the last operand load (the dependent's launch latency and prologue
-// overlap this kernel's last MMAs and epilogue, and the chain of early launches stops at the next GEMM).
-inline int pdl_mode() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("B200_PDL");
-    v = (e && e[0] >= '1' && e[0] <= '2') ? e[0] - '0' : 0;
-  }
-  return v;
-}
-inline bool pdl_enabled() { return pdl_mode() != 0; }
-
-template <typename... KArgs, typename... Args>
-inline cudaError_t launch_cluster(void (*kernel)(KArgs...), int cluster_x, dim3 grid, dim3 block, size_t smem,
-                                  cudaStream_t stream, Args&&... args) {
+// Every kernel of the library goes out through this: launch_kernel(k, grid, block, smem, stream, args...), or
+// launch_kernel<Cluster>(...) for a kernel that runs in thread-block clusters of Cluster CTAs along x.
+template <int Cluster = 1, typename... KArgs, typename... Args>
+inline cudaError_t launch_kernel(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream,
+                                 Args&&... args) {
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = grid;
   cfg.blockDim = block;
   cfg.dynamicSmemBytes = smem;
   cfg.stream = stream;
-  cudaLaunchAttribute attr[2];
-  int n = 0;
-  if (pdl_enabled()) {
-    attr[n].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[n].val.programmaticStreamSerializationAllowed = 1;
-    ++n;
+  cudaLaunchAttribute attr;
+  if (Cluster > 1) {
+    attr.id = cudaLaunchAttributeClusterDimension;
+    attr.val.clusterDim.x = Cluster;
+    attr.val.clusterDim.y = 1;
+    attr.val.clusterDim.z = 1;
+    cfg.attrs = &attr;
+    cfg.numAttrs = 1;
   }
-  if (cluster_x > 1) {        // thread-block cluster of cluster_x CTAs along x
-    attr[n].id = cudaLaunchAttributeClusterDimension;
-    attr[n].val.clusterDim.x = cluster_x;
-    attr[n].val.clusterDim.y = 1;
-    attr[n].val.clusterDim.z = 1;
-    ++n;
-  }
-  cfg.attrs = attr;
-  cfg.numAttrs = n;
   return cudaLaunchKernelEx(&cfg, kernel, KArgs(std::forward<Args>(args))...);
-}
-
-template <typename... KArgs, typename... Args>
-inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream,
-                              Args&&... args) {
-  return launch_cluster(kernel, 1, grid, block, smem, stream, std::forward<Args>(args)...);
 }
 
 __device__ __forceinline__ float silu_f(float x) { return x / (1.0f + __expf(-x)); }
@@ -125,7 +84,6 @@ __device__ __forceinline__ float apply_act(float x, int act) {
 #ifdef B200_H16_IS_BF16
 typedef __nv_bfloat16 h16;
 typedef __nv_bfloat162 h162;
-#define B200_H16_FMT 1u                                   /* tcgen05 instruction-descriptor a/b format: BF16 */
 #define B200_H16_TMAP CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
 #define B200_H16_NAME "bf16"
 __device__ __forceinline__ h16 f2h(float x) { return __float2bfloat16_rn(x); }
@@ -135,7 +93,6 @@ __device__ __forceinline__ float2 h22f2(h162 v) { return __bfloat1622float2(v); 
 #else
 typedef __half h16;
 typedef __half2 h162;
-#define B200_H16_FMT 0u                                   /* F16 */
 #define B200_H16_TMAP CU_TENSOR_MAP_DATA_TYPE_FLOAT16
 #define B200_H16_NAME "fp16"
 __device__ __forceinline__ h162 f2h2(float a, float b) {  // low half = a, high half = b; saturating

@@ -18,7 +18,6 @@ __global__ void __launch_bounds__(256) rows_linear_kernel(const h16* __restrict_
                                                           int O, const float* __restrict__ bias, int act,
                                                           const h16* __restrict__ res, int r_pitch, void* out,
                                                           int o_pitch, int out_f32) {
-  pdl_entry();
   extern __shared__ __align__(16) uint8_t dsm[];
   h16* xs = reinterpret_cast<h16*>(dsm);        // [M][Kp], Kp = K rounded up to 8
   const int Kp = (K + 7) & ~7;
@@ -85,7 +84,6 @@ __global__ void __launch_bounds__(256) attention_decode_kernel(const h16* __rest
                                                                h16* __restrict__ out, int S, int heads, int dh,
                                                                int q_pitch, int k_pitch, int v_pitch, int o_pitch,
                                                                float scale, int kv_rows, const int* __restrict__ pos_dev) {
-  pdl_entry();
   if (pos_dev) S = *pos_dev + 1;
   const int h = blockIdx.x % heads, b = blockIdx.x / heads;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -169,7 +167,7 @@ extern "C" int b200_rows_linear(const void* x, int32_t x_pitch, int32_t M, int32
   B200_CHECK_ARG(smem <= 48 * 1024, "rows_linear: M * K too large (%d bytes of rows)", smem);
   int blocks = (O + 7) / 8;
   if (blocks > 8 * sm_count()) blocks = 8 * sm_count();
-  B200_CUDA(b200::launch_pdl(rows_linear_kernel, blocks, 256, smem, stream, 
+  B200_CUDA(b200::launch_kernel(rows_linear_kernel, blocks, 256, smem, stream, 
       reinterpret_cast<const h16*>(x), x_pitch, M, K, ln_gamma, ln_beta, ln_eps,
       reinterpret_cast<const h16*>(w), w_pitch, O, bias, act, reinterpret_cast<const h16*>(res),
       r_pitch, out, o_pitch, out_dtype == B200_DT_F32 ? 1 : 0));
@@ -188,7 +186,7 @@ extern "C" int b200_attention_decode(const void* q, const void* k, const void* v
   const h16* kk = reinterpret_cast<const h16*>(k);
   const h16* vv = reinterpret_cast<const h16*>(v);
   h16* oo = reinterpret_cast<h16*>(out);
-#define LAUNCH(R) B200_CUDA(b200::launch_pdl(attention_decode_kernel<R>, B * heads, 256, 0, stream, qq, kk, vv, oo, S, heads, dh, q_pitch, k_pitch, \
+#define LAUNCH(R) B200_CUDA(b200::launch_kernel(attention_decode_kernel<R>, B * heads, 256, 0, stream, qq, kk, vv, oo, S, heads, dh, q_pitch, k_pitch, \
                                                                           v_pitch, o_pitch, scale, kv_rows, pos_dev))
   if (dh <= 32) LAUNCH(1);
   else if (dh <= 64) LAUNCH(2);

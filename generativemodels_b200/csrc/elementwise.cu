@@ -11,7 +11,6 @@ namespace b200 {
 // ------------------------------------------------------------------------------------------------
 __global__ void nchw_to_nhwc_kernel(const float* __restrict__ x, int C, long long spatial,
                                     h16* __restrict__ y, int pitch) {
-  pdl_entry();
   __shared__ float tile[32][33];
   const int n = blockIdx.z;
   const long long s0 = (long long)blockIdx.x * 32;
@@ -34,7 +33,6 @@ __global__ void nchw_to_nhwc_kernel(const float* __restrict__ x, int C, long lon
 template <typename T>
 __global__ void nhwc_to_nchw_kernel(const T* __restrict__ x, int C, long long spatial, int pitch,
                                     float* __restrict__ y) {
-  pdl_entry();
   __shared__ float tile[32][33];
   const int n = blockIdx.z;
   const long long s0 = (long long)blockIdx.x * 32;
@@ -64,7 +62,6 @@ __global__ void nhwc_to_nchw_kernel(const T* __restrict__ x, int C, long long sp
 // ------------------------------------------------------------------------------------------------
 __global__ void upsample2x_kernel(const uint4* __restrict__ x, int N, int D, int H, int W, int pv, int dims,
                                   uint4* __restrict__ y) {
-  pdl_entry();
   const int OD = dims == 3 ? 2 * D : D, OH = 2 * H, OW = 2 * W;
   const long long total = (long long)N * OD * OH * OW * pv;
   for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < total;
@@ -110,7 +107,6 @@ __device__ __forceinline__ void interp_taps_cubic(int o, int n, int* idx, float*
 template <int MODE>
 __global__ void upsample2x_interp_kernel(const uint4* __restrict__ x, int N, int H, int W, int pv,
                                          uint4* __restrict__ y) {
-  pdl_entry();
   constexpr int T = MODE == B200_INTERP_BICUBIC ? 4 : 2;
   const int OH = 2 * H, OW = 2 * W;
   const long long total = (long long)N * OH * OW * pv;
@@ -155,7 +151,6 @@ __global__ void upsample2x_interp_kernel(const uint4* __restrict__ x, int N, int
 
 __global__ void avgpool2_kernel(const uint4* __restrict__ x, int N, int D, int H, int W, int pv, int dims,
                                 uint4* __restrict__ y) {
-  pdl_entry();
   const int OD = dims == 3 ? D / 2 : D, OH = H / 2, OW = W / 2;
   const int kd = dims == 3 ? 2 : 1;
   const float inv = 1.0f / (float)(kd * 4);
@@ -195,7 +190,6 @@ __global__ void avgpool2_kernel(const uint4* __restrict__ x, int N, int D, int H
 template <int MODE>
 __global__ void pool_s2_kernel(const uint4* __restrict__ x, int N, int D, int H, int W, int pv, int dims, int k,
                                int pad, int OD, int OH, int OW, uint4* __restrict__ y) {
-  pdl_entry();
   const int kd = dims == 3 ? k : 1;
   const float div = (float)(kd * k * k);
   const long long total = (long long)N * OD * OH * OW * pv;
@@ -342,7 +336,6 @@ __device__ __forceinline__ void interp_taps_cubic_any(int o, int in, float r, in
 
 template <int FAM, int V>
 __global__ void __launch_bounds__(256) interpolate_kernel(const InterpArgs a) {
-  pdl_entry();
   const int CG = V == 8 ? (a.C + 7) >> 3 : a.C;
   const long long total = (long long)a.N * CG * a.OD * a.OH * a.OW;
   for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < total;
@@ -431,7 +424,6 @@ __global__ void __launch_bounds__(256) interpolate_kernel(const InterpArgs a) {
 
 __global__ void axpy_h16_kernel(const uint4* __restrict__ a, const uint4* __restrict__ b, float alpha,
                                  uint4* __restrict__ y, long long nvec) {
-  pdl_entry();
   for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < nvec;
        idx += (long long)gridDim.x * blockDim.x) {
     float fa[8], fb[8];
@@ -445,7 +437,6 @@ __global__ void axpy_h16_kernel(const uint4* __restrict__ a, const uint4* __rest
 
 __global__ void copy_channels_kernel(const h16* __restrict__ src, int C, int src_pitch,
                                      h16* __restrict__ dst, int dst_pitch, int dst_off, long long rows, int vec) {
-  pdl_entry();
   const int per_row = C / vec;
   const long long total = rows * per_row;
   for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < total;
@@ -466,7 +457,6 @@ __device__ __forceinline__ float gelu_erf(float x) { return 0.5f * x * (1.0f + e
 
 __global__ void geglu_kernel(const h16* __restrict__ x, long long M, int H, int x_pitch,
                              h16* __restrict__ y, int y_pitch) {
-  pdl_entry();
   const int HV = H / 8;
   const long long total = M * HV;
   for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < total;
@@ -488,7 +478,6 @@ __global__ void geglu_kernel(const h16* __restrict__ x, long long M, int H, int 
 template <int TPR>
 __global__ void softmax_rows_kernel(const float* __restrict__ s, long long M, int S, long long s_pitch,
                                     h16* __restrict__ p, long long p_pitch) {
-  pdl_entry();
   constexpr int RPB = 256 / TPR;
   const long long row = (long long)blockIdx.x * RPB + threadIdx.x / TPR;
   const int t = threadIdx.x % TPR;
@@ -530,7 +519,6 @@ __global__ void softmax_rows_kernel(const float* __restrict__ s, long long M, in
 __global__ void softmax_rows_partials_kernel(const float* __restrict__ s, int S, long long s_pitch,
                                              const float2* __restrict__ part, int n_tiles,
                                              h16* __restrict__ p, long long p_pitch) {
-  pdl_entry();
   const long long row = blockIdx.x;
   const int t = threadIdx.x;
   __shared__ float red[8];
@@ -583,7 +571,6 @@ __global__ void softmax_rows_partials_kernel(const float* __restrict__ s, int S,
 // ------------------------------------------------------------------------------------------------
 __global__ void timestep_embedding_kernel(const float* __restrict__ t, int N, int dim, float max_period,
                                           float* __restrict__ emb) {
-  pdl_entry();
   const int half = dim / 2;
   const int idx = blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= N * dim) return;
@@ -606,7 +593,6 @@ template <bool VEC>
 __global__ void small_linear_kernel(const float* __restrict__ x, int M, int K, const float* __restrict__ W,
                                     const float* __restrict__ b, int O, int act_in, int act_out,
                                     float* __restrict__ y) {
-  pdl_entry();
   const int o = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (o >= O) return;
   const int lane = threadIdx.x & 31;
@@ -671,7 +657,6 @@ template <int VEC>
 __global__ void __launch_bounds__(256) ddim_step_kernel(const float* __restrict__ eps_in, const float* __restrict__ x,
                                                         const float* __restrict__ noise, b200_ddim_coef c,
                                                         float* __restrict__ prev, float* __restrict__ x0_out, long long n) {
-  pdl_entry();
   const long long tid = (long long)blockIdx.x * blockDim.x + threadIdx.x, nthr = (long long)gridDim.x * blockDim.x;
   const bool has_noise = noise != nullptr;
   long long done = 0;
@@ -712,7 +697,6 @@ __global__ void ddpm_step_kernel(const float* __restrict__ eps_in, const float* 
                                  const float* __restrict__ noise, const float* __restrict__ pred_var,
                                  b200_ddpm_coef c, float* __restrict__ prev, float* __restrict__ x0_out,
                                  long long n) {
-  pdl_entry();
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n;
        i += (long long)gridDim.x * blockDim.x) {
     const float m = eps_in[i], s = x[i];
@@ -744,7 +728,6 @@ __device__ __forceinline__ float approx_normal_cdf(float x) {
 __global__ void ddpm_kl_kernel(const float* __restrict__ x0, const float* __restrict__ xt,
                                const float* __restrict__ mo, b200_kl_coef c, float* __restrict__ kl_out,
                                double* __restrict__ sample_sum, long long per_sample) {
-  pdl_entry();
   const int n = blockIdx.y;
   const long long base = (long long)n * per_sample;
   float acc = 0.f;
@@ -794,7 +777,6 @@ struct PndmPtrs { const float* h[4]; };
 
 __global__ void pndm_step_kernel(PndmPtrs hp, const float* __restrict__ x, b200_pndm_coef c,
                                  float* __restrict__ prev, float* __restrict__ eps_out, long long n) {
-  pdl_entry();
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n;
        i += (long long)gridDim.x * blockDim.x) {
     float e = 0.f;
@@ -813,7 +795,6 @@ __global__ void pndm_step_kernel(PndmPtrs hp, const float* __restrict__ x, b200_
 __global__ void add_noise_kernel(const float* __restrict__ x0, const float* __restrict__ noise,
                                  const float* __restrict__ ca, const float* __restrict__ cb, float sign_b,
                                  long long per_sample, float* __restrict__ out) {
-  pdl_entry();
   const int n = blockIdx.y;
   const float a = ca[n], b = cb[n] * sign_b;
   const long long base = (long long)n * per_sample;
@@ -823,14 +804,12 @@ __global__ void add_noise_kernel(const float* __restrict__ x0, const float* __re
 }
 
 __global__ void exp_half_clamped_kernel(const float* __restrict__ x, float lo, float hi, float* __restrict__ y, long long n) {
-  pdl_entry();
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
     y[i] = expf(fminf(fmaxf(x[i], lo), hi) / 2.0f);
 }
 
 __global__ void fma_f32_kernel(const float* __restrict__ a, const float* __restrict__ b, const float* __restrict__ c,
                                float* __restrict__ y, long long n) {
-  pdl_entry();
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
     y[i] = a[i] + b[i] * c[i];
 }
@@ -840,7 +819,6 @@ __global__ void __launch_bounds__(256) vae_reparam_kld_kernel(const float* __res
                                                               const float* __restrict__ logvar,
                                                               const float* __restrict__ eps, float* __restrict__ z,
                                                               float* __restrict__ kld, long long n) {
-  pdl_entry();
   double s = 0.0;
   for (long long i = threadIdx.x; i < n; i += blockDim.x) {
     const float m = mu[i], lv = logvar[i];
@@ -860,7 +838,6 @@ __global__ void __launch_bounds__(256) vae_reparam_kld_kernel(const float* __res
 }
 
 __global__ void scale_f32_kernel(const float* __restrict__ x, float mul, float div, float* __restrict__ y, long long n) {
-  pdl_entry();
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
     y[i] = x[i] * mul / div;
 }
@@ -886,7 +863,6 @@ struct TapGeom {
 
 __global__ void tap_gather_kernel(const h16* __restrict__ x, int C, int x_pitch, TapGeom g,
                                   h16* __restrict__ out, int out_pitch) {
-  pdl_entry();
   // one thread per (output voxel, 8-column vector): the voxel coordinates are decoded once, the row is written with
   // 16-byte stores (out_pitch is a multiple of 8: it is the K pitch of the GEMM that follows)
   const int taps = g.kd * g.kh * g.kw;
@@ -922,7 +898,6 @@ __global__ void tap_gather_kernel(const h16* __restrict__ x, int C, int x_pitch,
 template <int COUT>
 __global__ void tap_sum_kernel(const float* __restrict__ y, int y_pitch, TapGeom g, const float* __restrict__ bias,
                                void* __restrict__ out, int out_pitch, int out_dtype) {
-  pdl_entry();
   const long long total = (long long)g.N * g.OD * g.OH * g.OW;
   for (long long v = (long long)blockIdx.x * blockDim.x + threadIdx.x; v < total;
        v += (long long)gridDim.x * blockDim.x) {
@@ -964,7 +939,6 @@ __global__ void tap_sum_kernel(const float* __restrict__ y, int y_pitch, TapGeom
 __global__ void embed_tokens_kernel(const long long* __restrict__ tokens, long long M, int seq_len, int pos0,
                                     const float* __restrict__ tok_emb, const float* __restrict__ pos_emb, int C,
                                     h16* __restrict__ out, int pitch, const int* __restrict__ pos_dev) {
-  pdl_entry();
   if (pos_dev) pos0 = *pos_dev;
   const long long total = M * pitch;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total;
@@ -988,7 +962,7 @@ extern "C" int b200_nchw_to_nhwc(const float* x, int32_t N, int32_t C, int64_t s
   const long long bx = (spatial + 31) / 32;
   B200_CHECK_ARG(bx < (1ll << 31) && N <= 65535, "nchw_to_nhwc: extent too large");
   dim3 grid((unsigned)bx, (pitch + 31) / 32, N);
-  B200_CUDA(b200::launch_pdl(nchw_to_nhwc_kernel, grid, dim3(32, 8), 0, stream, x, C, spatial, reinterpret_cast<h16*>(y), pitch));
+  B200_CUDA(b200::launch_kernel(nchw_to_nhwc_kernel, grid, dim3(32, 8), 0, stream, x, C, spatial, reinterpret_cast<h16*>(y), pitch));
   B200_LAUNCH_CHECK("nchw_to_nhwc_kernel");
   return B200_OK;
 }
@@ -1001,9 +975,9 @@ extern "C" int b200_nhwc_to_nchw(const void* x, int32_t x_dtype, int32_t N, int3
   B200_CHECK_ARG(bx < (1ll << 31) && N <= 65535, "nhwc_to_nchw: extent too large");
   dim3 grid((unsigned)bx, (C + 31) / 32, N);
   if (x_dtype == B200_DT_H16)
-    B200_CUDA(b200::launch_pdl(nhwc_to_nchw_kernel<h16>, grid, dim3(32, 8), 0, stream, reinterpret_cast<const h16*>(x), C, spatial, pitch, y));
+    B200_CUDA(b200::launch_kernel(nhwc_to_nchw_kernel<h16>, grid, dim3(32, 8), 0, stream, reinterpret_cast<const h16*>(x), C, spatial, pitch, y));
   else
-    B200_CUDA(b200::launch_pdl(nhwc_to_nchw_kernel<float>, grid, dim3(32, 8), 0, stream, reinterpret_cast<const float*>(x), C, spatial, pitch, y));
+    B200_CUDA(b200::launch_kernel(nhwc_to_nchw_kernel<float>, grid, dim3(32, 8), 0, stream, reinterpret_cast<const float*>(x), C, spatial, pitch, y));
   B200_LAUNCH_CHECK("nhwc_to_nchw_kernel");
   return B200_OK;
 }
@@ -1013,7 +987,7 @@ extern "C" int b200_upsample_nearest2x(const void* x, int32_t N, int32_t D, int3
   cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
   B200_CHECK_ARG(x && y && pitch % 8 == 0 && (dims == 2 || dims == 3), "upsample2x: bad arguments");
   const long long total = (long long)N * (dims == 3 ? 2 * D : D) * 2 * H * 2 * W * (pitch / 8);
-  B200_CUDA(b200::launch_pdl(upsample2x_kernel, grid_for(total), 256, 0, stream, reinterpret_cast<const uint4*>(x), N, D, H, W, pitch / 8, dims,
+  B200_CUDA(b200::launch_kernel(upsample2x_kernel, grid_for(total), 256, 0, stream, reinterpret_cast<const uint4*>(x), N, D, H, W, pitch / 8, dims,
                                                         reinterpret_cast<uint4*>(y)));
   B200_LAUNCH_CHECK("upsample2x_kernel");
   return B200_OK;
@@ -1027,10 +1001,10 @@ extern "C" int b200_upsample2x_interp(const void* x, int32_t N, int32_t H, int32
   B200_CHECK_ARG(mode == B200_INTERP_BILINEAR || mode == B200_INTERP_BICUBIC, "upsample2x_interp: unknown mode %d", mode);
   const long long total = (long long)N * 2 * H * 2 * W * (pitch / 8);
   if (mode == B200_INTERP_BICUBIC)
-    B200_CUDA(b200::launch_pdl(upsample2x_interp_kernel<B200_INTERP_BICUBIC>, grid_for(total), 256, 0, stream,
+    B200_CUDA(b200::launch_kernel(upsample2x_interp_kernel<B200_INTERP_BICUBIC>, grid_for(total), 256, 0, stream,
                                reinterpret_cast<const uint4*>(x), N, H, W, pitch / 8, reinterpret_cast<uint4*>(y)));
   else
-    B200_CUDA(b200::launch_pdl(upsample2x_interp_kernel<B200_INTERP_BILINEAR>, grid_for(total), 256, 0, stream,
+    B200_CUDA(b200::launch_kernel(upsample2x_interp_kernel<B200_INTERP_BILINEAR>, grid_for(total), 256, 0, stream,
                                reinterpret_cast<const uint4*>(x), N, H, W, pitch / 8, reinterpret_cast<uint4*>(y)));
   B200_LAUNCH_CHECK("upsample2x_interp_kernel");
   return B200_OK;
@@ -1040,7 +1014,7 @@ extern "C" int b200_vae_reparam_kld(const float* mu, const float* logvar, const 
                                     int64_t n, void* stream_v) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
   B200_CHECK_ARG(mu && logvar && eps && z && kld && n >= 1, "vae_reparam_kld: bad arguments");
-  B200_CUDA(b200::launch_pdl(vae_reparam_kld_kernel, 1, 256, 0, stream, mu, logvar, eps, z, kld, (long long)n));
+  B200_CUDA(b200::launch_kernel(vae_reparam_kld_kernel, 1, 256, 0, stream, mu, logvar, eps, z, kld, (long long)n));
   B200_LAUNCH_CHECK("vae_reparam_kld_kernel");
   return B200_OK;
 }
@@ -1051,7 +1025,7 @@ extern "C" int b200_avgpool2(const void* x, int32_t N, int32_t D, int32_t H, int
   B200_CHECK_ARG(x && y && pitch % 8 == 0 && (dims == 2 || dims == 3), "avgpool2: bad arguments");
   const long long total = (long long)N * (dims == 3 ? D / 2 : D) * (H / 2) * (W / 2) * (pitch / 8);
   if (total == 0) return B200_OK;
-  B200_CUDA(b200::launch_pdl(avgpool2_kernel, grid_for(total), 256, 0, stream, reinterpret_cast<const uint4*>(x), N, D, H, W, pitch / 8, dims,
+  B200_CUDA(b200::launch_kernel(avgpool2_kernel, grid_for(total), 256, 0, stream, reinterpret_cast<const uint4*>(x), N, D, H, W, pitch / 8, dims,
                                                       reinterpret_cast<uint4*>(y)));
   B200_LAUNCH_CHECK("avgpool2_kernel");
   return B200_OK;
@@ -1072,11 +1046,11 @@ extern "C" int b200_pool_s2(const void* x, int32_t N, int32_t D, int32_t H, int3
   const int OH = (H + 2 * padding - kernel) / 2 + 1, OW = (W + 2 * padding - kernel) / 2 + 1;
   const long long total = (long long)N * OD * OH * OW * (pitch / 8);
   if (mode == B200_POOL_MAX)
-    B200_CUDA(b200::launch_pdl(pool_s2_kernel<B200_POOL_MAX>, grid_for(total), 256, 0, stream,
+    B200_CUDA(b200::launch_kernel(pool_s2_kernel<B200_POOL_MAX>, grid_for(total), 256, 0, stream,
                                reinterpret_cast<const uint4*>(x), N, D, H, W, pitch / 8, dims, kernel, padding, OD, OH,
                                OW, reinterpret_cast<uint4*>(y)));
   else
-    B200_CUDA(b200::launch_pdl(pool_s2_kernel<B200_POOL_AVG>, grid_for(total), 256, 0, stream,
+    B200_CUDA(b200::launch_kernel(pool_s2_kernel<B200_POOL_AVG>, grid_for(total), 256, 0, stream,
                                reinterpret_cast<const uint4*>(x), N, D, H, W, pitch / 8, dims, kernel, padding, OD, OH,
                                OW, reinterpret_cast<uint4*>(y)));
   B200_LAUNCH_CHECK("pool_s2_kernel");
@@ -1086,8 +1060,8 @@ extern "C" int b200_pool_s2(const void* x, int32_t N, int32_t D, int32_t H, int3
 template <int FAM>
 static cudaError_t launch_interpolate(const b200::InterpArgs& a, bool vec, cudaStream_t stream) {
   const long long total = (long long)a.N * (vec ? (a.C + 7) / 8 : a.C) * a.OD * a.OH * a.OW;
-  if (vec) return b200::launch_pdl(interpolate_kernel<FAM, 8>, grid_for(total), 256, 0, stream, a);
-  return b200::launch_pdl(interpolate_kernel<FAM, 1>, grid_for(total), 256, 0, stream, a);
+  if (vec) return b200::launch_kernel(interpolate_kernel<FAM, 8>, grid_for(total), 256, 0, stream, a);
+  return b200::launch_kernel(interpolate_kernel<FAM, 1>, grid_for(total), 256, 0, stream, a);
 }
 
 extern "C" int b200_interpolate(const void* x, int32_t x_dtype, const int64_t* x_strides, void* y, int32_t y_dtype,
@@ -1156,7 +1130,7 @@ extern "C" int b200_axpy_h16(const void* a, const void* b, float alpha, void* y,
   cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
   B200_CHECK_ARG(a && b && y && n % 8 == 0, "axpy_h16: element count must be a multiple of 8");
   if (n == 0) return B200_OK;
-  B200_CUDA(b200::launch_pdl(axpy_h16_kernel, grid_for(n / 8), 256, 0, stream, reinterpret_cast<const uint4*>(a), reinterpret_cast<const uint4*>(b),
+  B200_CUDA(b200::launch_kernel(axpy_h16_kernel, grid_for(n / 8), 256, 0, stream, reinterpret_cast<const uint4*>(a), reinterpret_cast<const uint4*>(b),
                                                        alpha, reinterpret_cast<uint4*>(y), n / 8));
   B200_LAUNCH_CHECK("axpy_h16_kernel");
   return B200_OK;
@@ -1177,7 +1151,7 @@ extern "C" int b200_tap_gather(const void* x, int32_t C, int32_t x_pitch, const 
   B200_CHECK_ARG(tap_geom_ok(g) && out_pitch >= g.kd * g.kh * g.kw * C && out_pitch % 8 == 0 &&
                  ((uintptr_t)out % 16) == 0, "tap_gather: bad geometry (out_pitch must be a multiple of 8)");
   const long long total = (long long)g.N * g.OD * g.OH * g.OW * (out_pitch / 8);
-  B200_CUDA(b200::launch_pdl(tap_gather_kernel, grid_for(total), 256, 0, stream, reinterpret_cast<const h16*>(x), C, x_pitch, g,
+  B200_CUDA(b200::launch_kernel(tap_gather_kernel, grid_for(total), 256, 0, stream, reinterpret_cast<const h16*>(x), C, x_pitch, g,
                                                         reinterpret_cast<h16*>(out), out_pitch));
   B200_LAUNCH_CHECK("tap_gather_kernel");
   return B200_OK;
@@ -1194,10 +1168,10 @@ extern "C" int b200_tap_sum(const float* y, int32_t y_pitch, const int32_t* geom
   const long long total = (long long)g.N * g.OD * g.OH * g.OW;
   const unsigned grid = grid_for(total);
   switch (cout) {
-    case 1: B200_CUDA(b200::launch_pdl(tap_sum_kernel<1>, grid, 256, 0, stream, y, y_pitch, g, bias, out, out_pitch, out_dtype)); break;
-    case 2: B200_CUDA(b200::launch_pdl(tap_sum_kernel<2>, grid, 256, 0, stream, y, y_pitch, g, bias, out, out_pitch, out_dtype)); break;
-    case 3: B200_CUDA(b200::launch_pdl(tap_sum_kernel<3>, grid, 256, 0, stream, y, y_pitch, g, bias, out, out_pitch, out_dtype)); break;
-    default: B200_CUDA(b200::launch_pdl(tap_sum_kernel<4>, grid, 256, 0, stream, y, y_pitch, g, bias, out, out_pitch, out_dtype)); break;
+    case 1: B200_CUDA(b200::launch_kernel(tap_sum_kernel<1>, grid, 256, 0, stream, y, y_pitch, g, bias, out, out_pitch, out_dtype)); break;
+    case 2: B200_CUDA(b200::launch_kernel(tap_sum_kernel<2>, grid, 256, 0, stream, y, y_pitch, g, bias, out, out_pitch, out_dtype)); break;
+    case 3: B200_CUDA(b200::launch_kernel(tap_sum_kernel<3>, grid, 256, 0, stream, y, y_pitch, g, bias, out, out_pitch, out_dtype)); break;
+    default: B200_CUDA(b200::launch_kernel(tap_sum_kernel<4>, grid, 256, 0, stream, y, y_pitch, g, bias, out, out_pitch, out_dtype)); break;
   }
   B200_LAUNCH_CHECK("tap_sum_kernel");
   return B200_OK;
@@ -1207,7 +1181,6 @@ extern "C" int b200_tap_sum(const float* y, int32_t y_pitch, const int32_t* geom
 // rows of T new tokens per sequence appended to a [B, L, pitch] key/value cache at the device-side position
 __global__ void cache_append_kernel(const h16* __restrict__ src, h16* __restrict__ cache, int B,
                                     int T, int L, int pitch, const int* __restrict__ pos_dev) {
-  pdl_entry();
   const int pos = *pos_dev;
   const long long total = (long long)B * T * pitch;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total;
@@ -1218,14 +1191,13 @@ __global__ void cache_append_kernel(const h16* __restrict__ src, h16* __restrict
     if (pos + t < L) cache[((long long)b * L + pos + t) * pitch + c] = src[i];
   }
 }
-__global__ void advance_i32_kernel(int* p, int delta) {
-  pdl_entry(); *p += delta; }
+__global__ void advance_i32_kernel(int* p, int delta) { *p += delta; }
 
 extern "C" int b200_cache_append(const void* src, void* cache, int32_t B, int32_t T, int32_t L, int32_t pitch,
                                  const int32_t* pos_dev, void* stream_v) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
   B200_CHECK_ARG(src && cache && pos_dev && B >= 1 && T >= 1 && L >= T && pitch >= 1, "cache_append: bad arguments");
-  B200_CUDA(b200::launch_pdl(cache_append_kernel, grid_for((long long)B * T * pitch), 256, 0, stream, 
+  B200_CUDA(b200::launch_kernel(cache_append_kernel, grid_for((long long)B * T * pitch), 256, 0, stream, 
       reinterpret_cast<const h16*>(src), reinterpret_cast<h16*>(cache), B, T, L, pitch, pos_dev));
   B200_LAUNCH_CHECK("cache_append_kernel");
   return B200_OK;
@@ -1234,7 +1206,7 @@ extern "C" int b200_cache_append(const void* src, void* cache, int32_t B, int32_
 extern "C" int b200_advance_i32(int32_t* p, int32_t delta, void* stream_v) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
   B200_CHECK_ARG(p != nullptr, "advance_i32: null pointer");
-  B200_CUDA(b200::launch_pdl(advance_i32_kernel, 1, 1, 0, stream, p, delta));
+  B200_CUDA(b200::launch_kernel(advance_i32_kernel, 1, 1, 0, stream, p, delta));
   B200_LAUNCH_CHECK("advance_i32_kernel");
   return B200_OK;
 }
@@ -1245,7 +1217,7 @@ extern "C" int b200_embed_tokens(const int64_t* tokens, int64_t M, int32_t seq_l
   cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
   B200_CHECK_ARG(tokens && tok_emb && pos_emb && out && M >= 1 && seq_len >= 1 && pos0 >= 0 && C >= 1 && pitch >= C,
                  "embed_tokens: bad arguments");
-  B200_CUDA(b200::launch_pdl(embed_tokens_kernel, grid_for(M * pitch), 256, 0, stream, reinterpret_cast<const long long*>(tokens), M, seq_len,
+  B200_CUDA(b200::launch_kernel(embed_tokens_kernel, grid_for(M * pitch), 256, 0, stream, reinterpret_cast<const long long*>(tokens), M, seq_len,
                                                               pos0, tok_emb, pos_emb, C,
                                                               reinterpret_cast<h16*>(out), pitch, pos_dev));
   B200_LAUNCH_CHECK("embed_tokens_kernel");
@@ -1258,7 +1230,7 @@ extern "C" int b200_copy_channels(const void* src, int32_t C, int32_t src_pitch,
   B200_CHECK_ARG(src && dst && C >= 1 && src_pitch >= C && dst_pitch >= dst_off + C && rows >= 1, "copy_channels: bad arguments");
   const int vec = (C % 8 == 0 && src_pitch % 8 == 0 && dst_pitch % 8 == 0 && dst_off % 8 == 0 &&
                    ((uintptr_t)src % 16 == 0) && ((uintptr_t)dst % 16 == 0)) ? 8 : 1;
-  B200_CUDA(b200::launch_pdl(copy_channels_kernel, grid_for(rows * (C / vec)), 256, 0, stream, reinterpret_cast<const h16*>(src), C, src_pitch,
+  B200_CUDA(b200::launch_kernel(copy_channels_kernel, grid_for(rows * (C / vec)), 256, 0, stream, reinterpret_cast<const h16*>(src), C, src_pitch,
                                                                      reinterpret_cast<h16*>(dst), dst_pitch, dst_off, rows, vec));
   B200_LAUNCH_CHECK("copy_channels_kernel");
   return B200_OK;
@@ -1269,7 +1241,7 @@ extern "C" int b200_geglu(const void* x, int64_t M, int32_t H, int32_t x_pitch, 
   cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
   B200_CHECK_ARG(x && y && H % 8 == 0 && x_pitch % 8 == 0 && y_pitch % 8 == 0 && x_pitch >= 2 * H && y_pitch >= H,
                  "geglu: bad arguments");
-  B200_CUDA(b200::launch_pdl(geglu_kernel, grid_for(M * (H / 8)), 256, 0, stream, reinterpret_cast<const h16*>(x), M, H, x_pitch,
+  B200_CUDA(b200::launch_kernel(geglu_kernel, grid_for(M * (H / 8)), 256, 0, stream, reinterpret_cast<const h16*>(x), M, H, x_pitch,
                                                          reinterpret_cast<h16*>(y), y_pitch));
   B200_LAUNCH_CHECK("geglu_kernel");
   return B200_OK;
@@ -1283,10 +1255,10 @@ extern "C" int b200_softmax_rows(const float* s, int64_t M, int32_t S, int64_t s
   if (S <= 1024) {
     const long long blocks = (M + 7) / 8;
     B200_CHECK_ARG(blocks < (1ll << 31), "softmax_rows: too many rows");
-    B200_CUDA(b200::launch_pdl(softmax_rows_kernel<32>, (unsigned)blocks, 256, 0, stream, s, M, S, s_pitch, pp, p_pitch));
+    B200_CUDA(b200::launch_kernel(softmax_rows_kernel<32>, (unsigned)blocks, 256, 0, stream, s, M, S, s_pitch, pp, p_pitch));
   } else {
     B200_CHECK_ARG(M < (1ll << 31), "softmax_rows: too many rows");
-    B200_CUDA(b200::launch_pdl(softmax_rows_kernel<256>, (unsigned)M, 256, 0, stream, s, M, S, s_pitch, pp, p_pitch));
+    B200_CUDA(b200::launch_kernel(softmax_rows_kernel<256>, (unsigned)M, 256, 0, stream, s, M, S, s_pitch, pp, p_pitch));
   }
   B200_LAUNCH_CHECK("softmax_rows_kernel");
   return B200_OK;
@@ -1297,7 +1269,7 @@ extern "C" int b200_softmax_rows_partials(const float* s, int64_t M, int32_t S, 
   cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
   B200_CHECK_ARG(s && p && partials && M >= 1 && M < (1ll << 31) && S >= 1 && s_pitch >= S && p_pitch >= S && n_tiles >= 1,
                  "softmax_rows_partials: bad arguments");
-  B200_CUDA(b200::launch_pdl(softmax_rows_partials_kernel, (unsigned)M, 256, 0, stream, s, S, s_pitch, reinterpret_cast<const float2*>(partials),
+  B200_CUDA(b200::launch_kernel(softmax_rows_partials_kernel, (unsigned)M, 256, 0, stream, s, S, s_pitch, reinterpret_cast<const float2*>(partials),
                                                                n_tiles, reinterpret_cast<h16*>(p), p_pitch));
   B200_LAUNCH_CHECK("softmax_rows_partials_kernel");
   return B200_OK;
@@ -1307,7 +1279,7 @@ extern "C" int b200_timestep_embedding(const float* t, int32_t N, int32_t dim, f
                                        void* stream_v) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
   B200_CHECK_ARG(t && emb && N >= 1 && dim >= 1, "timestep_embedding: bad arguments");
-  B200_CUDA(b200::launch_pdl(timestep_embedding_kernel, (N * dim + 255) / 256, 256, 0, stream, t, N, dim, max_period, emb));
+  B200_CUDA(b200::launch_kernel(timestep_embedding_kernel, (N * dim + 255) / 256, 256, 0, stream, t, N, dim, max_period, emb));
   B200_LAUNCH_CHECK("timestep_embedding_kernel");
   return B200_OK;
 }
@@ -1317,8 +1289,8 @@ extern "C" int b200_small_linear(const float* x, int32_t M, int32_t K, const flo
   cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
   B200_CHECK_ARG(x && W && y && M >= 1 && M <= 4096 && K >= 1 && O >= 1, "small_linear: bad arguments");
   const bool vec = (K % 128 == 0) && (((uintptr_t)x | (uintptr_t)W) & 15) == 0;
-  if (vec) B200_CUDA(b200::launch_pdl(small_linear_kernel<true>, (O + 7) / 8, 256, 0, stream, x, M, K, W, b, O, act_in, act_out, y));
-  else B200_CUDA(b200::launch_pdl(small_linear_kernel<false>, (O + 7) / 8, 256, 0, stream, x, M, K, W, b, O, act_in, act_out, y));
+  if (vec) B200_CUDA(b200::launch_kernel(small_linear_kernel<true>, (O + 7) / 8, 256, 0, stream, x, M, K, W, b, O, act_in, act_out, y));
+  else B200_CUDA(b200::launch_kernel(small_linear_kernel<false>, (O + 7) / 8, 256, 0, stream, x, M, K, W, b, O, act_in, act_out, y));
   B200_LAUNCH_CHECK("small_linear_kernel");
   return B200_OK;
 }
@@ -1328,8 +1300,8 @@ extern "C" int b200_ddim_step(const float* model_out, const float* sample, const
   cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
   B200_CHECK_ARG(model_out && sample && c && prev_sample && n >= 1, "ddim_step: bad arguments");
   const bool vec = (((uintptr_t)model_out | (uintptr_t)sample | (uintptr_t)noise | (uintptr_t)prev_sample | (uintptr_t)pred_x0) & 15) == 0;
-  if (vec) B200_CUDA(b200::launch_pdl(ddim_step_kernel<1>, grid_for((n + 7) / 8, 256, 16), 256, 0, stream, model_out, sample, noise, *c, prev_sample, pred_x0, (long long)n));
-  else B200_CUDA(b200::launch_pdl(ddim_step_kernel<0>, grid_for(n), 256, 0, stream, model_out, sample, noise, *c, prev_sample, pred_x0, (long long)n));
+  if (vec) B200_CUDA(b200::launch_kernel(ddim_step_kernel<1>, grid_for((n + 7) / 8, 256, 16), 256, 0, stream, model_out, sample, noise, *c, prev_sample, pred_x0, (long long)n));
+  else B200_CUDA(b200::launch_kernel(ddim_step_kernel<0>, grid_for(n), 256, 0, stream, model_out, sample, noise, *c, prev_sample, pred_x0, (long long)n));
   B200_LAUNCH_CHECK("ddim_step_kernel");
   return B200_OK;
 }
@@ -1339,7 +1311,7 @@ extern "C" int b200_ddpm_step(const float* model_out, const float* sample, const
   cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
   B200_CHECK_ARG(model_out && sample && c && prev_sample && n >= 1, "ddpm_step: bad arguments");
   B200_CHECK_ARG(c->var_mode == 0 || pred_var, "ddpm_step: learned variance needs pred_var");
-  B200_CUDA(b200::launch_pdl(ddpm_step_kernel, grid_for(n), 256, 0, stream, model_out, sample, noise, pred_var, *c, prev_sample, pred_x0, n));
+  B200_CUDA(b200::launch_kernel(ddpm_step_kernel, grid_for(n), 256, 0, stream, model_out, sample, noise, pred_var, *c, prev_sample, pred_x0, n));
   B200_LAUNCH_CHECK("ddpm_step_kernel");
   return B200_OK;
 }
@@ -1352,7 +1324,7 @@ extern "C" int b200_pndm_step(const float* const* hist, const float* sample, con
   PndmPtrs hp;
   for (int k = 0; k < 4; ++k) hp.h[k] = k < c->n_hist ? hist[k] : nullptr;
   for (int k = 0; k < c->n_hist; ++k) B200_CHECK_ARG(hp.h[k], "pndm_step: null history tensor %d", k);
-  B200_CUDA(b200::launch_pdl(pndm_step_kernel, grid_for(n), 256, 0, stream, hp, sample, *c, prev_sample, eps_out, n));
+  B200_CUDA(b200::launch_kernel(pndm_step_kernel, grid_for(n), 256, 0, stream, hp, sample, *c, prev_sample, eps_out, n));
   B200_LAUNCH_CHECK("pndm_step_kernel");
   return B200_OK;
 }
@@ -1362,7 +1334,7 @@ extern "C" int b200_add_noise(const float* x0, const float* noise, const float* 
   cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
   B200_CHECK_ARG(x0 && noise && ca && cb && out && N >= 1 && N <= 65535 && per_sample >= 1, "add_noise: bad arguments");
   dim3 grid(grid_for(per_sample, 256, 4), N);
-  B200_CUDA(b200::launch_pdl(add_noise_kernel, grid, 256, 0, stream, x0, noise, ca, cb, sign_b, per_sample, out));
+  B200_CUDA(b200::launch_kernel(add_noise_kernel, grid, 256, 0, stream, x0, noise, ca, cb, sign_b, per_sample, out));
   B200_LAUNCH_CHECK("add_noise_kernel");
   return B200_OK;
 }
@@ -1370,7 +1342,7 @@ extern "C" int b200_add_noise(const float* x0, const float* noise, const float* 
 extern "C" int b200_exp_half_clamped(const float* log_var, float lo, float hi, float* sigma, int64_t n, void* stream_v) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
   B200_CHECK_ARG(log_var && sigma && n >= 1, "exp_half_clamped: bad arguments");
-  B200_CUDA(b200::launch_pdl(exp_half_clamped_kernel, grid_for(n), 256, 0, stream, log_var, lo, hi, sigma, n));
+  B200_CUDA(b200::launch_kernel(exp_half_clamped_kernel, grid_for(n), 256, 0, stream, log_var, lo, hi, sigma, n));
   B200_LAUNCH_CHECK("exp_half_clamped_kernel");
   return B200_OK;
 }
@@ -1378,7 +1350,7 @@ extern "C" int b200_exp_half_clamped(const float* log_var, float lo, float hi, f
 extern "C" int b200_fma_f32(const float* a, const float* b, const float* c, float* out, int64_t n, void* stream_v) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
   B200_CHECK_ARG(a && b && c && out && n >= 1, "fma_f32: bad arguments");
-  B200_CUDA(b200::launch_pdl(fma_f32_kernel, grid_for(n), 256, 0, stream, a, b, c, out, n));
+  B200_CUDA(b200::launch_kernel(fma_f32_kernel, grid_for(n), 256, 0, stream, a, b, c, out, n));
   B200_LAUNCH_CHECK("fma_f32_kernel");
   return B200_OK;
 }
@@ -1386,7 +1358,7 @@ extern "C" int b200_fma_f32(const float* a, const float* b, const float* c, floa
 extern "C" int b200_scale_f32(const float* x, float mul, float div, float* out, int64_t n, void* stream_v) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
   B200_CHECK_ARG(x && out && n >= 1 && div != 0.f, "scale_f32: bad arguments");
-  B200_CUDA(b200::launch_pdl(scale_f32_kernel, grid_for(n), 256, 0, stream, x, mul, div, out, n));
+  B200_CUDA(b200::launch_kernel(scale_f32_kernel, grid_for(n), 256, 0, stream, x, mul, div, out, n));
   B200_LAUNCH_CHECK("scale_f32_kernel");
   return B200_OK;
 }
@@ -1396,7 +1368,7 @@ extern "C" int b200_ddpm_kl(const float* x0, const float* xt, const float* model
   cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
   B200_CHECK_ARG(x0 && xt && model_out && c && sample_sum && N >= 1 && N <= 65535 && per_sample >= 1, "ddpm_kl: bad arguments");
   dim3 grid(grid_for(per_sample, 256, 4), N);
-  B200_CUDA(b200::launch_pdl(ddpm_kl_kernel, grid, 256, 0, stream, x0, xt, model_out, *c, kl_out, sample_sum, per_sample));
+  B200_CUDA(b200::launch_kernel(ddpm_kl_kernel, grid, 256, 0, stream, x0, xt, model_out, *c, kl_out, sample_sum, per_sample));
   B200_LAUNCH_CHECK("ddpm_kl_kernel");
   return B200_OK;
 }

@@ -78,7 +78,6 @@ __global__ void __launch_bounds__(kThreads, 1) flash_attn_kernel(const __grid_co
   const int qc = h * p.dh;                  // first channel of this head
   const int vc = qc;                        // first output channel
 
-  pdl_launch_dependents();
   if (tid == 0) {
     mbar_init(q_bar, 1);
     mbar_init(k_bar, 1);
@@ -87,7 +86,6 @@ __global__ void __launch_bounds__(kThreads, 1) flash_attn_kernel(const __grid_co
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
   }
   __syncthreads();
-  pdl_wait();
   if (tid == 0) {
     mbar_arrive_expect_tx(q_bar, DCH * kChunkBytes);
     for (int c = 0; c < DCH; ++c) tma_load_3d(&p.tmQ, q_bar, q_base + c * kChunkBytes, qc + 64 * c, q0, b);
@@ -265,7 +263,6 @@ __global__ void __launch_bounds__(d512::kThreads, 1) flash_attn_d512_kernel(cons
   const int q0 = (rows_valid ? qt : p.q_tiles - 1) * kBM;
   const int qc = h * 512;
 
-  pdl_launch_dependents();
   if (tid == 0) {
     mbar_init(q_bar, 1);
     for (int s = 0; s < kRing; ++s) {
@@ -275,7 +272,6 @@ __global__ void __launch_bounds__(d512::kThreads, 1) flash_attn_d512_kernel(cons
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   cluster_sync();                             // both CTAs' barriers exist before any multicast or remote arrival
-  pdl_wait();
 
   if (wg == 0) {
     // ---------------------------------------------------------------- producer
@@ -503,7 +499,7 @@ static int launch(const FlashDev& d, cudaStream_t stream) {
     attr_rc = cudaFuncSetAttribute(flash_attn_kernel<DCH>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
   });
   B200_CUDA(attr_rc);
-  B200_CUDA(b200::launch_pdl(flash_attn_kernel<DCH>, d.n_items, kThreads, smem, stream, d));
+  B200_CUDA(b200::launch_kernel(flash_attn_kernel<DCH>, d.n_items, kThreads, smem, stream, d));
   B200_LAUNCH_CHECK("flash_attn_kernel");
   return B200_OK;
 }
@@ -516,8 +512,7 @@ static int launch_d512(const FlashDev& d, cudaStream_t stream) {
     attr_rc = cudaFuncSetAttribute(flash_attn_d512_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, d512::kSmem);
   });
   B200_CUDA(attr_rc);
-  B200_CUDA(b200::launch_cluster(flash_attn_d512_kernel, d512::kCluster, d.n_items, d512::kThreads, d512::kSmem,
-                                 stream, d));
+  B200_CUDA(b200::launch_kernel<d512::kCluster>(flash_attn_d512_kernel, d.n_items, d512::kThreads, d512::kSmem, stream, d));
   B200_LAUNCH_CHECK("flash_attn_d512_kernel");
   return B200_OK;
 }

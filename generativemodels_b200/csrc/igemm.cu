@@ -23,7 +23,6 @@
 #include <cuda.h>
 #include <cudaTypedefs.h>
 #include <mutex>
-#include <stdlib.h>
 #include <string.h>
 
 namespace b200 {
@@ -58,14 +57,8 @@ struct IgemmDev {
   int N, OD, OH, OW;
   int BW, BH, BD, bw_log2, bh_log2;
   int tiles_w, tiles_h, tiles_d, tiles_n, num_tiles;
-  int pdl_late;             // programmatic dependent launch: trigger after the last operand load instead of at entry
   int k_splits;             // >= 1: the reduction of every tile is cut into this many chunk ranges (fastest tile index)
   long long split_stride;   // output elements between the partial results of consecutive ranges
-  // one-launch split-K: fp32 partials [k_splits][split_rows][ws_cols] + per-output-tile tickets (see the epilogue)
-  float* split_ws;
-  int* split_counters;
-  long long split_rows;
-  int ws_cols;
   // epilogue
   void* out_ptr;
   int out_dtype, cout, out_cols, out_vec, out_staged, out_v256;
@@ -79,7 +72,6 @@ struct IgemmDev {
   long long rowvec_bstride;
   const float* row_bias;
   int act1, act2;
-  int bias_prefetch;        // the next tile's bias / row vector is requested during this tile's epilogue
   int geglu;                // act1 was B200_ACT_GEGLU: [32 a | 32 gate] column groups -> a * gelu(gate), cout / 2 output channels
   float scale;
   const void* res_ptr;
@@ -420,7 +412,6 @@ __global__ void __launch_bounds__(kThreads, 1) igemm_tc_kernel(const __grid_cons
   constexpr int kAccLd = BN + 4;          // padded fp32 row: row-per-thread 16-byte reads are conflict-free
   constexpr int CH = (BN >= 32) ? 32 : 16;
 
-  if (!p.pdl_late) pdl_launch_dependents();   // the next kernel's prologue may overlap this kernel (it blocks in its own pdl_wait)
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t acc_base = smem_base + STAGES * kStageBytes;
@@ -449,7 +440,6 @@ __global__ void __launch_bounds__(kThreads, 1) igemm_tc_kernel(const __grid_cons
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
   }
   __syncthreads();
-  pdl_wait();                       // barriers are set up: now wait for the producer of our inputs
 
   const int num_k = p.num_k_chunks;
   // work-unit index -> (k-split, column tile, spatial tile, sample)
@@ -496,7 +486,6 @@ __global__ void __launch_bounds__(kThreads, 1) igemm_tc_kernel(const __grid_cons
           }
         }
       }
-      if (p.pdl_late) pdl_launch_dependents();     // every operand load of this CTA is issued
     }
   } else if (warp >= kMmaWarp0) {
     // ============================== MMA warpgroups ==============================
@@ -588,120 +577,7 @@ __global__ void __launch_bounds__(kThreads, 1) igemm_tc_kernel(const __grid_cons
       const int nb = ti.nb;
       const int ow = wt * p.BW + rw, oh = ht * p.BH + rh, od = dt * p.BD + rd;
       const bool row_ok = (ow < p.OW) && (oh < p.OH) && (od < p.OD);
-      const long long out_off = nb * p.out_sN + od * p.out_sD + oh * p.out_sH + ow * p.out_sW + ks * p.split_stride;
-      const long long res_off = nb * p.res_sN + od * p.res_sD + oh * p.res_sH + ow * p.res_sW;
       const int n0 = nt * BN;
-
-      {
-        if (p.split_counters) {
-          // ---- one-launch split-K: this range's raw accumulators go to the workspace; the CTA that draws the last
-          //      ticket of the output tile sums the ranges in order and applies the call's epilogue ----
-          mbar_wait(tfull_bar, it & 1);
-          const long long lin_row = (((long long)nb * p.OD + od) * p.OH + oh) * p.OW + ow;
-          float* wrow = p.split_ws + ((long long)ks * p.split_rows + lin_row) * p.ws_cols;
-#pragma unroll 1
-          for (int c0 = 0; c0 < BN; c0 += CH) {
-            if (n0 + c0 >= p.ws_cols) break;             // warp-uniform
-            uint32_t raw[CH];
-            acc_ld<CH>(acc_row + c0, raw);
-            if (row_ok) {
-#pragma unroll
-              for (int g = 0; g < CH / 4; ++g)
-                if (n0 + c0 + g * 4 < p.ws_cols)
-                  *reinterpret_cast<float4*>(wrow + n0 + c0 + g * 4) =
-                      make_float4(__uint_as_float(raw[g * 4]), __uint_as_float(raw[g * 4 + 1]),
-                                  __uint_as_float(raw[g * 4 + 2]), __uint_as_float(raw[g * 4 + 3]));
-            }
-          }
-          __syncwarp();
-          if (lane == 0) mbar_arrive(tempty_bar);                // the accumulator buffer may be refilled
-          // ---- cooperative reduction: every CTA of the output tile draws a ticket once its partial rows are visible,
-          //      waits until all k_splits tickets are drawn (the k_splits CTAs of a tile are distinct CTAs of one wave:
-          //      the grid never exceeds one CTA per SM, and a CTA only ever waits for CTAs working on lower or equal
-          //      tile indices, so the wait cannot cycle), then sums ITS share of the tile's rows in range order —
-          //      threads run along the columns, so the fp32 partials are read as contiguous 32-byte pieces — and
-          //      applies the call's epilogue.  The CTA that draws ticket 2 * k_splits - 1 leaves the counter at zero.
-          const int out_tile = tile / p.k_splits;
-          int* counter = p.split_counters + out_tile;
-          __threadfence();                                        // this thread's partial rows are visible device-wide
-          asm volatile("bar.sync 1, 128;" ::: "memory");          // ... and so are the other 127 epilogue threads'
-          if (warp == 0 && lane == 0) {
-            atomicAdd(counter, 1);
-            int seen;
-            do {
-              asm volatile("ld.acquire.gpu.global.s32 %0, [%1];" : "=r"(seen) : "l"(counter) : "memory");
-            } while (seen < p.k_splits);
-          }
-          asm volatile("bar.sync 1, 128;" ::: "memory");
-          __threadfence();
-          {
-            const int et = warp * 32 + lane;                      // 0..127 (warps 0..3)
-            const int r_begin = split_begin(kBM, p.k_splits, ks), r_end = split_begin(kBM, p.k_splits, ks + 1);
-            int ncols = p.out_cols - n0;
-            if (ncols > BN) ncols = BN;
-            const int ncg = (ncols + 7) >> 3;
-            const int items = (r_end - r_begin) * ncg;
-            for (int item = et; item < items; item += 128) {
-              const int rr = r_begin + item / ncg;
-              const int col0 = n0 + (item % ncg) * 8;
-              const int ow2 = wt * p.BW + (rr & (p.BW - 1));
-              const int oh2 = ht * p.BH + ((rr >> p.bw_log2) & (p.BH - 1));
-              const int od2 = dt * p.BD + (rr >> (p.bw_log2 + p.bh_log2));
-              if (ow2 >= p.OW || oh2 >= p.OH || od2 >= p.OD) continue;
-              const long long lin2 = (((long long)nb * p.OD + od2) * p.OH + oh2) * p.OW + ow2;
-              const float* src = p.split_ws + lin2 * p.ws_cols + col0;
-              float v[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-              const long long sstride = p.split_rows * p.ws_cols;
-              int s = 0;
-              // eight ranges' loads in flight per thread (one SM reads the whole share: a serial load -> add chain of
-              // up to 32 L2 round trips per item was the 4-20 % this form first lost to the separate reduction kernel);
-              // the additions stay in range order
-              for (; s + 8 <= p.k_splits; s += 8, src += 8 * sstride) {
-                float4 a[8], b[8];
-#pragma unroll
-                for (int j = 0; j < 8; ++j) {
-                  a[j] = __ldcg(reinterpret_cast<const float4*>(src + j * sstride));
-                  b[j] = __ldcg(reinterpret_cast<const float4*>(src + j * sstride + 4));
-                }
-#pragma unroll
-                for (int j = 0; j < 8; ++j) {
-                  v[0] += a[j].x; v[1] += a[j].y; v[2] += a[j].z; v[3] += a[j].w;
-                  v[4] += b[j].x; v[5] += b[j].y; v[6] += b[j].z; v[7] += b[j].w;
-                }
-              }
-              if (s + 4 <= p.k_splits) {
-                float4 a[4], b[4];
-#pragma unroll
-                for (int j = 0; j < 4; ++j) {
-                  a[j] = __ldcg(reinterpret_cast<const float4*>(src + j * sstride));
-                  b[j] = __ldcg(reinterpret_cast<const float4*>(src + j * sstride + 4));
-                }
-#pragma unroll
-                for (int j = 0; j < 4; ++j) {
-                  v[0] += a[j].x; v[1] += a[j].y; v[2] += a[j].z; v[3] += a[j].w;
-                  v[4] += b[j].x; v[5] += b[j].y; v[6] += b[j].z; v[7] += b[j].w;
-                }
-                s += 4; src += 4 * sstride;
-              }
-              for (; s < p.k_splits; ++s, src += sstride) {
-                const float4 a = __ldcg(reinterpret_cast<const float4*>(src));
-                const float4 b = __ldcg(reinterpret_cast<const float4*>(src + 4));
-                v[0] += a.x; v[1] += a.y; v[2] += a.z; v[3] += a.w;
-                v[4] += b.x; v[5] += b.y; v[6] += b.z; v[7] += b.w;
-              }
-              const long long out2 = nb * p.out_sN + od2 * p.out_sD + oh2 * p.out_sH + ow2 * p.out_sW;
-              const long long res2 = nb * p.res_sN + od2 * p.res_sD + oh2 * p.res_sH + ow2 * p.res_sW;
-              epilogue_math<8>(p, v, nb, ow2, res2, col0);
-              store_direct<8>(p, v, out2, col0);
-            }
-          }
-          asm volatile("bar.sync 1, 128;" ::: "memory");          // every thread is done reading the partials
-          if (warp == 0 && lane == 0) {
-            if (atomicAdd(counter, 1) == 2 * p.k_splits - 1) *counter = 0;     // leave the tickets zero for the next call
-          }
-          continue;
-        }
-      }
 
       constexpr int PER = (BN + 31) / 32;
       if (fast_ok && add_key != nb * p.tiles_n + nt && next_key == nb * p.tiles_n + nt) {
@@ -737,7 +613,7 @@ __global__ void __launch_bounds__(kThreads, 1) igemm_tc_kernel(const __grid_cons
       // exposed L2 round trip per tile otherwise)
       float nbv[PER], nrw[PER];
       int want_key = -1;
-      if (fast_ok && p.bias_prefetch && tile + n_workers < p.num_tiles) {
+      if (fast_ok && tile + n_workers < p.num_tiles) {
         const TileIdx tn = decode_tile(tile + n_workers);
         if (tn.nb < p.N && tn.nb * p.tiles_n + tn.nt != add_key) {
           want_key = tn.nb * p.tiles_n + tn.nt;
@@ -754,11 +630,15 @@ __global__ void __launch_bounds__(kThreads, 1) igemm_tc_kernel(const __grid_cons
       // residual of the first full chunk: in flight while this warp waits for the accumulator; every later chunk's
       // residual is requested one chunk ahead (a load -> use chain per chunk exposed one HBM / L2 latency per 32
       // columns: the epilogue warps are one per scheduler, nothing else hides it)
+      const long long res_off = nb * p.res_sN + od * p.res_sD + oh * p.res_sH + ow * p.res_sW;
       const bool res_fast = fast_ok && p.res_ptr && row_ok;
       uint4 rv_next[CH / 8];
       if (res_fast && n0 + CH <= p.cout) load_res_fast<CH>(p, rv_next, res_off, n0);
 
       mbar_wait(tfull_bar, it & 1);
+      // out_off (like res_off above) is formed next to its first use: held across the wait and the vector refresh, the
+      // two pushed the 32-column instantiation into per-tile spills at the 128-register cap
+      const long long out_off = nb * p.out_sN + od * p.out_sD + oh * p.out_sH + ow * p.out_sW + ks * p.split_stride;
       float run_max = -INFINITY, run_sum = 0.f;
       float* my_tile = stage_tiles + warp * (32 * (CH + 1));
       int c0 = 0;
@@ -996,7 +876,6 @@ __device__ __forceinline__ float gn_reduce16(const float* gs, int lane, int gn_s
 // p.num_tiles is the number of units: ceil(M tiles / 2) x column tiles.
 __global__ void __launch_bounds__(wide::kThreads, 1) igemm_wide_kernel(const __grid_constant__ IgemmDev p) {
   using namespace wide;
-  if (!p.pdl_late) pdl_launch_dependents();
   extern __shared__ uint8_t smem_raw[];
   uint8_t* sm = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   const uint32_t ring = smem_u32(sm);
@@ -1020,7 +899,6 @@ __global__ void __launch_bounds__(wide::kThreads, 1) igemm_wide_kernel(const __g
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   cluster_sync();                   // both CTAs' barriers exist before any multicast or remote arrival
-  pdl_wait();
 
   // unit u -> column tile u % tiles_n and M tile 2 (u / tiles_n) + rank (column tile fastest: neighbouring units share
   // their A halos in L2).  The partner of an odd last M tile loads a valid tile, runs the whole protocol, stores nothing.
@@ -1063,7 +941,6 @@ __global__ void __launch_bounds__(wide::kThreads, 1) igemm_wide_kernel(const __g
           }
         }
       }
-      if (p.pdl_late) pdl_launch_dependents();     // every operand load of this CTA is issued
     }
   } else {
     // ============================== consumers ==============================
@@ -1197,7 +1074,6 @@ __global__ void __launch_bounds__(wide::kThreads, 1) igemm_wide_kernel(const __g
 // One thread per (output voxel, 16-column group).  Used by tests and for debugging only.
 // ------------------------------------------------------------------------------------------------
 __global__ void igemm_check_kernel(const __grid_constant__ IgemmDev p) {
-  pdl_entry();
   const long long rows = (long long)p.N * p.OD * p.OH * p.OW;
   const int col_groups = (p.out_cols + 15) / 16;
   const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -1287,7 +1163,6 @@ static TileShape choose_tile(int OW, int OH, int OD, int sw, int sh, int sd) {
 // GroupNorm partials for the cross-check implementation: (sum, sumsq) of the stored bf16 outputs per 8-channel
 // group, accumulated into slot gn_slot0 (fp32 atomics: test path only).
 __global__ void gn8_partial_check_kernel(const __grid_constant__ IgemmDev p) {
-  pdl_entry();
   const long long rows = (long long)p.N * p.OD * p.OH * p.OW;
   const int gw = 1 << p.gn_sh;                      // channels per partial group (8 or 4)
   const int groups = p.cout >> p.gn_sh;
@@ -1313,7 +1188,6 @@ __global__ void gn8_partial_check_kernel(const __grid_constant__ IgemmDev p) {
 // one-pass kernels use.
 __global__ void __launch_bounds__(256) igemm_split_reduce_kernel(const IgemmDev p, const float* __restrict__ ws,
                                                                  int splits, int ws_cols, long long ws_stride) {
-  pdl_entry();
   const int groups = (p.out_cols + 7) >> 3;
   const long long rows = (long long)p.N * p.OD * p.OH * p.OW;
   const long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x;
@@ -1387,15 +1261,6 @@ struct Plan {
   bool wide;                         // igemm_wide_kernel (BN = 256)
 };
 
-static int env_impl() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("B200_IGEMM_IMPL");
-    v = (e && strcmp(e, "check") == 0) ? 1 : 0;
-  }
-  return v;
-}
-
 // The calls igemm_wide_kernel can compute: its epilogue is the vectorised 16-bit one with every column real.
 static bool wide_fits(const b200_igemm_params* p) {
   auto v8 = [](long long a, long long b, long long c, long long d) { return a % 8 == 0 && b % 8 == 0 && c % 8 == 0 && d % 8 == 0; };
@@ -1408,21 +1273,13 @@ static bool wide_fits(const b200_igemm_params* p) {
 // Reductions shorter than this many 64-channel chunks stay on the 128-column kernel, whose epilogue overlaps the next
 // tile's main loop (the wide kernel's consumers run their own epilogue).
 static constexpr int kWideMinChunks = 32;
-// dev knobs (read once): the shortest reduction, in 64-element chunks, for which an under-filled grid narrows its
-// column tile within one wave (B200_NARROW_MIN_CHUNKS, default 4), and the fewest ranges a split reduction must have to be worth its
-// fp32 partials + second kernel (B200_SPLIT_MIN, default 3), and the shortest range, in chunks, a split may leave each
-// CTA (B200_SPLIT_RANGE_MIN, default 32: a split only pays when every range still has ~2 000 elements of reduction to
-// hide its partial stores and the second kernel behind)
-static int env_int(const char* name, int dflt) {
-  const char* e = getenv(name);
-  return (e && *e) ? atoi(e) : dflt;
-}
-static int narrow_min_chunks() { static int v = env_int("B200_NARROW_MIN_CHUNKS", 4); return v; }
-static int bias_prefetch_mode() { static int v = env_int("B200_BIAS_PREFETCH", 1); return v; }
-static int no_v256() { static int v = env_int("B200_NO_V256", 0); return v; }
-static int narrow_one_wave() { static int v = env_int("B200_NARROW_ONE_WAVE", 1); return v; }
-static int split_min() { static int v = env_int("B200_SPLIT_MIN", 3); return v; }
-static int split_range_min() { static int v = env_int("B200_SPLIT_RANGE_MIN", 32); return v < 1 ? 1 : v; }
+// The shortest reduction, in 64-channel chunks, for which an under-filled grid narrows its column tile.
+static constexpr int kNarrowMinChunks = 4;
+// The fewest ranges a split reduction must have to be worth its fp32 partials and second kernel.
+static constexpr int kSplitMin = 3;
+// The shortest range, in chunks, a split may leave each CTA: a split only pays when every range still has ~2 000
+// elements of reduction to hide its partial stores and the second kernel behind.
+static constexpr int kSplitRangeMin = 32;
 static Plan make_plan(const b200_igemm_params* p, bool allow_split, int nsm = 0) {
   if (nsm <= 0) nsm = sm_count();       // nsm > 0: the planning query of a machine of that size (no CUDA call at all)
   Plan pl;
@@ -1438,8 +1295,7 @@ static Plan make_plan(const b200_igemm_params* p, bool allow_split, int nsm = 0)
   pl.ws_bytes = 0;
   // 128 x 256 tiles in clusters of two (impl 3 forces them, impl 2 forbids them): convolutions (>= 8 taps) with a long
   // reduction whose units fill at least one wave of clusters.  GEMM-shaped calls keep the 128-column kernel.
-  const int impl = p->impl ? p->impl : env_impl();
-  pl.wide = wide_fits(p) && (impl == 3 || (impl == 0 && p->n_seg >= 8 && pl.kchunks >= kWideMinChunks &&
+  pl.wide = wide_fits(p) && (p->impl == 3 || (p->impl == 0 && p->n_seg >= 8 && pl.kchunks >= kWideMinChunks &&
                                             ((pl.m_tiles + 1) / 2) * (p->cout / wide::kBN) >= nsm / wide::kCluster));
   if (pl.wide) {
     pl.BN = wide::kBN;
@@ -1459,23 +1315,18 @@ static Plan make_plan(const b200_igemm_params* p, bool allow_split, int nsm = 0)
   if (allow_split && !p->stat_ptr && !p->gn_partial && p->impl != 1 && p->act1 != B200_ACT_GEGLU && pl.kchunks >= 16 &&
       wide_tiles * 2 <= nsm) {
     long long s = nsm / wide_tiles;
-    if (s > pl.kchunks / split_range_min()) s = pl.kchunks / split_range_min();
+    if (s > pl.kchunks / kSplitRangeMin) s = pl.kchunks / kSplitRangeMin;
     if (s > 32) s = 32;
-    if (s >= split_min()) {
+    if (s >= kSplitMin) {
       pl.splits = (int)s;
       pl.ws_bytes = s * pl.rows * pl.ws_cols * 4;
     }
   }
-  // otherwise narrower tiles, down to 64 columns, to put more CTAs on the problem
+  // otherwise narrower tiles, down to 64 columns, to put more CTAs on the problem: halve the column tile while the
+  // narrower tiles still fit ONE wave (a second wave of 64-column tiles streams every A tile four times from L2).  Short
+  // reductions (K = 256 / 384: the transformer linears) are epilogue-bound and narrow the same way.
   if (pl.splits == 1) {
-    if (!narrow_one_wave())   // B200_NARROW_ONE_WAVE=0: narrow while the grid is under-filled, into a second wave
-      while (!p->stat_ptr && BN > 64 && pl.m_tiles * ((cols16 + BN - 1) / BN) < nsm && pl.kchunks >= 8) BN >>= 1;
-    else      // stop at ONE wave: a second wave of 64-column tiles streams every A tile four times from L2
-      while (!p->stat_ptr && BN > 64 && pl.kchunks >= 8 &&
-             pl.m_tiles * ((cols16 + BN / 2 - 1) / (BN / 2)) <= nsm) BN >>= 1;
-    // short reductions (K = 256 / 384: the transformer linears) are epilogue-bound: halve the column tile while the
-    // narrower tiles still fit ONE wave
-    while (!p->stat_ptr && BN > 64 && pl.kchunks >= narrow_min_chunks() && pl.kchunks < 8 &&
+    while (!p->stat_ptr && BN > 64 && pl.kchunks >= kNarrowMinChunks &&
            pl.m_tiles * ((cols16 + BN / 2 - 1) / (BN / 2)) <= nsm) BN >>= 1;
   }
   pl.BN = BN;
@@ -1496,7 +1347,7 @@ static int launch_tc(const IgemmDev& d, cudaStream_t stream) {
   });
   B200_CUDA(attr_rc);
   const int grid = d.num_tiles < sm_count() ? d.num_tiles : sm_count();
-  B200_CUDA(b200::launch_pdl(igemm_tc_kernel<BN, STAGES>, grid, kThreads, smem, stream, d));
+  B200_CUDA(b200::launch_kernel(igemm_tc_kernel<BN, STAGES>, grid, kThreads, smem, stream, d));
   B200_LAUNCH_CHECK("igemm_tc_kernel");
   return B200_OK;
 }
@@ -1526,8 +1377,8 @@ static int launch_wide(const IgemmDev& d, cudaStream_t stream) {
   B200_CUDA(rc);
   if (max_clusters < 1) { set_error("igemm: no cluster of igemm_wide_kernel fits on this device"); return B200_ECUDA; }
   const int clusters = d.num_tiles < max_clusters ? d.num_tiles : max_clusters;
-  B200_CUDA(b200::launch_cluster(igemm_wide_kernel, wide::kCluster, clusters * wide::kCluster, wide::kThreads,
-                                 wide::kSmem, stream, d));
+  B200_CUDA(b200::launch_kernel<wide::kCluster>(igemm_wide_kernel, clusters * wide::kCluster, wide::kThreads,
+                                                wide::kSmem, stream, d));
   B200_LAUNCH_CHECK("igemm_wide_kernel");
   return B200_OK;
 }
@@ -1540,7 +1391,7 @@ extern "C" int64_t b200_igemm_split_workspace_bytes(const b200_igemm_params* p) 
   if (!p || p->n_seg < 1 || p->n_seg > B200_IGEMM_MAX_SEG || p->out_N < 1 || p->out_D < 1 || p->out_H < 1 ||
       p->out_W < 1 || p->out_cols < 1 || p->stride_d < 1 || p->stride_h < 1 || p->stride_w < 1)
     return 0;
-  if ((p->impl ? p->impl : env_impl()) == 1) return 0;
+  if (p->impl == 1) return 0;
   return make_plan(p, true).ws_bytes;
 }
 
@@ -1571,7 +1422,7 @@ extern "C" int b200_igemm(const b200_igemm_params* p, void* stream_v) {
   if (geglu) {
     B200_CHECK_ARG(p->cout % 64 == 0 && p->out_cols == p->cout / 2 && p->out_dtype == B200_DT_H16 && !p->res_ptr &&
                    p->scale == 1.0f && p->act2 == B200_ACT_NONE && !p->stat_ptr && !p->gn_partial && !p->row_bias &&
-                   p->impl != 1 && env_impl() != 1,
+                   p->impl != 1,
                    "igemm: B200_ACT_GEGLU needs cout %% 64 == 0, out_cols == cout / 2, a h16 output and no residual / "
                    "scale / act2 / statistics / row bias (and has no cross-check kernel)");
   }
@@ -1620,19 +1471,16 @@ extern "C" int b200_igemm(const b200_igemm_params* p, void* stream_v) {
   d.bias = p->bias; d.rowvec = p->rowvec; d.rowvec_bstride = p->rowvec_bstride; d.row_bias = p->row_bias;
   d.act1 = geglu ? B200_ACT_NONE : p->act1; d.act2 = p->act2; d.scale = p->scale;
   d.geglu = geglu ? 1 : 0;
-  d.bias_prefetch = bias_prefetch_mode();
   if (geglu) d.out_cols = p->cout;        // the kernel's column loops run over the GEMM's columns
   d.res_ptr = p->res_ptr; d.res_dtype = p->res_dtype;
   d.res_sN = p->res_sN; d.res_sD = p->res_sD; d.res_sH = p->res_sH; d.res_sW = p->res_sW;
   {
     const int g = (p->out_dtype == B200_DT_H16) ? 8 : 4;
-    const int esz = (p->out_dtype == B200_DT_H16) ? 2 : 4;
     d.out_vec = (p->out_cols % g == 0) && (p->out_sN % g == 0) && (p->out_sD % g == 0) &&
                 (p->out_sH % g == 0) && (p->out_sW % g == 0) && (((uintptr_t)p->out_ptr) % 16 == 0);
-    (void)esz;
     d.out_v256 = d.out_vec && p->out_dtype == B200_DT_H16 && (p->out_cols % 16 == 0) && (p->out_sN % 16 == 0) &&
                  (p->out_sD % 16 == 0) && (p->out_sH % 16 == 0) && (p->out_sW % 16 == 0) &&
-                 (((uintptr_t)p->out_ptr) % 32 == 0) && !no_v256();
+                 (((uintptr_t)p->out_ptr) % 32 == 0);
   }
   B200_CHECK_ARG(!geglu || d.out_vec, "igemm: B200_ACT_GEGLU needs a 16-byte-aligned output (out_cols, strides %% 8 == 0)");
   {
@@ -1663,7 +1511,7 @@ extern "C" int b200_igemm(const b200_igemm_params* p, void* stream_v) {
                    "igemm: gn_partial needs a vector-aligned h16 residual");
   }
 
-  const int impl = p->impl ? p->impl : env_impl();
+  const int impl = p->impl;
   B200_CHECK_ARG(impl >= 0 && impl <= 3, "igemm: impl %d not in 0..3", impl);
   B200_CHECK_ARG(impl != 1 || !p->stat_ptr, "igemm: stat_ptr has no cross-check kernel (impl 1)");
   B200_CHECK_ARG(impl != 3 || wide_fits(p),
@@ -1676,11 +1524,11 @@ extern "C" int b200_igemm(const b200_igemm_params* p, void* stream_v) {
     const int threads = 128;
     const long long blocks = (total + threads - 1) / threads;
     B200_CHECK_ARG(blocks < (1ll << 31), "igemm(check): problem too large");
-    B200_CUDA(b200::launch_pdl(igemm_check_kernel, (unsigned)blocks, threads, 0, stream, d));
+    B200_CUDA(b200::launch_kernel(igemm_check_kernel, (unsigned)blocks, threads, 0, stream, d));
     B200_LAUNCH_CHECK("igemm_check_kernel");
     if (d.gn_partial) {
       const long long tot = rows * (d.cout >> d.gn_sh);
-      B200_CUDA(b200::launch_pdl(gn8_partial_check_kernel, (unsigned)((tot + 255) / 256), 256, 0, stream, d));
+      B200_CUDA(b200::launch_kernel(gn8_partial_check_kernel, (unsigned)((tot + 255) / 256), 256, 0, stream, d));
       B200_LAUNCH_CHECK("gn8_partial_check_kernel");
     }
     return B200_OK;
@@ -1697,7 +1545,6 @@ extern "C" int b200_igemm(const b200_igemm_params* p, void* stream_v) {
   const int BN = pl.BN;
   d.tiles_n = pl.tiles_n;
   d.k_splits = 1;
-  d.pdl_late = (b200::pdl_mode() == 2) ? 1 : 0;
   d.split_stride = 0;
   const int splits = (p->split_ws && pl.splits > 1) ? pl.splits : 1;
   if (splits > 1) {
@@ -1760,20 +1607,6 @@ extern "C" int b200_igemm(const b200_igemm_params* p, void* stream_v) {
   };
   if (splits == 1) return launch(d);
 
-  if (p->split_counters) {
-    // ---- one-launch split-K: partials + per-tile tickets; the last CTA of a tile reduces and applies the epilogue ----
-    B200_CHECK_ARG(pl.ntiles <= B200_IGEMM_SPLIT_COUNTERS, "igemm: %lld output tiles exceed the %d split-K tickets",
-                   pl.ntiles, B200_IGEMM_SPLIT_COUNTERS);
-    IgemmDev df = d;
-    df.k_splits = splits;
-    df.num_tiles = (int)(pl.ntiles * splits);
-    df.split_ws = static_cast<float*>(p->split_ws);
-    df.split_counters = p->split_counters;
-    df.split_rows = pl.rows;
-    df.ws_cols = pl.ws_cols;
-    df.split_stride = 0;             // out_off addresses the REAL output in this mode
-    return launch(df);
-  }
   // ---- split-K: S partial GEMMs into the fp32 workspace, then the reduction applies this call's epilogue ----
   IgemmDev ds = d;
   ds.k_splits = splits;
@@ -1791,7 +1624,7 @@ extern "C" int b200_igemm(const b200_igemm_params* p, void* stream_v) {
   if (rc != B200_OK) return rc;
   const long long total = pl.rows * ((d.out_cols + 7) / 8);
   B200_CHECK_ARG((total + 255) / 256 < (1ll << 31), "igemm: split reduction too large");
-  B200_CUDA(b200::launch_pdl(igemm_split_reduce_kernel, (unsigned)((total + 255) / 256), 256, 0, stream, 
+  B200_CUDA(b200::launch_kernel(igemm_split_reduce_kernel, (unsigned)((total + 255) / 256), 256, 0, stream, 
       d, static_cast<const float*>(p->split_ws), splits, pl.ws_cols, ds.split_stride));
   B200_LAUNCH_CHECK("igemm_split_reduce_kernel");
   return B200_OK;

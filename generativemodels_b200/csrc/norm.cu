@@ -23,7 +23,6 @@ template <int VEC>
 __global__ void gn_partial_kernel(const h16* __restrict__ x0, const h16* __restrict__ x1,
                                   int C0, int C1, int pitch0, int pitch1, long long spatial,
                                   long long vox_per_chunk, float* __restrict__ partial) {
-  pdl_entry();
   const int C = C0 + C1;
   const int CV = C / VEC;
   const int rows = blockDim.x / CV;
@@ -100,7 +99,6 @@ __global__ void gn_partial_kernel(const h16* __restrict__ x0, const h16* __restr
 __global__ void gn_finalize_kernel(const float* __restrict__ partial, int chunks, int C, int groups,
                                    long long spatial, float eps, const float* __restrict__ gamma,
                                    const float* __restrict__ beta, float* __restrict__ affine) {
-  pdl_entry();
   const int g = blockIdx.x, n = blockIdx.y;
   const int cpg = C / groups;
   double s = 0.0, q = 0.0;
@@ -164,7 +162,6 @@ __global__ void gn_finalize_partials_kernel(const float* __restrict__ p0, const 
                                             int slots1, int C0, int C1, int sh0, int sh1, int groups, long long spatial,
                                             float eps, const float* __restrict__ gamma, const float* __restrict__ beta,
                                             float* __restrict__ affine) {
-  pdl_entry();
   const int g = blockIdx.x, n = blockIdx.y;
   const int C = C0 + C1;
   const int cpg = C / groups;
@@ -238,7 +235,6 @@ __global__ void gn_apply_kernel(const h16* __restrict__ x0, const h16* __restric
                                 int C0, int C1, int pitch0, int pitch1, long long spatial, long long vox_per_chunk,
                                 const float* __restrict__ affine, int act, h16* __restrict__ y,
                                 int y_pitch) {
-  pdl_entry();
   const int C = C0 + C1;
   const int CV = C / VEC;
   const int rows = blockDim.x / CV;
@@ -354,7 +350,6 @@ __global__ void __launch_bounds__(512) gn_fused_small_kernel(const h16* __restri
                                                              const float* __restrict__ gamma,
                                                              const float* __restrict__ beta, int act,
                                                              h16* __restrict__ y, int y_pitch) {
-  pdl_entry();
   const int g = blockIdx.x, n = blockIdx.y;
   const int C = C0 + C1, cpg = C / groups;
   const int c_first = g * cpg;                       // the host guarantees a group never straddles the two sources
@@ -472,7 +467,6 @@ __global__ void __launch_bounds__(512) gn_fused_small_kernel(const h16* __restri
 
 // zero the pad channels [C, pitch) of a channels-last tensor (only when pitch > C)
 __global__ void zero_pad_channels_kernel(h16* y, long long rows, int C, int pitch) {
-  pdl_entry();
   const int padw = pitch - C;
   const long long total = rows * padw;
   for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < total;
@@ -490,7 +484,6 @@ __global__ void spade_apply_kernel(const h16* __restrict__ x0, const h16* __rest
                                    const float* __restrict__ affine, const h16* __restrict__ gb, int gb_pitch,
                                    const float* __restrict__ gb_affine, int act, h16* __restrict__ y,
                                    int y_pitch) {
-  pdl_entry();
   const int C = C0 + C1;
   const int CV = C / VEC;
   const long long total = (long long)N * spatial * CV;
@@ -528,7 +521,6 @@ __global__ void spade_apply_kernel(const h16* __restrict__ x0, const h16* __rest
 
 __global__ void resize_nearest_kernel(const h16* __restrict__ x, int N, int D, int H, int W, int pitch,
                                       h16* __restrict__ y, int OD, int OH, int OW) {
-  pdl_entry();
   const long long total = (long long)N * OD * OH * OW * pitch;
   const float sd = (float)D / OD, sh = (float)H / OH, sw = (float)W / OW;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total;
@@ -549,7 +541,6 @@ __global__ void resize_nearest_kernel(const h16* __restrict__ x, int N, int D, i
 __global__ void layernorm_kernel(const h16* __restrict__ x, long long M, int C, int x_pitch,
                                  const float* __restrict__ gamma, const float* __restrict__ beta, float eps,
                                  h16* __restrict__ y, int y_pitch) {
-  pdl_entry();
   const long long row = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (row >= M) return;
   const int lane = threadIdx.x & 31;
@@ -578,7 +569,6 @@ template <int VPL>
 __global__ void layernorm_vec_kernel(const h16* __restrict__ x, long long M, int C, int x_pitch,
                                      const float* __restrict__ gamma, const float* __restrict__ beta, float eps,
                                      h16* __restrict__ y, int y_pitch) {
-  pdl_entry();
   const long long row = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (row >= M) return;
   const int lane = threadIdx.x & 31;
@@ -678,11 +668,11 @@ extern "C" int b200_groupnorm_stats(const b200_gn_stats_params* p, void* stream_
   const h16* x0 = reinterpret_cast<const h16*>(p->x_ptr[0]);
   const h16* x1 = reinterpret_cast<const h16*>(p->x_ptr[1]);
   if (vec == 8)
-    B200_CUDA(b200::launch_pdl(gn_partial_kernel<8>, grid, threads, smem, stream, x0, x1, C0, C1, p->x_pitch[0], p->x_pitch[1], p->spatial, vpc, p->partial));
+    B200_CUDA(b200::launch_kernel(gn_partial_kernel<8>, grid, threads, smem, stream, x0, x1, C0, C1, p->x_pitch[0], p->x_pitch[1], p->spatial, vpc, p->partial));
   else
-    B200_CUDA(b200::launch_pdl(gn_partial_kernel<1>, grid, threads, smem, stream, x0, x1, C0, C1, p->x_pitch[0], p->x_pitch[1], p->spatial, vpc, p->partial));
+    B200_CUDA(b200::launch_kernel(gn_partial_kernel<1>, grid, threads, smem, stream, x0, x1, C0, C1, p->x_pitch[0], p->x_pitch[1], p->spatial, vpc, p->partial));
   B200_LAUNCH_CHECK("gn_partial_kernel");
-  B200_CUDA(b200::launch_pdl(gn_finalize_kernel, dim3(p->groups, p->N), 128, 0, stream, p->partial, chunks, C, p->groups, p->spatial, p->eps,
+  B200_CUDA(b200::launch_kernel(gn_finalize_kernel, dim3(p->groups, p->N), 128, 0, stream, p->partial, chunks, C, p->groups, p->spatial, p->eps,
                                                                 p->gamma, p->beta, p->affine));
   B200_LAUNCH_CHECK("gn_finalize_kernel");
   return B200_OK;
@@ -702,7 +692,7 @@ extern "C" int b200_groupnorm_from_partials_ex(const b200_gn_stats_params* p, co
                      (!C1 || slots[1] >= 1),
                  "groupnorm_from_partials: groups of %d channels do not tile the %d / %d-channel partials", cpg, g0, g1);
   dim3 grid(p->groups, p->N);
-  B200_CUDA(b200::launch_pdl(gn_finalize_partials_kernel, grid, 256, 0, stream, partial[0], partial[1], slots[0], C1 ? slots[1] : 0, C0, C1,
+  B200_CUDA(b200::launch_kernel(gn_finalize_partials_kernel, grid, 256, 0, stream, partial[0], partial[1], slots[0], C1 ? slots[1] : 0, C0, C1,
                                                         g0 == 4 ? 2 : 3, g1 == 4 ? 2 : 3, p->groups, p->spatial, p->eps, p->gamma, p->beta,
                                                         p->affine));
   B200_LAUNCH_CHECK("gn_finalize_partials_kernel");
@@ -740,15 +730,15 @@ extern "C" int b200_groupnorm_apply(const b200_gn_apply_params* p, void* stream_
   const h16* x1 = reinterpret_cast<const h16*>(p->x_ptr[1]);
   h16* y = reinterpret_cast<h16*>(p->y_ptr);
   if (vec == 8)
-    B200_CUDA(b200::launch_pdl(gn_apply_kernel<8>, grid, threads, 0, stream, x0, x1, C0, C1, p->x_pitch[0], p->x_pitch[1], p->spatial, vpc, p->affine, p->act, y, p->y_pitch));
+    B200_CUDA(b200::launch_kernel(gn_apply_kernel<8>, grid, threads, 0, stream, x0, x1, C0, C1, p->x_pitch[0], p->x_pitch[1], p->spatial, vpc, p->affine, p->act, y, p->y_pitch));
   else
-    B200_CUDA(b200::launch_pdl(gn_apply_kernel<1>, grid, threads, 0, stream, x0, x1, C0, C1, p->x_pitch[0], p->x_pitch[1], p->spatial, vpc, p->affine, p->act, y, p->y_pitch));
+    B200_CUDA(b200::launch_kernel(gn_apply_kernel<1>, grid, threads, 0, stream, x0, x1, C0, C1, p->x_pitch[0], p->x_pitch[1], p->spatial, vpc, p->affine, p->act, y, p->y_pitch));
   B200_LAUNCH_CHECK("gn_apply_kernel");
   if (p->y_pitch > C) {
     const long long rows = (long long)p->N * p->spatial;
     long long zb = (rows * (p->y_pitch - C) + 255) / 256;
     if (zb > 4ll * sm_count()) zb = 4ll * sm_count();
-    B200_CUDA(b200::launch_pdl(zero_pad_channels_kernel, (unsigned)zb, 256, 0, stream, y, rows, C, p->y_pitch));
+    B200_CUDA(b200::launch_kernel(zero_pad_channels_kernel, (unsigned)zb, 256, 0, stream, y, rows, C, p->y_pitch));
     B200_LAUNCH_CHECK("zero_pad_channels_kernel");
   }
   return B200_OK;
@@ -783,14 +773,14 @@ extern "C" int b200_groupnorm_fused(const b200_gn_stats_params* sp, const b200_g
   h16* y = reinterpret_cast<h16*>(ap->y_ptr);
   dim3 grid(sp->groups, sp->N);
 #define B200_GN_FUSED(V)                                                                                           \
-  B200_CUDA(b200::launch_pdl(gn_fused_small_kernel<V>, grid, 512, 0, stream, x0, x1, C0, C1, sp->x_pitch[0], sp->x_pitch[1], (int)sp->spatial, \
+  B200_CUDA(b200::launch_kernel(gn_fused_small_kernel<V>, grid, 512, 0, stream, x0, x1, C0, C1, sp->x_pitch[0], sp->x_pitch[1], (int)sp->spatial, \
                                                      sp->groups, sp->eps, sp->gamma, sp->beta, ap->act, y, ap->y_pitch))
   if (vec == 8) {
     // rows each thread visits: 512 threads / (cpg / 8) vectors per row
     const int rows_per_iter = 512 / (cpg / 8);
     const long long iters = (sp->spatial + rows_per_iter - 1) / rows_per_iter;
 #define B200_GN_FUSED_K(K)                                                                                          \
-  B200_CUDA(b200::launch_pdl(gn_fused_small_kernel<8, K>, grid, 512, 0, stream, x0, x1, C0, C1, sp->x_pitch[0], sp->x_pitch[1], (int)sp->spatial, \
+  B200_CUDA(b200::launch_kernel(gn_fused_small_kernel<8, K>, grid, 512, 0, stream, x0, x1, C0, C1, sp->x_pitch[0], sp->x_pitch[1], (int)sp->spatial, \
                                                      sp->groups, sp->eps, sp->gamma, sp->beta, ap->act, y, ap->y_pitch))
     if (iters <= 2) B200_GN_FUSED_K(2);
     else if (iters <= 4) B200_GN_FUSED_K(4);
@@ -825,17 +815,17 @@ extern "C" int b200_spade_apply(const b200_gn_apply_params* p, const void* gb, i
   const h16* g = reinterpret_cast<const h16*>(gb);
   h16* y = reinterpret_cast<h16*>(p->y_ptr);
   if (vec)
-    B200_CUDA(b200::launch_pdl(spade_apply_kernel<8>, (unsigned)blocks, 256, 0, stream, x0, x1, C0, C1, p->x_pitch[0], p->x_pitch[1], p->spatial,
+    B200_CUDA(b200::launch_kernel(spade_apply_kernel<8>, (unsigned)blocks, 256, 0, stream, x0, x1, C0, C1, p->x_pitch[0], p->x_pitch[1], p->spatial,
                                                                 p->N, p->affine, g, gb_pitch, gb_affine, p->act, y, p->y_pitch));
   else
-    B200_CUDA(b200::launch_pdl(spade_apply_kernel<1>, (unsigned)blocks, 256, 0, stream, x0, x1, C0, C1, p->x_pitch[0], p->x_pitch[1], p->spatial,
+    B200_CUDA(b200::launch_kernel(spade_apply_kernel<1>, (unsigned)blocks, 256, 0, stream, x0, x1, C0, C1, p->x_pitch[0], p->x_pitch[1], p->spatial,
                                                                 p->N, p->affine, g, gb_pitch, gb_affine, p->act, y, p->y_pitch));
   B200_LAUNCH_CHECK("spade_apply_kernel");
   if (p->y_pitch > C) {
     const long long rows = (long long)p->N * p->spatial;
     long long zb = (rows * (p->y_pitch - C) + 255) / 256;
     if (zb > 4ll * sm_count()) zb = 4ll * sm_count();
-    B200_CUDA(b200::launch_pdl(zero_pad_channels_kernel, (unsigned)zb, 256, 0, stream, y, rows, C, p->y_pitch));
+    B200_CUDA(b200::launch_kernel(zero_pad_channels_kernel, (unsigned)zb, 256, 0, stream, y, rows, C, p->y_pitch));
     B200_LAUNCH_CHECK("zero_pad_channels_kernel");
   }
   return B200_OK;
@@ -849,7 +839,7 @@ extern "C" int b200_resize_nearest(const void* x, int32_t N, int32_t D, int32_t 
   const long long total = (long long)N * OD * OH * OW * pitch;
   long long blocks = (total + 255) / 256;
   if (blocks > 16ll * sm_count()) blocks = 16ll * sm_count();
-  B200_CUDA(b200::launch_pdl(resize_nearest_kernel, (unsigned)blocks, 256, 0, stream, reinterpret_cast<const h16*>(x), N, D, H, W, pitch,
+  B200_CUDA(b200::launch_kernel(resize_nearest_kernel, (unsigned)blocks, 256, 0, stream, reinterpret_cast<const h16*>(x), N, D, H, W, pitch,
                                                              reinterpret_cast<h16*>(y), OD, OH, OW));
   B200_LAUNCH_CHECK("resize_nearest_kernel");
   return B200_OK;
@@ -865,7 +855,7 @@ extern "C" int b200_layernorm(const void* x, int64_t M, int32_t C, int32_t x_pit
   const bool vec = C % 8 == 0 && C <= 2048 && x_pitch % 8 == 0 && y_pitch % 8 == 0 && ((uintptr_t)x % 16 == 0) &&
                    ((uintptr_t)y % 16 == 0) && ((uintptr_t)gamma % 16 == 0) && ((uintptr_t)beta % 16 == 0);
 #define B200_LN_LAUNCH(K)                                                                                              \
-  B200_CUDA(b200::launch_pdl(K, (unsigned)blocks, wpb * 32, 0, stream, reinterpret_cast<const h16*>(x), M, C, x_pitch, \
+  B200_CUDA(b200::launch_kernel(K, (unsigned)blocks, wpb * 32, 0, stream, reinterpret_cast<const h16*>(x), M, C, x_pitch, \
                              gamma, beta, eps, reinterpret_cast<h16*>(y), y_pitch))
   if (!vec) B200_LN_LAUNCH(layernorm_kernel);
   else if (C <= 256) B200_LN_LAUNCH(layernorm_vec_kernel<1>);

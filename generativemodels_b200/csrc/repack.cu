@@ -22,7 +22,6 @@ __device__ __forceinline__ float src_at(const RepackDev& p, int co, int c, int t
 }
 
 __global__ void __launch_bounds__(256) repack_kernel(const __grid_constant__ RepackDev p) {
-  pdl_entry();
   const int groups = p.pitch >> 3;
   const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= (long long)p.rows_pad * groups) return;
@@ -82,7 +81,6 @@ __global__ void __launch_bounds__(256) batchnorm_fold_kernel(const float* __rest
                                                              const float* __restrict__ var, float eps, int cout,
                                                              long long per_out, float* __restrict__ w_out,
                                                              float* __restrict__ b_out) {
-  pdl_entry();
   const long long stride = (long long)gridDim.x * blockDim.x;
   const long long i0 = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   for (long long i = i0; i < (long long)cout * per_out; i += stride)
@@ -131,7 +129,7 @@ extern "C" int b200_repack_weight(const float* src, int32_t cout, int32_t cin, i
   }
   const long long total = (long long)rows_pad * (dst_pitch / 8);
   B200_CHECK_ARG((total + 255) / 256 < (1ll << 31), "repack_weight: weight too large");
-  B200_CUDA(b200::launch_pdl(repack_kernel, (unsigned)((total + 255) / 256), 256, 0, stream, d));
+  B200_CUDA(b200::launch_kernel(repack_kernel, (unsigned)((total + 255) / 256), 256, 0, stream, d));
   B200_LAUNCH_CHECK("repack_kernel");
   return B200_OK;
 }
@@ -145,7 +143,7 @@ extern "C" int b200_batchnorm_fold(const float* w, const float* b, const float* 
                  (long long)per_out);
   const long long blocks = ((long long)cout * per_out + 255) / 256;
   B200_CHECK_ARG(blocks < (1ll << 31), "batchnorm_fold: weight too large");
-  B200_CUDA(b200::launch_pdl(batchnorm_fold_kernel, (unsigned)blocks, 256, 0, stream, w, b, gamma, beta, mean, var, eps,
+  B200_CUDA(b200::launch_kernel(batchnorm_fold_kernel, (unsigned)blocks, 256, 0, stream, w, b, gamma, beta, mean, var, eps,
                              (int)cout, (long long)per_out, w_out, b_out));
   B200_LAUNCH_CHECK("batchnorm_fold_kernel");
   return B200_OK;

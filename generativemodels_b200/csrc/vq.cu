@@ -17,7 +17,6 @@ __global__ void vq_argmin_kernel(const float* __restrict__ x, long long M, int D
                                  const float* __restrict__ cb, int K, long long* __restrict__ idx_out,
                                  h16* __restrict__ q16, int q_pitch, float* __restrict__ q32, int ste,
                                  double* __restrict__ sqerr, int* __restrict__ hist) {
-  pdl_entry();
   extern __shared__ float sm[];
   const int DP = D + 1;                       // padded pitch: lanes hit distinct banks
   float* s_cb = sm;                           // [K][DP]
@@ -91,7 +90,6 @@ __global__ void __launch_bounds__(kVqWarps * 32) vq_argmin_tiled_kernel(
     const float* __restrict__ x, long long M, int x_pitch, const float* __restrict__ cb, int K,
     long long* __restrict__ idx_out, h16* __restrict__ q16, int q_pitch, float* __restrict__ q32, int ste,
     double* __restrict__ sqerr, int* __restrict__ hist) {
-  pdl_entry();
   extern __shared__ float sm[];
   constexpr int DP = DD + 1;
   float* s_cb = sm;                           // [K][DP]
@@ -180,7 +178,6 @@ __global__ void __launch_bounds__(kVqWarps * 32) vq_argmin_tiled_kernel(
 
 __global__ void vq_gather_kernel(const long long* __restrict__ idx, long long M, const float* __restrict__ cb, int K,
                                  int D, h16* __restrict__ q16, int q_pitch) {
-  pdl_entry();
   const long long total = M * q_pitch;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total;
        i += (long long)gridDim.x * blockDim.x) {
@@ -223,7 +220,7 @@ extern "C" int b200_vq_argmin_gather(const float* x, int64_t M, int32_t D, int32
     const long long cap = 2ll * sm_count();
     if (blocks > cap) blocks = cap;
     const size_t smem_t = ((size_t)K * (D + 1) + K) * sizeof(float);
-    B200_CUDA(b200::launch_pdl(vq_argmin_tiled_kernel<32, 4>, (unsigned)blocks, kVqWarps * 32, smem_t, stream, x, (long long)M, x_pitch,
+    B200_CUDA(b200::launch_kernel(vq_argmin_tiled_kernel<32, 4>, (unsigned)blocks, kVqWarps * 32, smem_t, stream, x, (long long)M, x_pitch,
                                codebook, K, reinterpret_cast<long long*>(indices), reinterpret_cast<h16*>(q_h16), q_pitch,
                                q_f32, ste, sqerr_sum, hist));
     B200_LAUNCH_CHECK("vq_argmin_tiled_kernel");
@@ -232,7 +229,7 @@ extern "C" int b200_vq_argmin_gather(const float* x, int64_t M, int32_t D, int32
   long long blocks = (M + kVqWarps - 1) / kVqWarps;
   const long long cap = 2ll * sm_count();
   if (blocks > cap) blocks = cap;
-  B200_CUDA(b200::launch_pdl(vq_argmin_kernel, (unsigned)blocks, kVqWarps * 32, smem, stream,
+  B200_CUDA(b200::launch_kernel(vq_argmin_kernel, (unsigned)blocks, kVqWarps * 32, smem, stream,
       x, (long long)M, D, x_pitch, codebook, K, reinterpret_cast<long long*>(indices), reinterpret_cast<h16*>(q_h16),
       q_pitch, q_f32, ste, sqerr_sum, hist));
   B200_LAUNCH_CHECK("vq_argmin_kernel");
@@ -246,7 +243,7 @@ extern "C" int b200_vq_gather(const int64_t* indices, int64_t M, const float* co
   long long blocks = (M * q_pitch + 255) / 256;
   const long long cap = 8ll * sm_count();
   if (blocks > cap) blocks = cap;
-  B200_CUDA(b200::launch_pdl(vq_gather_kernel, (unsigned)blocks, 256, 0, stream, reinterpret_cast<const long long*>(indices), M, codebook, K, D,
+  B200_CUDA(b200::launch_kernel(vq_gather_kernel, (unsigned)blocks, 256, 0, stream, reinterpret_cast<const long long*>(indices), M, codebook, K, D,
                                                          reinterpret_cast<h16*>(q_h16), q_pitch));
   B200_LAUNCH_CHECK("vq_gather_kernel");
   return B200_OK;

@@ -8,7 +8,6 @@ from __future__ import annotations
 
 import ctypes as C
 import numbers
-import os
 import struct
 import weakref
 from dataclasses import dataclass
@@ -34,7 +33,6 @@ def _stream() -> int:
     return torch.cuda.current_stream().cuda_stream
 
 
-_FORK = os.environ.get("B200_FORK", "1") != "0"
 _SIDE_STREAMS: dict = {}
 
 
@@ -52,7 +50,7 @@ class fork:
     """
 
     def __enter__(self):
-        self.active = _FORK and torch.cuda.is_available() and torch.cuda.is_current_stream_capturing()
+        self.active = torch.cuda.is_available() and torch.cuda.is_current_stream_capturing()
         if self.active:
             self.main = torch.cuda.current_stream()
             idx = self.main.device.index
@@ -460,18 +458,7 @@ def _fill_segs(p: IgemmParams, segs) -> None:
         s.src, s.dw, s.dh, s.dd, s.c0, s.nchunks = src, dw, dh, dd, c0, nch
 
 
-_SPLIT_K = os.environ.get("B200_SPLIT_K", "1") != "0"    # dev switch (tests compare split and one-pass reductions)
-# one launch (per-tile tickets, the CTAs of a tile reduce it cooperatively) instead of GEMM + reduce kernel.  Off by default:
-# B200_SPLIT_FUSED=1 selects the cooperative form for A/B runs.
-_SPLIT_FUSED = os.environ.get("B200_SPLIT_FUSED", "0") != "0"
-_SPLIT_COUNTERS: dict = {}       # device index -> int32 [IGEMM_SPLIT_COUNTERS] zeros (self-resetting tickets)
-
-
-def _split_counters(device: torch.device) -> torch.Tensor:
-    t = _SPLIT_COUNTERS.get(device.index)
-    if t is None:
-        t = _SPLIT_COUNTERS[device.index] = torch.zeros(_lib.IGEMM_SPLIT_COUNTERS, dtype=torch.int32, device=device)
-    return t
+_SPLIT_K = True          # tests and probes set it to False to compare split and one-pass reductions
 _SPLIT_LAUNCHES = 0      # calls that went through the split-K pair of kernels (tests / probes read it)
 
 
@@ -488,12 +475,11 @@ def igemm_raw(p: IgemmParams) -> None:
             dev = torch.device("cuda", torch.cuda.current_device())
             ws = torch.empty(need, dtype=torch.uint8, device=dev)
             p.split_ws, p.split_ws_bytes = ws.data_ptr(), need
-            p.split_counters = _split_counters(dev).data_ptr() if _SPLIT_FUSED else None
     try:
         check(lib.b200_igemm(C.byref(p), _stream()), "b200_igemm")
     finally:
         if ws is not None:       # the struct may be a cached template: never keep the pointers
-            p.split_ws, p.split_ws_bytes, p.split_counters = None, 0, None
+            p.split_ws, p.split_ws_bytes = None, 0
 
 
 def _conv_params(srcs: Sequence[CL], w: torch.Tensor, segs, stride, out_t: torch.Tensor, out_dims, cout: int,
@@ -716,9 +702,9 @@ def groupnorm_affine(srcs: CL | Sequence[CL], groups: int, eps: float, gamma: to
 
 
 # Single-launch GroupNorm for small tensors (b200_groupnorm_fused): one CTA per (sample, group) computes the statistics
-# and applies them — GroupNorm is 138 of the 309 launches of a C2 latent-UNet step as three kernels (the -m gpu suite
-# runs with it on).  B200_GN_SMALL=0 turns it off.
-_GN_SMALL = os.environ.get("B200_GN_SMALL", "1") != "0"
+# and applies them — GroupNorm is 138 of the 309 launches of a C2 latent-UNet step as three kernels.  Tests and probes
+# set _GN_SMALL to False to compare it with the three-kernel path.
+_GN_SMALL = True
 _GN_SMALL_MAX_ELEMS = 1 << 17           # spatial * channels-per-group handled by one CTA
 
 

@@ -148,12 +148,6 @@ typedef struct {
    * unsplit kernel).  NULL / 0 = never split. */
   void*   split_ws;
   int64_t split_ws_bytes;
-  /* Optional: B200_IGEMM_SPLIT_COUNTERS int32 counters, zero before the FIRST call and left zero by every call, not
-   * shared by calls running concurrently on different streams.  With it the split happens in ONE launch: the S CTAs
-   * of an output tile (all resident: the grid never exceeds one CTA per SM) draw a per-tile ticket after storing
-   * their partials, wait for the S-th ticket, and each sums 1/S of the tile's rows in range order and applies the
-   * epilogue — same arithmetic and summation order as the two-kernel form.  NULL = two kernels. */
-  int32_t* split_counters;
   /* 1: the A sources hold ONE sample that every one of the in_N samples reads (the operand-swapped projection
    * V^T[n] = W x[n]^T of a whole batch in one launch: A = the shared weight matrix, the per-sample activations are the
    * batched K-major operand, w_batched = 1).  0: sample n reads A at batch index n. */
@@ -163,15 +157,15 @@ typedef struct {
    * AutoencoderKL). */
   int32_t gn_group;
 } b200_igemm_params;
-#define B200_IGEMM_SPLIT_COUNTERS 256
 
 int b200_igemm(const b200_igemm_params* p, void* stream);
 /* Host-only planning query, no CUDA call: what b200_igemm would choose for this call on a GPU with sm_count SMs —
  * out = {column tile (16..256), split factor (1 = one pass; > 1 only if with_workspace), work items, 0 (reserved)}.
  * The rules (DESIGN.md section 2): a convolution of >= 8 taps with a long reduction, 16-bit output and cout a multiple
  * of 256 whose units fill one wave of two-CTA clusters takes the 256-column kernel (work items = units of two M tiles);
- * otherwise an under-filled grid narrows its column tile while
- * the tiles still fit one wave; a reduction is split only into >= 3 ranges of >= 32 chunks of 64. */
+ * otherwise, given a workspace, a call whose tiles fill at most half the SMs splits its reduction into
+ * min(SMs / tiles, chunks of 64 / 32, 32) ranges when that is >= 3, and an unsplit call of >= 4 chunks halves its
+ * column tile, down to 64, while the narrower tiles still fit one wave.  The rules are fixed: no setting changes them. */
 int b200_igemm_plan(const b200_igemm_params* p, int32_t sm_count, int32_t with_workspace, int32_t out[4]);
 /* Bytes of split_ws with which b200_igemm would split the reduction of this call; 0 when it would not (enough tiles
  * to fill the SMs, short reduction, stat_ptr / gn_partial requested, impl = 1).  Host-only, no launch. */

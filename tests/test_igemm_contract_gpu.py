@@ -9,8 +9,7 @@ device and once with host pointers, runs the library on the first and the emulat
   ignored    A channels [a_C, a_pitch), W columns [w_K, w_pitch) and weight rows between batches hold NaN;
   partials   GroupNorm partials summed over slots equal the float64 (sum, sum of squares) of the kernel's own stored
              output and the emulator's slot; softmax partials equal the max / sum of exp of the kernel's own fp32 row;
-  determinism  a second identical call is bit-identical (except the check kernel's atomic GroupNorm partials), and a
-             one-launch split leaves its tickets at zero;
+  determinism  a second identical call is bit-identical (except the check kernel's atomic GroupNorm partials);
   kernel     b200_igemm_plan's column tile and split factor (256 = the two-CTA wide kernel) are what the case names.
 
 Value bound.  mag = the emulator on |A| and |W| without epilogue (sum |a w| per output).  The fp32 accumulation of
@@ -31,8 +30,7 @@ Case matrix (predicates from generativemodels_b200/csrc/igemm.cu; BN = column ti
   general scalar    out_vec == 0: out_cols % 8 != 0 (h16) or a misaligned out_ptr
   staged            out_staged: fp32 output with out_sW * 4 > 2048
   wide              wide_fits (impl 3)
-  split, 2 kernels  make_plan splits > 1, split_ws, no split_counters -> igemm_split_reduce_kernel
-  split, 1 launch   the same with split_counters (per-tile tickets in igemm_tc_kernel)
+  split, 2 kernels  make_plan splits > 1, split_ws -> igemm_split_reduce_kernel
   check             impl 1: igemm_check_kernel (+ gn8_partial_check_kernel)
 
 Each CASES row names its path; the persistence rows have N = 2 or 3 with more tiles than SMs (128-column kernel) or
@@ -97,7 +95,7 @@ class Case:
     stat: bool = False
     gn: int = 0                   # gn_group: 8 or 4 (0 = no partials)
     impl: int = 2
-    split: str | None = None      # "two" (split_ws) or "one" (split_ws + split_counters)
+    split: str | None = None      # "two" (split_ws)
     huge: bool = False            # bias of +-1e5 on two thirds of the columns: outputs past the fp16 range
 
     @property
@@ -186,8 +184,8 @@ CASES = [
          act1=ACT_SILU, scale=0.5, act2=ACT_TANH, res="h16", rowvec="sample"),
     conv("split_two_kernels_f32_ragged", "split, 2 kernels", (128, 3), 1, (4, 4, 8), [256], 97, out_cols=100,
          w_rows=112, out_f32=True, impl=0, split="two", act1=ACT_GELU, res="f32", res_pad=4),
-    conv("split_one_launch", "split, 1 launch", (128, 3), 2, (4, 4, 8), [256], 96, impl=0, split="one", out_off=1,
-         res="f32", res_off=1, act2=ACT_LEAKYRELU, rowvec="sample"),
+    conv("split_two_kernels_n2_misaligned", "split, 2 kernels", (128, 3), 2, (4, 4, 8), [256], 96, impl=0,
+         split="two", out_off=1, res="f32", res_off=1, act2=ACT_LEAKYRELU, rowvec="sample"),
     # ---- CUDA-core cross-check kernel ----
     conv("check_gn8_res_gelu_silu", "check", None, 2, (1, 9, 11), [64, 48], 64, out_cols=72, w_rows=70, impl=1, gn=8,
          res="h16", act1=ACT_GELU, act2=ACT_SILU, rowvec="sample"),
@@ -203,7 +201,6 @@ SATURATION = [
     conv("sat_general_vector", "general vector", (64, 1), 2, (1, 8, 12), [64], 64, huge=True, res="f32"),
     gemm("sat_general_scalar", "general scalar", (128, 1), 130, 64, 67, out_cols=70, huge=True),
     conv("sat_split_two", "split, 2 kernels", (128, 3), 1, (4, 4, 8), [256], 96, impl=0, split="two", huge=True),
-    conv("sat_split_one", "split, 1 launch", (128, 3), 1, (4, 4, 8), [256], 96, impl=0, split="one", huge=True),
     conv("sat_wide_gn8", "wide", (256, 1), 1, (4, 6, 10), [64], 256, impl=3, huge=True, gn=8),
     conv("sat_check_gn8", "check", None, 1, (1, 8, 12), [64], 64, impl=1, huge=True, gn=8),
 ]
@@ -390,15 +387,10 @@ def launch(lib, c: Case, g: Geom, d, nsm):
         assert need > 0, "the planner does not split this call"
         ws = torch.empty(need, dtype=torch.uint8, device="cuda")
         p.split_ws, p.split_ws_bytes = ws.data_ptr(), need
-        if c.split == "one":
-            p.split_counters = ops._split_counters(torch.device("cuda", torch.cuda.current_device())).data_ptr()
     plan = (C.c_int32 * 4)()
     assert lib.b200_igemm_plan(C.byref(p), nsm, int(c.split is not None), plan) == 0
     rc = lib.b200_igemm(C.byref(p), ops._stream())
     torch.cuda.synchronize()
-    if c.split == "one":
-        counters = ops._split_counters(torch.device("cuda", torch.cuda.current_device()))
-        assert int(counters.abs().sum()) == 0, "the one-launch split left its tickets non-zero"
     return rc, tuple(plan)[:2]
 
 
