@@ -1,9 +1,13 @@
-"""App edge of the sampling path (SURVEY.md §8f rank 4): the reference's brain-LDM model-zoo bundle
-(model-zoo/models/brain_image_synthesis_latent_diffusion_model) running on this package's classes — its ``Sampler`` and
-``NiftiSaver`` scripts, a resolver for the bundle's ``inference.json`` and a pre-packed weight cache file."""
+"""App edge of the sampling path (SURVEY.md §8f rank 4): the reference's two latent-diffusion model-zoo bundles running
+on this package's classes — the brain-LDM bundle (model-zoo/models/brain_image_synthesis_latent_diffusion_model: its
+``Sampler`` and ``NiftiSaver`` scripts) and the chest X-ray text-to-image bundle (model-zoo/models/
+cxr_image_synthesis_latent_diffusion_model: its guided ``Sampler`` and ``JPGSaver``) — a resolver for the bundles'
+``inference.json`` and a pre-packed weight cache file."""
 from .config import BundleConfig
+from .cxr_sampler import Sampler as CXRSampler
 from .packed_cache import fingerprint, load_packed, save_packed
 from .sampler import Sampler
-from .saver import NiftiSaver, nifti1_bytes
+from .saver import JPGSaver, NiftiSaver, nifti1_bytes
 
-__all__ = ["BundleConfig", "Sampler", "NiftiSaver", "nifti1_bytes", "save_packed", "load_packed", "fingerprint"]
+__all__ = ["BundleConfig", "Sampler", "CXRSampler", "NiftiSaver", "JPGSaver", "nifti1_bytes", "save_packed",
+           "load_packed", "fingerprint"]

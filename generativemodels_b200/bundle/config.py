@@ -16,25 +16,44 @@ The bundle is driven by ``python -m monai.bundle run <id> --config_file configs/
 ``generative.…`` → ``generativemodels_b200.…`` and the bundle's ``scripts.sampler.Sampler`` / ``scripts.saver.
 NiftiSaver`` → :mod:`generativemodels_b200.bundle`.  Nothing here touches the GPU; it is the thin app edge of
 SURVEY.md §8f rank 4, not a re-implementation of MONAI's bundle machinery (no ``_mode_``, no macros ``%``, no YAML).
+
+The chest X-ray bundle (``model-zoo/models/cxr_image_synthesis_latent_diffusion_model``) runs the same way with
+``bundle="cxr"``: its ``scripts.sampler.Sampler`` is the guided sampler of :mod:`.cxr_sampler` and its
+``scripts.saver.JPGSaver`` the JPEG writer of :mod:`.saver`.  Items resolve lazily, so running ``save_jpg`` with an
+overridden ``prompt_embeds`` never builds the file's ``tokenizer`` / ``text_encoder``; only its ``imports`` still name
+``transformers`` and can be overridden where that package is absent.
 """
 from __future__ import annotations
 
 import importlib
 import json
+import os
 import re
+from pathlib import Path
 from typing import Any
 
 TARGET_MAP = {
     "scripts.sampler.Sampler": "generativemodels_b200.bundle.sampler.Sampler",
     "scripts.saver.NiftiSaver": "generativemodels_b200.bundle.saver.NiftiSaver",
 }
+CXR_TARGET_MAP = {
+    "scripts.sampler.Sampler": "generativemodels_b200.bundle.cxr_sampler.Sampler",
+    "scripts.saver.JPGSaver": "generativemodels_b200.bundle.saver.JPGSaver",
+}
+# Both bundles name their scripts ``scripts.sampler.Sampler``, so the ``scripts.*`` map is chosen per bundle:
+# short name -> (the bundle's directory name in the reference's model zoo, its script map).
+BUNDLES = {
+    "brain": ("brain_image_synthesis_latent_diffusion_model", TARGET_MAP),
+    "cxr": ("cxr_image_synthesis_latent_diffusion_model", CXR_TARGET_MAP),
+}
+DEFAULT_BUNDLE = "brain"
 _PREFIX_MAP = (("generative.", "generativemodels_b200."),)
 _REF = re.compile(r"@((?:\w+)(?:(?:#|::)\w+)*)")
 _SPECIAL = ("_target_", "_requires_", "_disabled_", "_desc_")
 
 
-def _locate(path: str):
-    path = TARGET_MAP.get(path, path)
+def _locate(path: str, target_map: dict = TARGET_MAP):
+    path = target_map.get(path, path)
     for old, new in _PREFIX_MAP:
         if path.startswith(old):
             path = new + path[len(old):]
@@ -44,9 +63,30 @@ def _locate(path: str):
     return getattr(importlib.import_module(module), name)
 
 
+def detect_bundle(config_path: str | os.PathLike | None) -> str:
+    """Short name of the bundle whose directory (its model-zoo name) contains ``config_path``; the brain bundle when
+    none does (or there is no path)."""
+    if config_path is not None:
+        parts = Path(os.path.abspath(config_path)).parts
+        for name, (dirname, _) in BUNDLES.items():
+            if dirname in parts:
+                return name
+    return DEFAULT_BUNDLE
+
+
 class BundleConfig:
-    def __init__(self, config: dict | str, overrides: dict | None = None) -> None:
-        if isinstance(config, str):
+    """A bundle's ``inference.json`` (a path or the parsed dict) with ``overrides`` applied.  ``bundle`` ("brain" or
+    "cxr") selects the map of the bundle's ``scripts.*`` targets; by default it is detected from the config path and
+    is the brain bundle otherwise."""
+
+    def __init__(self, config: dict | str, overrides: dict | None = None, bundle: str | None = None) -> None:
+        if bundle is None:
+            bundle = detect_bundle(config if isinstance(config, (str, os.PathLike)) else None)
+        if bundle not in BUNDLES:
+            raise ValueError(f"unknown bundle {bundle!r}; expected one of {sorted(BUNDLES)}")
+        self.bundle = bundle
+        self.target_map = BUNDLES[bundle][1]
+        if isinstance(config, (str, os.PathLike)):
             with open(config) as f:
                 config = json.load(f)
         self.config = dict(config)
@@ -117,7 +157,7 @@ class BundleConfig:
             if self._resolve(node.get("_disabled_", False)) in (True, "true", "True"):
                 return None
             kwargs = {k: self._resolve(v) for k, v in node.items() if k not in _SPECIAL}
-            return _locate(node["_target_"])(**kwargs)
+            return _locate(node["_target_"], self.target_map)(**kwargs)
         return node
 
     def get(self, id: str) -> Any:

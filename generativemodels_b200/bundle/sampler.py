@@ -17,7 +17,11 @@ import torch.nn as nn
 from ..cuda_graph import GraphedModule, graphed
 
 
-class Sampler:
+class GraphedUNetSampler:
+    """The UNet replay shared by the bundle samplers: on a CUDA device the diffusion model runs from a CUDA graph
+    captured on its first call (one capture per input signature, kept per model); ``use_cuda_graph=False`` runs it
+    eagerly.  Both give bit-identical results."""
+
     def __init__(self, use_cuda_graph: bool = True) -> None:
         super().__init__()
         self.use_cuda_graph = use_cuda_graph
@@ -31,6 +35,8 @@ class Sampler:
             g = self._graphed[id(diffusion_model)] = graphed(diffusion_model)
         return g
 
+
+class Sampler(GraphedUNetSampler):
     @torch.no_grad()
     def sampling_fn(self, input_noise: torch.Tensor, autoencoder_model: nn.Module, diffusion_model: nn.Module,
                     scheduler: nn.Module, conditioning: torch.Tensor) -> torch.Tensor:

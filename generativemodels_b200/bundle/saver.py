@@ -1,5 +1,6 @@
 """``NiftiSaver`` of the brain-LDM bundle (model-zoo/models/brain_image_synthesis_latent_diffusion_model/scripts/
-saver.py:8-33): crop the decoded volume, min-max normalise to uint8 and write ``<name>.nii.gz``.
+saver.py:8-33): crop the decoded volume, min-max normalise to uint8 and write ``<name>.nii.gz``; and ``JPGSaver`` of
+the chest X-ray bundle (below).
 
 The reference delegates the file format to ``nibabel`` (not vendored under /root/reference and not installed in this
 image); the writer below restates the published NIfTI-1 single-file layout (348-byte header, 4-byte extension flag,
@@ -102,3 +103,33 @@ class NiftiSaver:
         payload = nifti1_bytes(self.quantise(image_data), self.affine)
         with gzip.open(f"{str(self.output_dir)}/{file_name}.nii.gz", "wb") as f:
             f.write(payload)
+
+
+class JPGSaver:
+    """``JPGSaver`` of the chest X-ray bundle (model-zoo/models/cxr_image_synthesis_latent_diffusion_model/scripts/
+    saver.py:8-17): clip the decoded image to [0, 1], scale by 255, truncate to uint8 and write plane ``[0, 0]`` as
+    ``<output_dir>/<file_name>.jpg`` through PIL.
+
+    The clip / scale / truncate runs on the sample's device in its own dtype — the IEEE operations numpy performs in the
+    reference, so the array handed to PIL is identical — and only the uint8 plane crosses PCIe.  PIL is needed only
+    to write the file: a missing PIL raises ``ImportError`` at ``save``, not at import."""
+
+    def __init__(self, output_dir: str) -> None:
+        super().__init__()
+        self.output_dir = output_dir
+
+    @staticmethod
+    def quantise(image_data: torch.Tensor) -> np.ndarray:
+        """saver.py:14-16 up to the PIL call: ``(clip(x, 0, 1) * 255).astype(uint8)`` of plane [0, 0]."""
+        v = image_data[0, 0]
+        if v.dtype not in (torch.float16, torch.float32, torch.float64):
+            v = v.float()
+        return (v.clamp(0, 1) * 255).to(torch.uint8).cpu().numpy()
+
+    def save(self, image_data: torch.Tensor, file_name: str) -> None:
+        try:
+            from PIL import Image
+        except ImportError as e:
+            raise ImportError("JPGSaver writes its .jpg through Pillow (PIL), which is not installed: "
+                              "pip install pillow") from e
+        Image.fromarray(self.quantise(image_data)).save(f"{str(self.output_dir)}/{file_name}.jpg")
