@@ -26,11 +26,17 @@ __global__ void __launch_bounds__(256) rows_linear_kernel(const h16* __restrict_
   for (int m = warp; m < M; m += 8) {
     const h16* xr = x + (long long)m * x_pitch;
     if (ln_g) {
-      float s = 0.f, q = 0.f;
-      for (int k = lane; k < K; k += 32) { const float v = h2f(xr[k]); s += v; q = fmaf(v, v, q); }
-      s = warp_sum(s); q = warp_sum(q);
-      const float mean = s / K;
-      const float rstd = rsqrtf(fmaxf(q / K - mean * mean, 0.f) + ln_eps);
+      // two passes, as layernorm_kernel: the variance from x - mean, not E[x^2] - mean^2 (which cancels when the
+      // row's mean is large against its spread)
+      float s = 0.f;
+      for (int k = lane; k < K; k += 32) s += h2f(xr[k]);
+      const float mean = warp_sum(s) / K;
+      float q = 0.f;
+      for (int k = lane; k < K; k += 32) {
+        const float d = h2f(xr[k]) - mean;
+        q = fmaf(d, d, q);
+      }
+      const float rstd = rsqrtf(warp_sum(q) / K + ln_eps);
       for (int k = lane; k < Kp; k += 32)
         xs[m * Kp + k] = k < K ? f2h((h2f(xr[k]) - mean) * rstd * ln_g[k] + ln_b[k])
                                : f2h(0.f);

@@ -6,9 +6,11 @@
 // BasicTransformerBlock (diffusion_model_unet.py:221-223).
 //
 // GroupNorm is split in two phases so that neither pass re-reads more than it must:
-//   stats : every block reduces a slab of voxels to per-channel (sum, sumsq) partials in fp32;
-//           a tiny finalize kernel folds partials -> group mean / rstd in fp64 and emits the per-(n, c)
-//           affine pair a = rstd * gamma, b = beta - mean * a.
+//   stats : every block reduces a slab of voxels to per-channel (sum, sumsq) partials of x - p in fp32, where the
+//           pivot p is one element of the group (its first channel at voxel 0); a tiny finalize kernel folds the
+//           partials -> group mean / rstd in fp64 and emits the per-(n, c) affine pair a = rstd * gamma,
+//           b = beta - mean * a.  Summing x - p instead of x keeps E[x^2] - mean^2 from cancelling when a group's
+//           mean is large against its spread (the fp32 error of a raw sum of squares grows with (mean / std)^2).
 //   apply : y = silu(a * x + b), one read + one write, optionally reading a virtual concat of two tensors
 //           (the up-path torch.cat at diffusion_model_unet.py:1232/1340/1461 is never materialised raw).
 #include "common.cuh"
@@ -17,11 +19,17 @@ namespace b200 {
 
 static constexpr int kGnMaxChunks = 512;
 
+// The statistics pivot of the group whose first channel is c (of the virtual concat): x[n, voxel 0, c].
+__device__ __forceinline__ float gn_pivot(const h16* x0, const h16* x1, int C0, int pitch0, int pitch1,
+                                          long long spatial, int n, int c) {
+  return c < C0 ? h2f(x0[(long long)n * spatial * pitch0 + c]) : h2f(x1[(long long)n * spatial * pitch1 + (c - C0)]);
+}
+
 // ---- stats --------------------------------------------------------------------------------------
 // grid = (chunks, N); block = CV * rows threads, CV = C_total / VEC channel vectors.
 template <int VEC>
 __global__ void gn_partial_kernel(const h16* __restrict__ x0, const h16* __restrict__ x1,
-                                  int C0, int C1, int pitch0, int pitch1, long long spatial,
+                                  int C0, int C1, int pitch0, int pitch1, long long spatial, int cpg,
                                   long long vox_per_chunk, float* __restrict__ partial) {
   const int C = C0 + C1;
   const int CV = C / VEC;
@@ -42,9 +50,13 @@ __global__ void gn_partial_kernel(const h16* __restrict__ x0, const h16* __restr
   else        { src = x1; pitch = pitch1; cc = c - C0; }
   src += (long long)n * spatial * pitch + cc;
 
-  float sum[VEC], sq[VEC];
+  float sum[VEC], sq[VEC], piv[VEC];
 #pragma unroll
-  for (int j = 0; j < VEC; ++j) { sum[j] = 0.f; sq[j] = 0.f; }
+  for (int j = 0; j < VEC; ++j) {
+    sum[j] = 0.f;
+    sq[j] = 0.f;
+    piv[j] = gn_pivot(x0, x1, C0, pitch0, pitch1, spatial, n, (c + j) / cpg * cpg);
+  }
 
   if (row < rows) {
     long long s = s0 + row;
@@ -60,7 +72,11 @@ __global__ void gn_partial_kernel(const h16* __restrict__ x0, const h16* __restr
           float f[8];
           unpack8(v[u], f);
 #pragma unroll
-          for (int j = 0; j < 8; ++j) { sum[j] += f[j]; sq[j] = fmaf(f[j], f[j], sq[j]); }
+          for (int j = 0; j < 8; ++j) {
+            const float d = f[j] - piv[j];
+            sum[j] += d;
+            sq[j] = fmaf(d, d, sq[j]);
+          }
         }
       }
     }
@@ -74,7 +90,11 @@ __global__ void gn_partial_kernel(const h16* __restrict__ x0, const h16* __restr
         for (int j = 0; j < VEC; ++j) f[j] = h2f(src[s * pitch + j]);
       }
 #pragma unroll
-      for (int j = 0; j < VEC; ++j) { sum[j] += f[j]; sq[j] = fmaf(f[j], f[j], sq[j]); }
+      for (int j = 0; j < VEC; ++j) {
+        const float d = f[j] - piv[j];
+        sum[j] += d;
+        sq[j] = fmaf(d, d, sq[j]);
+      }
     }
   }
   // reduce the `rows` threads that share a channel vector through shared memory
@@ -95,9 +115,10 @@ __global__ void gn_partial_kernel(const h16* __restrict__ x0, const h16* __restr
   }
 }
 
-// grid = (groups, N); folds the partials of one group in fp64 and writes the affine pairs.
-__global__ void gn_finalize_kernel(const float* __restrict__ partial, int chunks, int C, int groups,
-                                   long long spatial, float eps, const float* __restrict__ gamma,
+// grid = (groups, N); folds the partials of one group in fp64 around the group mean and writes the affine pairs.
+__global__ void gn_finalize_kernel(const float* __restrict__ partial, const h16* __restrict__ x0,
+                                   const h16* __restrict__ x1, int C0, int pitch0, int pitch1, int chunks, int C,
+                                   int groups, long long spatial, float eps, const float* __restrict__ gamma,
                                    const float* __restrict__ beta, float* __restrict__ affine) {
   const int g = blockIdx.x, n = blockIdx.y;
   const int cpg = C / groups;
@@ -142,10 +163,12 @@ __global__ void gn_finalize_kernel(const float* __restrict__ partial, int chunks
     if (l == 0) { ss[0] = s; sq[0] = q; }
   }
   __syncthreads();
+  // the partials are sums of x - p: mean = p + E[x - p], var = E[(x - p)^2] - E[x - p]^2
   const double cnt = (double)spatial * cpg;
-  const double mean = ss[0] / cnt;
-  double var = sq[0] / cnt - mean * mean;
+  const double dm = ss[0] / cnt;
+  double var = sq[0] / cnt - dm * dm;
   if (var < 0.0) var = 0.0;
+  const double mean = (double)gn_pivot(x0, x1, C0, pitch0, pitch1, spatial, n, g * cpg) + dm;
   const float rstd = (float)(1.0 / sqrt(var + (double)eps));
   for (int j = threadIdx.x; j < cpg; j += blockDim.x) {
     const int c = g * cpg + j;
@@ -363,6 +386,7 @@ __global__ void __launch_bounds__(512) gn_fused_small_kernel(const h16* __restri
   const int v = threadIdx.x % vpr, row0 = threadIdx.x / vpr;
   const bool active = row0 < rows_per_iter;
   const int c_off = v * VEC;
+  const float piv = h2f(src[0]);                     // statistics pivot: the group's first element (see stats)
 
   float s = 0.f, q = 0.f;
   uint4 keep[KREG > 0 ? KREG : 1];
@@ -376,10 +400,15 @@ __global__ void __launch_bounds__(512) gn_fused_small_kernel(const h16* __restri
       }
 #pragma unroll
       for (int k = 0; k < KREG; ++k) {          // same row order as the loop form: identical sums
+        if (row0 + k * rows_per_iter >= spatial) continue;   // a row past the slab adds nothing (not d = -piv)
         float f[8];
         unpack8(keep[k], f);
 #pragma unroll
-        for (int j = 0; j < 8; ++j) { s += f[j]; q = fmaf(f[j], f[j], q); }
+        for (int j = 0; j < 8; ++j) {
+          const float d = f[j] - piv;
+          s += d;
+          q = fmaf(d, d, q);
+        }
       }
     } else {
 #pragma unroll 4
@@ -387,7 +416,11 @@ __global__ void __launch_bounds__(512) gn_fused_small_kernel(const h16* __restri
         float f[VEC];
         gn_load_vec<VEC>(src + (long long)r * pitch + c_off, f);
 #pragma unroll
-        for (int j = 0; j < VEC; ++j) { s += f[j]; q = fmaf(f[j], f[j], q); }
+        for (int j = 0; j < VEC; ++j) {
+          const float d = f[j] - piv;
+          s += d;
+          q = fmaf(d, d, q);
+        }
       }
     }
   }
@@ -411,10 +444,10 @@ __global__ void __launch_bounds__(512) gn_fused_small_kernel(const h16* __restri
     }
     if (l == 0) {
       const double cnt = (double)spatial * cpg;
-      const double mean = ds / cnt;
-      double var = dq / cnt - mean * mean;
+      const double dm = ds / cnt;
+      double var = dq / cnt - dm * dm;
       if (var < 0.0) var = 0.0;
-      stat[0] = (float)mean;
+      stat[0] = (float)((double)piv + dm);
       stat[1] = (float)(1.0 / sqrt(var + (double)eps));
     }
   }
@@ -660,19 +693,22 @@ extern "C" int b200_groupnorm_stats(const b200_gn_stats_params* p, void* stream_
                       ((uintptr_t)p->x_ptr[0] % 16 == 0) && (C1 == 0 || (uintptr_t)p->x_ptr[1] % 16 == 0);
   gn_block_shape(C, vec_ok, vec, cv, rows);
   B200_CHECK_ARG(cv <= 1024, "gn_stats: too many channels (%d)", C);
+  const size_t smem = (size_t)rows * C * 2 * sizeof(float);
+  B200_CHECK_ARG(smem <= 48 * 1024, "gn_stats: %d channels need %zu bytes of shared memory (at most 6144 channels)", C,
+                 smem);
   const int chunks = gn_chunks(p->N, p->spatial, rows);
   const long long vpc = (p->spatial + chunks - 1) / chunks;
   const int threads = cv * rows;
-  const size_t smem = (size_t)rows * C * 2 * sizeof(float);
+  const int cpg = C / p->groups;
   dim3 grid(chunks, p->N);
   const h16* x0 = reinterpret_cast<const h16*>(p->x_ptr[0]);
   const h16* x1 = reinterpret_cast<const h16*>(p->x_ptr[1]);
   if (vec == 8)
-    B200_CUDA(b200::launch_kernel(gn_partial_kernel<8>, grid, threads, smem, stream, x0, x1, C0, C1, p->x_pitch[0], p->x_pitch[1], p->spatial, vpc, p->partial));
+    B200_CUDA(b200::launch_kernel(gn_partial_kernel<8>, grid, threads, smem, stream, x0, x1, C0, C1, p->x_pitch[0], p->x_pitch[1], p->spatial, cpg, vpc, p->partial));
   else
-    B200_CUDA(b200::launch_kernel(gn_partial_kernel<1>, grid, threads, smem, stream, x0, x1, C0, C1, p->x_pitch[0], p->x_pitch[1], p->spatial, vpc, p->partial));
+    B200_CUDA(b200::launch_kernel(gn_partial_kernel<1>, grid, threads, smem, stream, x0, x1, C0, C1, p->x_pitch[0], p->x_pitch[1], p->spatial, cpg, vpc, p->partial));
   B200_LAUNCH_CHECK("gn_partial_kernel");
-  B200_CUDA(b200::launch_kernel(gn_finalize_kernel, dim3(p->groups, p->N), 128, 0, stream, p->partial, chunks, C, p->groups, p->spatial, p->eps,
+  B200_CUDA(b200::launch_kernel(gn_finalize_kernel, dim3(p->groups, p->N), 128, 0, stream, p->partial, x0, x1, C0, p->x_pitch[0], p->x_pitch[1], chunks, C, p->groups, p->spatial, p->eps,
                                                                 p->gamma, p->beta, p->affine));
   B200_LAUNCH_CHECK("gn_finalize_kernel");
   return B200_OK;

@@ -175,7 +175,12 @@ int64_t b200_igemm_split_workspace_bytes(const b200_igemm_params* p);
  * GroupNorm (+SiLU) on NDHWC h16, optionally over the virtual concat of two tensors.
  * Replaces nn.GroupNorm + nn.SiLU in ResnetBlock / AttentionBlock / out head
  * (diffusion_model_unet.py:623-624,643,671,684, 372, 1853-1855; autoencoderkl.py:139-146,229).
- * Two phases: per-block partial sums -> per-(n,c) affine (a = rstd*gamma, b = beta - mean*a).
+ * Two phases: per-block partial sums -> per-(n,c) affine (a = fp32(rstd*gamma), b = fp32(beta - fp32(mean)*a)).
+ * Statistics: the biased mean and variance of each group of the h16 inputs, rstd = 1 / sqrt(var + eps).  They are
+ * summed as x - p with p the group's first element (channel g*C/groups at voxel 0), in fp32 per thread and folded in
+ * fp64, so a large mean against the spread costs no precision: with s = sqrt(var + eps), the stats and fused
+ * kernels give |d mean| <= 2^-12 (s + |mean - p|) and |d rstd| <= 2^-12 rstd (1 + (mean - p)^2 / s^2).
+ * Only channels [0, x_C[i]) of the first N * spatial rows of each source are read (pad channels may hold anything).
  * ---------------------------------------------------------------------------------------------- */
 typedef struct {
   const void* x_ptr[2];   /* h16 NDHWC sources (second may be NULL)      */
@@ -191,11 +196,17 @@ typedef struct {
   float*  affine;         /* out: [N][C0+C1][2] (a, b) fp32               */
 } b200_gn_stats_params;
 int64_t b200_groupnorm_workspace_bytes(int32_t N, int64_t spatial, int32_t C_total);
+/* Writes affine [N][C0+C1][2] and nothing else but the workspace.  A group may straddle the two sources.  At most 6144
+ * channels when every source is 16-byte aligned with C_i and x_pitch[i] multiples of 8 (the block reduction's shared
+ * memory), at most 1024 otherwise; B200_EINVAL beyond. */
 int b200_groupnorm_stats(const b200_gn_stats_params* p, void* stream);
 /* The same affine table from partial sums that b200_igemm left while it wrote the tensor(s) (see gn_partial there),
  * so the statistics pass over the activations disappears: source i contributes partial[i] = [N][slots[i]][x_C[i]/8][2].
  * x_ptr of p is not read; every group of the virtual concat must be a whole number of 8-channel producer groups
- * inside one source ((C0+C1)/groups % 8 == 0 and C0 % ((C0+C1)/groups) == 0). */
+ * inside one source ((C0+C1)/groups % 8 == 0 and C0 % ((C0+C1)/groups) == 0).  The fold is fp64 over the fp32
+ * partials (mean = sum / n, var = sumsq / n - mean^2), exact to them up to fp64 rounding.  b200_igemm's partials are
+ * raw fp32 sums of x and x^2, so unlike b200_groupnorm_stats this path loses rstd precision, about (mean / std)^2
+ * 2^-24 times the terms per sum, when a group's mean is large against its spread. */
 int b200_groupnorm_from_partials(const b200_gn_stats_params* p, const float* const partial[2],
                                  const int32_t slots[2], void* stream);
 /* The same with the producer group width of each source stated (b200_igemm's gn_group: 8 or 4 channels per partial
@@ -215,6 +226,9 @@ typedef struct {
   void*   y_ptr;          /* h16 NDHWC, channel pitch y_pitch            */
   int32_t y_pitch;
 } b200_gn_apply_params;
+/* y = h16(act(fma(x, a, b))) per element (SiLU with __expf / __fdividef: a few fp32 ulps); pad channels [C, y_pitch)
+ * of the N * spatial output rows are written +0, nothing past them.  Input pad channels are not read.  Another
+ * activation (RELU, GELU, ...) is B200_EINVAL. */
 int b200_groupnorm_apply(const b200_gn_apply_params* p, void* stream);
 
 /* nn.GroupNorm (+ nn.SiLU) in ONE launch for small tensors (the deep levels of a latent UNet normalise 10^4..10^6
@@ -222,21 +236,30 @@ int b200_groupnorm_apply(const b200_gn_apply_params* p, void* stream);
  * (sample, group) sums its slab, folds in fp64 and rewrites it; same arithmetic as stats + apply.  Reads x_ptr / x_C /
  * x_pitch / N / spatial / groups / eps / gamma / beta of `s` (partial and affine are not used) and act / y_ptr /
  * y_pitch of `a`.  With two sources no group may straddle them (C0 % (C / groups) == 0); at most 4096 channels per
- * group.  Meant for spatial * C / groups up to ~10^5 elements per group — larger tensors want the two-phase form. */
+ * group (and cpg / vec <= 512 for the widest vector vec in {8, 4, 2, 1} that channel counts, pitches and base
+ * pointers allow), spatial < 2^24.  Meant for spatial * C / groups up to ~10^5 elements per group — larger tensors
+ * want the two-phase form.  Statistics, output and footprint as stats + apply. */
 int b200_groupnorm_fused(const b200_gn_stats_params* s, const b200_gn_apply_params* a, void* stream);
 
 /* SPADE modulation (generative/networks/blocks/spade_norm.py:78-96), one pass:
  *   y = act( (x * ax + bx) * (1 + (g * ag + bg)) + (t * at + bt) )
  * x = virtual concat of the sources in p (GroupNorm affine table p->affine from b200_groupnorm_stats), g / t = the
  * gamma / beta halves of gb ([rows][gb_pitch] h16, channels [0,C) and [C,2C)) whose own per-(sample, channel)
- * InstanceNorm table gb_affine is [N][2C][2] (monai's Convolution default norm on mlp_gamma / mlp_beta). */
+ * InstanceNorm table gb_affine is [N][2C][2] (monai's Convolution default norm on mlp_gamma / mlp_beta).  Each factor
+ * is one fp32 fma and the result h16(act(fma(nx, 1 + gg, tt))); gb_pitch >= 2C, and gb columns [2C, gb_pitch) and
+ * input pad channels are not read; output pad channels [C, y_pitch) are written +0. */
 int b200_spade_apply(const b200_gn_apply_params* p, const void* gb, int32_t gb_pitch, const float* gb_affine,
                      void* stream);
-/* F.interpolate(mode="nearest", size=...) on NDHWC h16: src index = min(floor(dst * in / out), in - 1) per axis. */
+/* F.interpolate(mode="nearest", size=...) on NDHWC h16: src index = min(floor(dst * fp32(in / out)), in - 1) per axis,
+ * the product rounded to fp32 as PyTorch does for fp16 / bf16 / fp32 tensors (it differs from the exact-rational
+ * floor(dst * in / out) for some sizes, e.g. 26 -> 22, 6 -> 74, 14 -> 46).  Copies all `pitch` channels of a voxel. */
 int b200_resize_nearest(const void* x, int32_t N, int32_t D, int32_t H, int32_t W, int32_t pitch, void* y, int32_t OD,
                         int32_t OH, int32_t OW, void* stream);
 
-/* nn.LayerNorm over the last dim of a h16 [M, C] matrix (diffusion_model_unet.py:221-223). */
+/* nn.LayerNorm over the last dim of a h16 [M, C] matrix (diffusion_model_unet.py:221-223): two fp32 passes (mean, then
+ * the mean square of x - mean), one warp per row; with u = 2^-24 (C / 32 + 8) and s = sqrt(var + eps),
+ * |d mean| <= u (|mean| + s) and |d rstd| <= rstd (u + 2^-21 + (d mean / s)^2).  Output h16((x - mean) rstd gamma +
+ * beta), pad columns [C, y_pitch) +0; input columns [C, x_pitch) are not read. */
 int b200_layernorm(const void* x, int64_t M, int32_t C, int32_t x_pitch, const float* gamma,
                    const float* beta, float eps, void* y, int32_t y_pitch, void* stream);
 
@@ -404,8 +427,8 @@ int b200_cache_append(const void* src, void* cache, int32_t B, int32_t T, int32_
 int b200_advance_i32(int32_t* p, int32_t delta, void* stream);
 /* Decode-time linear layers (one new token per sequence: M <= 8 rows, HBM/L2-bound GEMVs):
  *   out[m, o] = act( LN?(x[m, :]) . w[o, :] + bias[o] ) + res[m, o]
- * x h16 rows; ln_gamma / ln_beta (NULL = no LayerNorm; nn.LayerNorm semantics, output rounded to h16 as the
- * stand-alone kernel does); w = the K-major h16 matrix b200_igemm consumes (row pitch w_pitch, multiple of 8);
+ * x h16 rows; ln_gamma / ln_beta (NULL = no LayerNorm; nn.LayerNorm semantics with b200_layernorm's arithmetic and
+ * accuracy, the row rounded to h16 as the stand-alone kernel does); w = the K-major h16 matrix b200_igemm consumes (row pitch w_pitch, multiple of 8);
  * out h16 or fp32 (out_dtype).  (blocks/transformerblock.py:87-92, blocks/selfattention.py:103-110, 145.) */
 int b200_rows_linear(const void* x, int32_t x_pitch, int32_t M, int32_t K, const float* ln_gamma,
                      const float* ln_beta, float ln_eps, const void* w, int32_t w_pitch, int32_t O, const float* bias,

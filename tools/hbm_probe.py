@@ -1,7 +1,8 @@
 """Dev probe for ncu: one launch each of the HBM-bound kernels at the sizes the BASELINE configs give them —
 GroupNorm statistics + apply(+SiLU) on a 1x160x224x160x256 tensor (C3 level 0), the DDIM step on 1x1x160x224x160 fp32,
-the VQ nearest-code search at M = 32 768 x 32 with 256 codes (C4 at 128^3).  CUDA-event timings are printed for the
-roofline table; under `ncu --set full -k regex:...` the same launches give dram__bytes_{read,write}."""
+the VQ nearest-code search at M = 32 768 x 32 with 256 codes (C4 at 128^3); and, launch-bound, the fused GroupNorm at
+the C2 UNet's deep levels and rows_linear's LayerNorm-prologue GEMV at M = 8, K = 512 (--norm-only: just those).
+CUDA-event timings are printed for the roofline table; under `ncu --set full -k regex:...` the same launches give dram__bytes_{read,write}."""
 import sys
 from pathlib import Path
 sys.path.insert(0, str(Path(__file__).resolve().parents[1]))
@@ -13,6 +14,7 @@ from generativemodels_b200.networks.schedulers import DDIMScheduler
 torch.manual_seed(0)
 dev = "cuda"
 HBM = 6582.5
+NORM_ONLY = "--norm-only" in sys.argv      # only the launch-bound normalisation timings below (for A/B runs)
 
 
 def timed(fn, n=5):
@@ -25,6 +27,39 @@ def timed(fn, n=5):
     return min(ts)
 
 
+def many(fn, n):
+    def run():
+        for _ in range(n):
+            fn()
+    return run
+
+
+# launch-bound normalisation: the fused GroupNorm at the C2 UNet's deep levels (N = 1, latent 64 x 64 -> 32^2 x 256
+# and 16^2 x 512, 32 groups) and the LayerNorm-prologue GEMV of decoding (rows_linear, M = 8, K = O = 512)
+from generativemodels_b200 import _lib
+import ctypes as Cc
+props = torch.cuda.get_device_properties(0)
+print(f"device: {props.name}")
+for hw, ch in ((32, 256), (16, 512)):
+    xs = ops.CL(torch.randn(1, 1, hw, hw, ch, device=dev).to(ops.H16), ch, 2)
+    g1, b1 = torch.ones(ch, device=dev), torch.zeros(ch, device=dev)
+    fn = lambda: ops.groupnorm(xs, 32, 1e-6, g1, b1, act=ops.ACT_SILU)
+    ms = timed(many(fn, 200), n=7) / 200
+    print(f"fused GroupNorm(32)+SiLU 1x{hw}x{hw}x{ch}: {ms*1e3:.2f} us per call (200 back-to-back calls, best of 7)")
+lib = _lib.require_device()
+M, K = 8, 512
+xr = torch.randn(M, K, device=dev).to(ops.H16)
+W = (torch.randn(K, K, device=dev) * 0.05).to(ops.H16)
+lg, lb = torch.ones(K, device=dev), torch.zeros(K, device=dev)
+yr = torch.empty(M, K, device=dev, dtype=ops.H16)
+def rows_linear():
+    _lib.check(lib.b200_rows_linear(xr.data_ptr(), K, M, K, lg.data_ptr(), lb.data_ptr(), 1e-5, W.data_ptr(), K, K,
+                                    None, 0, None, 0, yr.data_ptr(), K, 0, ops._stream()), "rows_linear")
+ms = timed(many(rows_linear, 500), n=7) / 500
+print(f"rows_linear + LayerNorm prologue M={M} K=O={K}: {ms*1e3:.2f} us per call (500 back-to-back calls, best of 7)")
+if NORM_ONLY:
+    sys.exit(0)
+
 C = 256
 x = ops.CL((torch.randn(1, 160, 224, 160, C, device=dev) * 0.7 + 0.1).to(ops.H16), C, 3)
 gamma, beta = torch.ones(C, device=dev), torch.zeros(C, device=dev)
@@ -34,8 +69,6 @@ print(f"GroupNorm(32)+SiLU stats+apply on {tuple(x.t.shape)} ({nbytes/1e9:.2f} G
       f"{3*nbytes/ms/1e6:.0f} GB/s algorithmic (2 reads + 1 write), {3*nbytes/ms/1e6/HBM:.3f} of measured copy bandwidth")
 aff = ops.groupnorm_affine(x, 32, 1e-6, gamma, beta)
 out = x.like()
-from generativemodels_b200 import _lib
-import ctypes as Cc
 def apply_only():
     _, ap = ops._gn_params([x])
     ap.affine, ap.act = aff.data_ptr(), ops.ACT_SILU
