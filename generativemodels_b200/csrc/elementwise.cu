@@ -730,7 +730,7 @@ __global__ void ddpm_kl_kernel(const float* __restrict__ x0, const float* __rest
                                double* __restrict__ sample_sum, long long per_sample) {
   const int n = blockIdx.y;
   const long long base = (long long)n * per_sample;
-  float acc = 0.f;
+  double acc = 0.0;                             // fp64 per thread: a thread sums per_sample / (grid threads) terms
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < per_sample;
        i += (long long)gridDim.x * blockDim.x) {
     const float a = x0[base + i], s = xt[base + i], m = mo[base + i];
@@ -759,10 +759,10 @@ __global__ void ddpm_kl_kernel(const float* __restrict__ x0, const float* __rest
                    d * d * expf(-c.log_pred_var));
     }
     if (kl_out) kl_out[base + i] = kl;
-    acc += kl;
+    acc += (double)kl;
   }
   __shared__ double red[8];
-  double d = (double)acc;
+  double d = acc;
   for (int o = 16; o > 0; o >>= 1) d += __shfl_xor_sync(0xffffffffu, d, o);
   if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = d;
   __syncthreads();
@@ -985,7 +985,9 @@ extern "C" int b200_nhwc_to_nchw(const void* x, int32_t x_dtype, int32_t N, int3
 extern "C" int b200_upsample_nearest2x(const void* x, int32_t N, int32_t D, int32_t H, int32_t W, int32_t pitch,
                                        int32_t dims, void* y, void* stream_v) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
-  B200_CHECK_ARG(x && y && pitch % 8 == 0 && (dims == 2 || dims == 3), "upsample2x: bad arguments");
+  B200_CHECK_ARG(x && y && N >= 1 && D >= 1 && H >= 1 && W >= 1 && pitch >= 8 && pitch % 8 == 0 &&
+                 (dims == 2 || dims == 3) && (uintptr_t)x % 16 == 0 && (uintptr_t)y % 16 == 0,
+                 "upsample2x: bad arguments");
   const long long total = (long long)N * (dims == 3 ? 2 * D : D) * 2 * H * 2 * W * (pitch / 8);
   B200_CUDA(b200::launch_kernel(upsample2x_kernel, grid_for(total), 256, 0, stream, reinterpret_cast<const uint4*>(x), N, D, H, W, pitch / 8, dims,
                                                         reinterpret_cast<uint4*>(y)));
@@ -1022,7 +1024,9 @@ extern "C" int b200_vae_reparam_kld(const float* mu, const float* logvar, const 
 extern "C" int b200_avgpool2(const void* x, int32_t N, int32_t D, int32_t H, int32_t W, int32_t pitch, int32_t dims,
                              void* y, void* stream_v) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
-  B200_CHECK_ARG(x && y && pitch % 8 == 0 && (dims == 2 || dims == 3), "avgpool2: bad arguments");
+  B200_CHECK_ARG(x && y && N >= 1 && D >= 1 && H >= 1 && W >= 1 && pitch >= 8 && pitch % 8 == 0 &&
+                 (dims == 2 || dims == 3) && (uintptr_t)x % 16 == 0 && (uintptr_t)y % 16 == 0,
+                 "avgpool2: bad arguments");
   const long long total = (long long)N * (dims == 3 ? D / 2 : D) * (H / 2) * (W / 2) * (pitch / 8);
   if (total == 0) return B200_OK;
   B200_CUDA(b200::launch_kernel(avgpool2_kernel, grid_for(total), 256, 0, stream, reinterpret_cast<const uint4*>(x), N, D, H, W, pitch / 8, dims,
@@ -1128,7 +1132,8 @@ extern "C" int b200_interpolate(const void* x, int32_t x_dtype, const int64_t* x
 
 extern "C" int b200_axpy_h16(const void* a, const void* b, float alpha, void* y, int64_t n, void* stream_v) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
-  B200_CHECK_ARG(a && b && y && n % 8 == 0, "axpy_h16: element count must be a multiple of 8");
+  B200_CHECK_ARG(a && b && y && n >= 0 && n % 8 == 0, "axpy_h16: element count must be a multiple of 8");
+  B200_CHECK_ARG(((uintptr_t)a | (uintptr_t)b | (uintptr_t)y) % 16 == 0, "axpy_h16: pointers must be 16-byte aligned");
   if (n == 0) return B200_OK;
   B200_CUDA(b200::launch_kernel(axpy_h16_kernel, grid_for(n / 8), 256, 0, stream, reinterpret_cast<const uint4*>(a), reinterpret_cast<const uint4*>(b),
                                                        alpha, reinterpret_cast<uint4*>(y), n / 8));
@@ -1188,7 +1193,7 @@ __global__ void cache_append_kernel(const h16* __restrict__ src, h16* __restrict
     const int c = (int)(i % pitch);
     const long long r = i / pitch;
     const int t = (int)(r % T), b = (int)(r / T);
-    if (pos + t < L) cache[((long long)b * L + pos + t) * pitch + c] = src[i];
+    if ((unsigned)(pos + t) < (unsigned)L) cache[((long long)b * L + pos + t) * pitch + c] = src[i];  // 0 <= pos + t < L
   }
 }
 __global__ void advance_i32_kernel(int* p, int delta) { *p += delta; }
@@ -1239,8 +1244,8 @@ extern "C" int b200_copy_channels(const void* src, int32_t C, int32_t src_pitch,
 extern "C" int b200_geglu(const void* x, int64_t M, int32_t H, int32_t x_pitch, void* y, int32_t y_pitch,
                           void* stream_v) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
-  B200_CHECK_ARG(x && y && H % 8 == 0 && x_pitch % 8 == 0 && y_pitch % 8 == 0 && x_pitch >= 2 * H && y_pitch >= H,
-                 "geglu: bad arguments");
+  B200_CHECK_ARG(x && y && M >= 1 && H >= 8 && H % 8 == 0 && x_pitch % 8 == 0 && y_pitch % 8 == 0 &&
+                 x_pitch >= 2 * H && y_pitch >= H && ((uintptr_t)x | (uintptr_t)y) % 16 == 0, "geglu: bad arguments");
   B200_CUDA(b200::launch_kernel(geglu_kernel, grid_for(M * (H / 8)), 256, 0, stream, reinterpret_cast<const h16*>(x), M, H, x_pitch,
                                                          reinterpret_cast<h16*>(y), y_pitch));
   B200_LAUNCH_CHECK("geglu_kernel");
@@ -1279,6 +1284,7 @@ extern "C" int b200_timestep_embedding(const float* t, int32_t N, int32_t dim, f
                                        void* stream_v) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
   B200_CHECK_ARG(t && emb && N >= 1 && dim >= 1, "timestep_embedding: bad arguments");
+  B200_CHECK_ARG((long long)N * dim < (1ll << 31), "timestep_embedding: N * dim must be below 2^31");
   B200_CUDA(b200::launch_kernel(timestep_embedding_kernel, (N * dim + 255) / 256, 256, 0, stream, t, N, dim, max_period, emb));
   B200_LAUNCH_CHECK("timestep_embedding_kernel");
   return B200_OK;

@@ -266,12 +266,15 @@ int b200_layernorm(const void* x, int64_t M, int32_t C, int32_t x_pitch, const f
 /* ------------------------------------------------------------------------------------------------
  * Layout / resampling / elementwise helpers on the API edge and between fused ops.
  * ---------------------------------------------------------------------------------------------- */
-/* NC[D]HW fp32 -> NDHWC h16 (channel pitch `pitch`, pad channels zeroed) and back. */
+/* NC[D]HW fp32 -> NDHWC h16 (channel pitch `pitch`, pad channels zeroed; RN, fp16 saturates) and back (x_dtype
+ * B200_DT_H16 or B200_DT_F32; input columns [C, pitch) are not read).  Both are exact apart from the one rounding. */
 int b200_nchw_to_nhwc(const float* x, int32_t N, int32_t C, int64_t spatial, void* y, int32_t pitch,
                       void* stream);
 int b200_nhwc_to_nchw(const void* x, int32_t x_dtype, int32_t N, int32_t C, int64_t spatial,
                       int32_t pitch, float* y, void* stream);
-/* F.interpolate(scale_factor=2, mode="nearest") (diffusion_model_unet.py:578; autoencoderkl.py:84). */
+/* F.interpolate(scale_factor=2, mode="nearest") (diffusion_model_unet.py:578; autoencoderkl.py:84): a copy of every
+ * `pitch` channel of x [N][D][H][W][pitch] into y [N][OD][2H][2W][pitch] (OD = 2D for dims == 3, D slices for dims == 2).
+ * N, D, H, W >= 1, pitch a positive multiple of 8, x and y 16-byte aligned (B200_EINVAL otherwise). */
 int b200_upsample_nearest2x(const void* x, int32_t N, int32_t D, int32_t H, int32_t W, int32_t pitch,
                             int32_t dims /*2 or 3*/, void* y, void* stream);
 /* nn.Upsample(scale_factor=2, mode="bilinear" | "bicubic") on a 2-D NHWC h16 tensor [N][H][W][pitch] -> [N][2H][2W][pitch]
@@ -286,7 +289,10 @@ int b200_upsample_nearest2x(const void* x, int32_t N, int32_t D, int32_t H, int3
 #define B200_INTERP_BICUBIC  1
 int b200_upsample2x_interp(const void* x, int32_t N, int32_t H, int32_t W, int32_t pitch, int32_t mode, void* y,
                            void* stream);
-/* nn.AvgPool{2,3}d(kernel=2, stride=2) (diffusion_model_unet.py:522). */
+/* nn.AvgPool{2,3}d(kernel=2, stride=2) (diffusion_model_unet.py:522) on [N][D][H][W][pitch] -> floor(extent / 2) per
+ * pooled axis (dims == 2 pools H and W of every D slice): the 4 (8) taps added in fp32 in d, h, w order, then scaled by
+ * 1/4 (1/8), one rounding on the store.  Every `pitch` channel is processed, so input pad channels must be finite (zeros
+ * stay zeros).  N, D, H, W >= 1, pitch a positive multiple of 8, x and y 16-byte aligned (B200_EINVAL otherwise). */
 int b200_avgpool2(const void* x, int32_t N, int32_t D, int32_t H, int32_t W, int32_t pitch,
                   int32_t dims, void* y, void* stream);
 /* nn.AvgPool{2,3}d / nn.MaxPool{2,3}d(kernel_size=kernel, stride=2, padding=padding) on NDHWC h16 [N][D][H][W][pitch]
@@ -343,10 +349,12 @@ int b200_interpolate(const void* x, int32_t x_dtype, const int64_t* x_strides, v
                      int32_t OH, int32_t OW, int32_t dims, int32_t mode, float ratio_d, float ratio_h, float ratio_w,
                      void* stream);
 /* y = a + alpha * b on h16 buffers of n elements (ControlNet residual adds,
- * diffusion_model_unet.py:1917-1925,1931-1932; controlnet.py:405-407,433-434). */
+ * diffusion_model_unet.py:1917-1925,1931-1932; controlnet.py:405-407,433-434): h16(fma(alpha, b, a)) per element, over
+ * all n elements (pad channels included: they must be finite).  n % 8 == 0; a, b and y 16-byte aligned. */
 int b200_axpy_h16(const void* a, const void* b, float alpha, void* y, int64_t n, void* stream);
 /* Copy C channels of every row of a channels-last h16 tensor into columns [dst_off, dst_off + C) of another
- * (materialises torch.cat([a, b], dim=1) only where a raw concatenated tensor is really needed). */
+ * (materialises torch.cat([a, b], dim=1) only where a raw concatenated tensor is really needed).  The rest of each
+ * destination row is left untouched; source columns [C, src_pitch) are not read. */
 int b200_copy_channels(const void* src, int32_t C, int32_t src_pitch, void* dst, int32_t dst_pitch, int32_t dst_off,
                        int64_t rows, void* stream);
 /* Tap reformulations for the degenerate convolutions at either end of the UNet (DiffusionModelUNet.conv_in with one
@@ -355,13 +363,18 @@ int b200_copy_channels(const void* src, int32_t C, int32_t src_pitch, void* dst,
  * low-side zero padding).
  * tap_gather: out[v][tap*C + c] = x[in_voxel(v, tap)][c] (zero outside the input), v over N*OD*OH*OW, h16 rows.
  * tap_sum:    out[v][co] = bias[co] + sum_tap y[v + off(tap)][tap*cout + co], y fp32 rows over the INPUT grid
- *             (stride 1, cout <= 4); out h16 or fp32, columns [cout, out_pitch) zeroed. */
+ *             (stride 1, cout <= 4); out h16 or fp32, columns [cout, out_pitch) zeroed.
+ * tap = (kd_i * kh + kh_i) * kw + kw_i.  tap_gather is a copy; it writes the whole row [0, out_pitch) (columns past
+ * taps*C zero) and does not read x columns [C, x_pitch).  tap_sum adds in fp32 in tap order starting from the bias and
+ * rounds once on an h16 store; y columns [taps*cout, y_pitch) are not read. */
 int b200_tap_gather(const void* x, int32_t C, int32_t x_pitch, const int32_t* geom, void* out, int32_t out_pitch,
                     void* stream);
 int b200_tap_sum(const float* y, int32_t y_pitch, const int32_t* geom, int32_t cout, const float* bias, void* out,
                  int32_t out_pitch, int32_t out_dtype, void* stream);
 /* GEGLU: y[m, j] = x[m, j] * gelu_erf(x[m, H + j])  (monai MLPBlock act="GEGLU",
- * diffusion_model_unet.py:211). x: [M, 2H] pitch x_pitch; y: [M, H] pitch y_pitch. */
+ * diffusion_model_unet.py:211). x: [M, 2H] pitch x_pitch; y: [M, H] pitch y_pitch.  fp32 with erff, one rounding on
+ * the store.  Columns [H, y_pitch) of y are not written, columns [2H, x_pitch) of x not read.  M >= 1, H, x_pitch and
+ * y_pitch multiples of 8 (H >= 8), x and y 16-byte aligned. */
 int b200_geglu(const void* x, int64_t M, int32_t H, int32_t x_pitch, void* y, int32_t y_pitch,
                void* stream);
 /* softmax over rows of an fp32 [M, S] score matrix -> h16 probabilities [M, p_pitch]
@@ -417,11 +430,12 @@ int b200_attention_small_ex(const void* q, const void* k, const void* v, void* o
                             int32_t q_pos0, const int32_t* pos_dev, void* stream);
 /* Token + absolute position embedding rows (nets/transformer.py:20-37, 97-99):
  * out[m, :] = tok_emb[tokens[m], :] + pos_emb[pos0 + m % seq_len, :], h16 rows of pitch `pitch`
- * (pos0 = *pos_dev when pos_dev != NULL). */
+ * (pos0 = *pos_dev when pos_dev != NULL): one fp32 add, one rounding; pad columns [C, pitch) +0.  Precondition, not
+ * checked: every token id indexes a row of tok_emb and every pos0 + m % seq_len a row of pos_emb. */
 int b200_embed_tokens(const int64_t* tokens, int64_t M, int32_t seq_len, int32_t pos0, const float* tok_emb,
                       const float* pos_emb, int32_t C, void* out, int32_t pitch, const int32_t* pos_dev, void* stream);
 /* Graph-captured decoding: append T rows per sequence to a [B, L, pitch] h16 cache at the device-side position,
- * and advance that position. */
+ * and advance that position.  cache[b][pos + t] = src[b * T + t] (a copy); rows with pos + t outside [0, L) are dropped. */
 int b200_cache_append(const void* src, void* cache, int32_t B, int32_t T, int32_t L, int32_t pitch,
                       const int32_t* pos_dev, void* stream);
 int b200_advance_i32(int32_t* p, int32_t delta, void* stream);
@@ -444,10 +458,12 @@ int b200_attention_decode(const void* q, const void* k, const void* v, void* out
 /* ------------------------------------------------------------------------------------------------
  * Time embedding path (diffusion_model_unet.py:461-485, 1759-1767, 1888-1902; ResnetBlock 641,686).
  * ---------------------------------------------------------------------------------------------- */
-/* emb[n, :] = [cos(t_n f_i) ..., sin(t_n f_i) ...], f_i = exp(-ln(max_period) i / half), zero-pad if odd */
+/* emb[n, :] = [cos(t_n f_i) ..., sin(t_n f_i) ...], f_i = exp(-ln(max_period) i / half), zero-pad if odd
+ * (half = dim / 2; dim == 1 is all zeros).  fp32 logf / expf / cosf / sinf.  N * dim < 2^31. */
 int b200_timestep_embedding(const float* t, int32_t N, int32_t dim, float max_period, float* emb,
                             void* stream);
-/* y[m, o] = act_out( b[o] + sum_k act_in(x[m, k]) W[o, k] ), fp32, M <= 64 rows (GEMV-class). */
+/* y[m, o] = act_out( b[o] + sum_k act_in(x[m, k]) W[o, k] ), fp32 (GEMV-class: one warp per output feature loops over
+ * the rows; 1 <= M <= 4096).  b may be NULL.  Each lane sums its k in an fp32 fma chain, the lanes fold in a warp tree. */
 int b200_small_linear(const float* x, int32_t M, int32_t K, const float* W, const float* b, int32_t O,
                       int32_t act_in, int32_t act_out, float* y, void* stream);
 
@@ -484,7 +500,9 @@ int b200_ddpm_step(const float* model_out, const float* sample, const float* noi
 /* One timestep of DiffusionInferer.get_likelihood (inferer.py:205-265, 279-321), fused: from x_0 (inputs), x_t
  * (noisy) and the model output compute the predicted and posterior means, then the per-element KL between the two
  * normals (t > 0) or the discretised-Gaussian decoder negative log-likelihood (t == 0); kl_out (optional) receives
- * the per-element term, sample_sum[n] += sum over the sample's elements (fp64).  Fixed-variance schedulers. */
+ * the per-element fp32 term, sample_sum[n] += the fp64 sum of those fp32 terms over the sample's elements.  The
+ * summation order is unspecified (fp64 atomics across CTAs), so sample_sum can differ between calls in its last bits.
+ * Fixed-variance schedulers. */
 typedef struct {
   float sqrt_alpha_prod_t, sqrt_beta_prod_t;
   float coef_x0, coef_xt;              /* shared by the predicted mean (ddpm.py:235-240) and _get_mean (133-156)   */
@@ -525,7 +543,10 @@ int b200_add_noise(const float* x0, const float* noise, const float* ca, const f
 /* ------------------------------------------------------------------------------------------------
  * Vector quantiser (vector_quantizer.py:86-138): nearest codebook row under
  * d = |x|^2 + |e|^2 - 2 x.e (fp32), first index wins ties; writes int64 indices and optionally the
- * gathered rows.  x: fp32 [M, D] (channels-last); codebook fp32 [K, D].
+ * gathered rows.  x: fp32 [M, D] (channels-last, row pitch x_pitch; columns [D, x_pitch) not read); codebook fp32 [K, D].
+ * Order: |x|^2, |e|^2 and x.e are each one fma chain over d = 0 .. D-1 from 0, then d = (|x|^2 + |e|^2) - 2 x.e.
+ * A row whose distances are all NaN (or +inf) gets index 0.  sqerr_sum is added to with fp64 atomics (order
+ * unspecified).  D == 32 takes a register-tiled kernel with the same arithmetic (bit-identical indices).
  * ---------------------------------------------------------------------------------------------- */
 /* Optional outputs (NULL to skip): q_h16 rows (pitch q_pitch, pad zeroed) for the decoder; q_f32 [M, D] with the
  * straight-through rounding x + (q - x) when ste != 0 (vector_quantizer.py:186) else q; sqerr_sum += sum (q-x)^2
@@ -533,7 +554,8 @@ int b200_add_noise(const float* x0, const float* noise, const float* ca, const f
 int b200_vq_argmin_gather(const float* x, int64_t M, int32_t D, int32_t x_pitch, const float* codebook,
                           int32_t K, int64_t* indices, void* q_h16, int32_t q_pitch, float* q_f32,
                           int32_t ste, double* sqerr_sum, int32_t* hist, void* stream);
-/* nn.Embedding gather for decode_samples (vqvae.py:445-450): idx int64 [M] -> h16 rows. */
+/* nn.Embedding gather for decode_samples (vqvae.py:445-450): idx int64 [M] -> h16 rows (pad columns +0).  Indices
+ * outside [0, K - 1] are clamped into it. */
 int b200_vq_gather(const int64_t* indices, int64_t M, const float* codebook, int32_t K, int32_t D,
                    void* q_h16, int32_t q_pitch, void* stream);
 

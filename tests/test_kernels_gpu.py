@@ -451,6 +451,9 @@ def test_layernorm_geglu(cuda_device):
 
 # ------------------------------------------------------------------------------------------------ resampling
 def test_resample(cuda_device):
+    """Through the ops wrappers (layout conversion, pitch, allocation): the F.interpolate / avg_pool / a + alpha b
+    checks, and the contract of tests/elementwise_emulator.py on top (avgpool2 bit-exact, axpy one ulp)."""
+    from tests import elementwise_emulator as E
     ops = _ops()
     for shape in ((2, 16, 5, 6), (1, 24, 3, 4, 5)):
         x = torch.randn(shape)
@@ -461,9 +464,12 @@ def test_resample(cuda_device):
         pool = F.avg_pool2d if len(shape) == 4 else F.avg_pool3d
         got = ops.from_cl(ops.avgpool2(ops.to_cl(x.cuda())))
         assert_close(got, pool(bf(x), 2, 2), 1e-2, "avgpool2")
+        assert torch.equal(got.cpu().double(), E.h16(pool(bf(x).double(), 2, 2))), "avgpool2 is not bit-exact"
     a, b = torch.randn(1, 16, 4, 4), torch.randn(1, 16, 4, 4)
     got = ops.from_cl(ops.axpy(ops.to_cl(a.cuda()), ops.to_cl(b.cuda()), 0.75))
     assert_close(got, bf(a) + 0.75 * bf(b), 1e-2, "axpy")
+    want = E.axpy_h16(a.to(ops.H16).reshape(-1), b.to(ops.H16).reshape(-1), 0.75, a.numel())
+    assert E.excess(want, got.cpu().reshape(-1)).max() <= 1, "axpy outside one ulp of fma(alpha, b, a)"
 
 
 # ------------------------------------------------------------------------------------------------ attention
@@ -647,6 +653,8 @@ def test_attention_decode(cuda_device, B, S, heads, dh):
 
 # ------------------------------------------------------------------------------------------------ time embedding
 def test_timestep_embedding_and_small_linear(cuda_device):
+    """Through the ops wrappers: the fp32 restatements, and the contract of tests/elementwise_emulator.py on top."""
+    from tests import elementwise_emulator as E
     ops = _ops()
     t = torch.tensor([0.0, 1.0, 250.0, 999.0])
     for dim in (32, 33, 256):
@@ -659,17 +667,22 @@ def test_timestep_embedding_and_small_linear(cuda_device):
             ref = F.pad(ref, (0, 1))
         got = ops.timestep_embedding(t.cuda(), dim).cpu()
         assert (got - ref).abs().max().item() < 2e-4
+        assert E.excess(E.timestep_embedding(t, 4, dim, 10000.0), got).max() <= 1, dim
     x = torch.randn(3, 100)
     w, b = torch.randn(70, 100) / 10, torch.randn(70)
     ref = F.silu(F.linear(F.silu(x), w, b))
     got = ops.small_linear(x.cuda(), w.cuda(), b.cuda(), ops.ACT_SILU, ops.ACT_SILU).cpu()
     assert (got - ref).abs().max().item() < 1e-4
+    want = E.small_linear(x.reshape(-1), 3, 100, w.reshape(-1), b, 70, E.ACT_SILU, E.ACT_SILU)
+    assert E.excess(want, got).max() <= 1
     for K in (1024, 384, 2176):                    # K % 128 == 0: the float4 path (one / partial / three 1024-blocks)
         x = torch.randn(2, K)
         w, b = torch.randn(300, K) / math.sqrt(K), torch.randn(300)
         ref = F.linear(F.silu(x), w, b)
         got = ops.small_linear(x.cuda(), w.cuda(), b.cuda(), ops.ACT_SILU, ops.ACT_NONE).cpu()
         assert (got - ref).abs().max().item() < 1e-4, K
+        want = E.small_linear(x.reshape(-1), 2, K, w.reshape(-1), b, 300, E.ACT_SILU, E.ACT_NONE)
+        assert E.excess(want, got).max() <= 1, K
 
 
 # ------------------------------------------------------------------------------------------------ perf smoke (prints)
