@@ -133,7 +133,6 @@ SIGNATURES = {
     "b200_igemm": [C.POINTER(IgemmParams), _P],
     "b200_groupnorm_workspace_bytes": [_I32, _I64, _I32],
     "b200_groupnorm_stats": [C.POINTER(GnStatsParams), _P],
-    "b200_groupnorm_from_partials": [C.POINTER(GnStatsParams), _P, _P, _P],
     "b200_groupnorm_from_partials_ex": [C.POINTER(GnStatsParams), _P, _P, _P, _P],
     "b200_spade_apply": [C.POINTER(GnApplyParams), _P, _I32, _P, _P],
     "b200_resize_nearest": [_P, _I32, _I32, _I32, _I32, _I32, _P, _I32, _I32, _I32, _P],
@@ -151,7 +150,6 @@ SIGNATURES = {
     "b200_axpy_h16": [_P, _P, _F, _P, _I64, _P],
     "b200_copy_channels": [_P, _I32, _I32, _P, _I32, _I32, _I64, _P],
     "b200_geglu": [_P, _I64, _I32, _I32, _P, _I32, _P],
-    "b200_softmax_rows": [_P, _I64, _I32, _I64, _P, _I64, _P],
     "b200_softmax_rows_partials": [_P, _I64, _I32, _I64, _P, _I32, _P, _I64, _P],
     "b200_attention_small_ex": [_P, _P, _P, _P, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _I32, C.c_float, _I32,
                                 _I32, _I32, _P, _P],

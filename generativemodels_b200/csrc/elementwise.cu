@@ -473,49 +473,10 @@ __global__ void geglu_kernel(const h16* __restrict__ x, long long M, int H, int 
 }
 
 // ------------------------------------------------------------------------------------------------
-// Row softmax: fp32 scores -> bf16 probabilities. TPR threads cooperate on one row.
+// Row softmax: fp32 scores -> 16-bit probabilities.  The score GEMM's epilogue already left (max, sum exp) per
+// 128-column tile of every row, so the row maximum and denominator come from a few hundred partials and the scores
+// are read exactly once.
 // ------------------------------------------------------------------------------------------------
-template <int TPR>
-__global__ void softmax_rows_kernel(const float* __restrict__ s, long long M, int S, long long s_pitch,
-                                    h16* __restrict__ p, long long p_pitch) {
-  constexpr int RPB = 256 / TPR;
-  const long long row = (long long)blockIdx.x * RPB + threadIdx.x / TPR;
-  const int t = threadIdx.x % TPR;
-  __shared__ float red[8];
-  const bool live = row < M;
-  const float* sr = s + (live ? row : 0) * s_pitch;
-  float mx = -INFINITY;
-  if (live)
-    for (int c = t; c < S; c += TPR) mx = fmaxf(mx, sr[c]);
-  mx = warp_max(mx);
-  if constexpr (TPR > 32) {
-    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = mx;
-    __syncthreads();
-    mx = red[0];
-#pragma unroll
-    for (int i = 1; i < 8; ++i) mx = fmaxf(mx, red[i]);
-    __syncthreads();
-  }
-  float sum = 0.f;
-  if (live)
-    for (int c = t; c < S; c += TPR) sum += __expf(sr[c] - mx);
-  sum = warp_sum(sum);
-  if constexpr (TPR > 32) {
-    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = sum;
-    __syncthreads();
-    sum = 0.f;
-#pragma unroll
-    for (int i = 0; i < 8; ++i) sum += red[i];
-  }
-  if (!live) return;
-  const float inv = 1.0f / sum;
-  h16* pr = p + row * p_pitch;
-  for (int c = t; c < S; c += TPR) pr[c] = f2h(__expf(sr[c] - mx) * inv);
-  for (long long c = S + t; c < p_pitch; c += TPR) pr[c] = f2h(0.f);
-}
-
-// One-pass variant: the score GEMM's epilogue already left (max, sum exp) per 128-column tile of every row, so the
-// row maximum and denominator come from a few hundred partials and the scores are read exactly once.
 __global__ void softmax_rows_partials_kernel(const float* __restrict__ s, int S, long long s_pitch,
                                              const float2* __restrict__ part, int n_tiles,
                                              h16* __restrict__ p, long long p_pitch) {
@@ -1249,23 +1210,6 @@ extern "C" int b200_geglu(const void* x, int64_t M, int32_t H, int32_t x_pitch, 
   B200_CUDA(b200::launch_kernel(geglu_kernel, grid_for(M * (H / 8)), 256, 0, stream, reinterpret_cast<const h16*>(x), M, H, x_pitch,
                                                          reinterpret_cast<h16*>(y), y_pitch));
   B200_LAUNCH_CHECK("geglu_kernel");
-  return B200_OK;
-}
-
-extern "C" int b200_softmax_rows(const float* s, int64_t M, int32_t S, int64_t s_pitch, void* p, int64_t p_pitch,
-                                 void* stream_v) {
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
-  B200_CHECK_ARG(s && p && M >= 1 && S >= 1 && s_pitch >= S && p_pitch >= S, "softmax_rows: bad arguments");
-  h16* pp = reinterpret_cast<h16*>(p);
-  if (S <= 1024) {
-    const long long blocks = (M + 7) / 8;
-    B200_CHECK_ARG(blocks < (1ll << 31), "softmax_rows: too many rows");
-    B200_CUDA(b200::launch_kernel(softmax_rows_kernel<32>, (unsigned)blocks, 256, 0, stream, s, M, S, s_pitch, pp, p_pitch));
-  } else {
-    B200_CHECK_ARG(M < (1ll << 31), "softmax_rows: too many rows");
-    B200_CUDA(b200::launch_kernel(softmax_rows_kernel<256>, (unsigned)M, 256, 0, stream, s, M, S, s_pitch, pp, p_pitch));
-  }
-  B200_LAUNCH_CHECK("softmax_rows_kernel");
   return B200_OK;
 }
 

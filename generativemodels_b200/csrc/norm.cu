@@ -735,11 +735,6 @@ extern "C" int b200_groupnorm_from_partials_ex(const b200_gn_stats_params* p, co
   return B200_OK;
 }
 
-extern "C" int b200_groupnorm_from_partials(const b200_gn_stats_params* p, const float* const partial[2],
-                                            const int32_t slots[2], void* stream_v) {
-  return b200_groupnorm_from_partials_ex(p, partial, slots, nullptr, stream_v);
-}
-
 extern "C" int b200_groupnorm_apply(const b200_gn_apply_params* p, void* stream_v) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
   B200_CHECK_ARG(p && p->x_ptr[0] && p->affine && p->y_ptr, "gn_apply: null pointer");

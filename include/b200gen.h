@@ -136,7 +136,7 @@ typedef struct {
   /* Optional GroupNorm partial sums for whoever normalises this output next (nn.GroupNorm after every conv of the
    * ResnetBlock, diffusion_model_unet.py:623-684): gn_partial[n][slot][cout/8][2] += (sum, sum of squares) of the
    * stored h16 values per 8-channel group; the kernel uses slots [gn_slot0, gn_slot0 + 4 * SM count) of the
-   * gn_slots per sample, the caller zero-fills the buffer and b200_groupnorm_from_partials reduces it.
+   * gn_slots per sample, the caller zero-fills the buffer and b200_groupnorm_from_partials_ex reduces it.
    * Needs a h16, 16-byte-aligned output with cout % 32 == 0.  NULL to skip. */
   float*  gn_partial;
   int32_t gn_slots, gn_slot0;
@@ -201,17 +201,13 @@ int64_t b200_groupnorm_workspace_bytes(int32_t N, int64_t spatial, int32_t C_tot
  * memory), at most 1024 otherwise; B200_EINVAL beyond. */
 int b200_groupnorm_stats(const b200_gn_stats_params* p, void* stream);
 /* The same affine table from partial sums that b200_igemm left while it wrote the tensor(s) (see gn_partial there),
- * so the statistics pass over the activations disappears: source i contributes partial[i] = [N][slots[i]][x_C[i]/8][2].
- * x_ptr of p is not read; every group of the virtual concat must be a whole number of 8-channel producer groups
- * inside one source ((C0+C1)/groups % 8 == 0 and C0 % ((C0+C1)/groups) == 0).  The fold is fp64 over the fp32
+ * so the statistics pass over the activations disappears.  group[i] is the producer group width of source i
+ * (b200_igemm's gn_group: 8 or 4 channels per partial group; group NULL or an entry 0 = 8), and source i contributes
+ * partial[i] = [N][slots[i]][x_C[i] / group[i]][2].  x_ptr of p is not read; every group of the virtual concat must be
+ * a whole number of producer groups inside one source (C0 % ((C0+C1)/groups) == 0).  The fold is fp64 over the fp32
  * partials (mean = sum / n, var = sumsq / n - mean^2), exact to them up to fp64 rounding.  b200_igemm's partials are
  * raw fp32 sums of x and x^2, so unlike b200_groupnorm_stats this path loses rstd precision, about (mean / std)^2
  * 2^-24 times the terms per sum, when a group's mean is large against its spread. */
-int b200_groupnorm_from_partials(const b200_gn_stats_params* p, const float* const partial[2],
-                                 const int32_t slots[2], void* stream);
-/* The same with the producer group width of each source stated (b200_igemm's gn_group: 8 or 4 channels per partial
- * group): partial[i] = [N][slots[i]][x_C[i] / group[i]][2]; every consumer group must be a whole number of producer
- * groups inside one source. */
 int b200_groupnorm_from_partials_ex(const b200_gn_stats_params* p, const float* const partial[2],
                                     const int32_t slots[2], const int32_t group[2], void* stream);
 
@@ -378,11 +374,10 @@ int b200_tap_sum(const float* y, int32_t y_pitch, const int32_t* geom, int32_t c
 int b200_geglu(const void* x, int64_t M, int32_t H, int32_t x_pitch, void* y, int32_t y_pitch,
                void* stream);
 /* softmax over rows of an fp32 [M, S] score matrix -> h16 probabilities [M, p_pitch]
- * (attention_scores.softmax(dim=-1), diffusion_model_unet.py:150,412): p = h16(exp(s - max) * (1 / sum)), normalised
- * in fp32 before the one rounding.  Pad columns [S, p_pitch) are written +0; rows past M are not written. */
-int b200_softmax_rows(const float* s, int64_t M, int32_t S, int64_t s_pitch, void* p, int64_t p_pitch,
-                      void* stream);
-/* Same result in ONE pass over the scores, given the per-(row, 128-column tile) partials b200_igemm wrote. */
+ * (attention_scores.softmax(dim=-1), diffusion_model_unet.py:150,412) in ONE pass over the scores: the row maximum and
+ * sum come from the per-(row, 128-column tile) partials b200_igemm wrote (stat_ptr), n_tiles per row.
+ * p = h16(exp(s - max) * (1 / sum)), normalised in fp32 before the one rounding.  Pad columns [S, p_pitch) are
+ * written +0; rows past M are not written. */
 int b200_softmax_rows_partials(const float* s, int64_t M, int32_t S, int64_t s_pitch, const float* partials,
                                int32_t n_tiles, void* p, int64_t p_pitch, void* stream);
 

@@ -17,7 +17,7 @@ of the store:
                             one rounding.
   attention_small(_ex)      fp32 throughout, nothing rounded but the output; the causal horizon s <= q_pos0 + t,
   attention_decode          kv_rows, and pos_dev (q_pos0 = *pos, S = *pos + T; decode: S = *pos + 1).
-  softmax_rows(_partials)   p = h16(fp32(exp(s - max) * (1 / sum))); pad columns [S, p_pitch) are +0.
+  softmax_rows_partials     p = h16(fp32(exp(s - max) * (1 / sum))); pad columns [S, p_pitch) are +0.
 
 16-bit rounding goes through fp32 (`.to(torch.float32).to(H16)`), as the kernels round their fp32 values with RN; a
 direct float64 -> 16-bit conversion can round differently.  fp16 stores saturate at +-65504 (cvt.rn.satfinite).
@@ -49,55 +49,18 @@ is several times over it (tests/test_attention_emulator_cpu.py shows each such m
 """
 from __future__ import annotations
 
-import contextlib
 import math
 from dataclasses import dataclass
 
 import numpy as np
 import torch
 
-from generativemodels_b200._lib import ACT_DTYPE
+from tests.norm_emulator import F64, f32, h16, rows_of, storage, ulp16  # noqa: F401  (storage: the flavour switch)
 
-F64 = torch.float64
 LN2 = math.log(2.0)
 ACC_TC, ACC_CC = 2.0 ** -16, 2.0 ** -17
 REL = 2.0 ** -17
 FTZ = 2.0 ** -126
-
-H16 = torch.float16 if ACT_DTYPE == "fp16" else torch.bfloat16
-
-
-@contextlib.contextmanager
-def storage(dtype):
-    """Emulate the library flavour whose 16-bit type is `dtype` (torch.float16 or torch.bfloat16) inside the block."""
-    global H16
-    old, H16 = H16, dtype
-    try:
-        yield
-    finally:
-        H16 = old
-
-
-def _mant():
-    return 10 if H16 is torch.float16 else 7
-
-
-def f32(x):
-    return x.to(torch.float32).to(F64)
-
-
-def h16(x):
-    """fp32 -> 16-bit with round-to-nearest-even, as the kernels store; fp16 saturates at +-65504."""
-    x = x.to(torch.float32)
-    if H16 is torch.float16:
-        x = x.clamp(-65504.0, 65504.0)
-    return x.to(H16).to(F64)
-
-
-def ulp16(x):
-    emin = -14 if H16 is torch.float16 else -126
-    m = x.abs().clamp_min(2.0 ** emin)
-    return torch.exp2(torch.floor(torch.log2(m)) - _mant())
 
 
 @dataclass
@@ -204,11 +167,6 @@ def fp32_head(Q, K, V, scale, end=None, chain=None):
 # ----------------------------------------------------------------------------------------------------------------
 # the entry points
 # ----------------------------------------------------------------------------------------------------------------
-def _rows(buf, row0, n, pitch):
-    """Rows [row0, row0 + n) of a flat buffer of `pitch`-element rows, as a 2-D view."""
-    return buf[row0 * pitch:(row0 + n) * pitch].view(n, pitch)
-
-
 def _finish(exact, err, res_rows=None):
     if res_rows is not None:
         exact = exact + res_rows
@@ -218,19 +176,17 @@ def _finish(exact, err, res_rows=None):
 def _tensor_core(head_fn, q, k, vt, res, B, T, S, heads, dh, q_pitch, k_pitch, vt_pitch, res_pitch, rows):
     C = heads * dh
     rows = torch.arange(T) if rows is None else torch.as_tensor(rows)
+    Q = rows_of(q, B * T, q_pitch, C).view(B, T, C)[:, rows]
+    K = rows_of(k, B * S, k_pitch, C).view(B, S, C)
+    Vt = rows_of(vt, B * C, vt_pitch, S).view(B, C, S)
     exact = torch.zeros(B, len(rows), C, dtype=F64)
     err = torch.zeros_like(exact)
     for b in range(B):
-        Qb = _rows(q, b * T, T, q_pitch)[rows]
-        Kb = _rows(k, b * S, S, k_pitch)
         for h in range(heads):
             cs = slice(h * dh, (h + 1) * dh)
-            V = _rows(vt, b * C + h * dh, dh, vt_pitch)[:, :S].T.to(F64)
-            r = head_fn(Qb[:, cs].to(F64), Kb[:, cs].to(F64), V)
+            r = head_fn(Q[b, :, cs], K[b, :, cs], Vt[b, cs].T)
             exact[b, :, cs], err[b, :, cs] = r["o"], r["err"]
-    R = None
-    if res is not None:
-        R = torch.stack([_rows(res, b * T, T, res_pitch)[rows, :C].to(F64) for b in range(B)])
+    R = None if res is None else rows_of(res, B * T, res_pitch, C).view(B, T, C)[:, rows]
     return _finish(exact, err, R)
 
 
@@ -248,6 +204,12 @@ def unfused(q, k, vt, res, B, T, S, heads, dh, q_pitch, k_pitch, vt_pitch, res_p
     return _tensor_core(fn, q, k, vt, res, B, T, S, heads, dh, q_pitch, k_pitch, vt_pitch, res_pitch, rows)
 
 
+def _cache(buf, B, S, kv_rows, pitch, C):
+    """The first S rows of each batch item's kv_rows-row block of a [B][kv_rows][pitch] cache: [B, S, C] float64."""
+    flat = rows_of(buf, (B - 1) * kv_rows + S, pitch, C)
+    return torch.stack([flat[b * kv_rows:b * kv_rows + S] for b in range(B)])
+
+
 def small(q, k, v, B, T, S, heads, dh, q_pitch, k_pitch, v_pitch, scale, kv_rows=None, causal=0, q_pos0=0, pos=None):
     """b200_attention_small(_ex): q [B][T][q_pitch]; k, v [B][kv_rows][pitch] (S valid rows); pos = *pos_dev or None.
     Returns [B, T, heads*dh]."""
@@ -256,13 +218,14 @@ def small(q, k, v, B, T, S, heads, dh, q_pitch, k_pitch, v_pitch, scale, kv_rows
     kv_rows = S if kv_rows is None else kv_rows
     C = heads * dh
     end = torch.clamp(q_pos0 + torch.arange(T) + 1, max=S) if causal else None
+    Q = rows_of(q, B * T, q_pitch, C)
+    K, V = _cache(k, B, S, kv_rows, k_pitch, C), _cache(v, B, S, kv_rows, v_pitch, C)
     exact = torch.zeros(B, T, C, dtype=F64)
     err = torch.zeros_like(exact)
     for b in range(B):
-        Qb, Kb, Vb = _rows(q, b * T, T, q_pitch), _rows(k, b * kv_rows, S, k_pitch), _rows(v, b * kv_rows, S, v_pitch)
         for h in range(heads):
             cs = slice(h * dh, (h + 1) * dh)
-            r = fp32_head(Qb[:, cs].to(F64), Kb[:, cs].to(F64), Vb[:, cs].to(F64), scale, end)
+            r = fp32_head(Q[b * T:(b + 1) * T, cs], K[b, :, cs], V[b, :, cs], scale, end)
             exact[b, :, cs], err[b, :, cs] = r["o"], r["err"]
     return _finish(exact, err)
 
@@ -274,13 +237,14 @@ def decode(q, k, v, B, S, heads, dh, q_pitch, k_pitch, v_pitch, scale, kv_rows, 
         S = pos + 1
     C = heads * dh
     chain = torch.full((1, 1), float(-(-S // 8) + 8), dtype=F64)      # per-warp re-scales + the 8-way merge
+    Q = rows_of(q, B, q_pitch, C)
+    K, V = _cache(k, B, S, kv_rows, k_pitch, C), _cache(v, B, S, kv_rows, v_pitch, C)
     exact = torch.zeros(B, C, dtype=F64)
     err = torch.zeros_like(exact)
     for b in range(B):
-        Qb, Kb, Vb = _rows(q, b, 1, q_pitch), _rows(k, b * kv_rows, S, k_pitch), _rows(v, b * kv_rows, S, v_pitch)
         for h in range(heads):
             cs = slice(h * dh, (h + 1) * dh)
-            r = fp32_head(Qb[:, cs].to(F64), Kb[:, cs].to(F64), Vb[:, cs].to(F64), scale, chain=chain)
+            r = fp32_head(Q[b:b + 1, cs], K[b, :, cs], V[b, :, cs], scale, chain=chain)
             exact[b, cs], err[b, cs] = r["o"][0], r["err"][0]
     return _finish(exact, err)
 
@@ -301,21 +265,10 @@ def _softmax_result(x, m, tot, sum_err, S, p_pitch):
     return Result(exact, h16(exact), err, floor=0.0)
 
 
-def softmax_rows(s, M, S, s_pitch, p_pitch):
-    """b200_softmax_rows: fp32 scores [M][s_pitch] -> [M, p_pitch]."""
-    x = _rows(s, 0, M, s_pitch)[:, :S].to(F64)
-    m = x.amax(1, keepdim=True)
-    e = torch.exp(x - m)
-    e[e < FTZ] = 0.0
-    tot = e.sum(1, keepdim=True)
-    sum_err = ((2 + 1.2 * (x - m).abs()) * e).sum(1, keepdim=True) / tot * 2.0 ** -24 + (S / 32 + 16) * 2.0 ** -24
-    return _softmax_result(x, m, tot, sum_err, S, p_pitch)
-
-
 def softmax_rows_partials(s, M, S, s_pitch, partials, n_tiles, p_pitch):
     """b200_softmax_rows_partials: the row maximum and sum come from partials [M][n_tiles] of (max, sum exp(v - max))
     per 128-column tile ((-inf, 0) for a tile without columns), the scores are read once."""
-    x = _rows(s, 0, M, s_pitch)[:, :S].to(F64)
+    x = rows_of(s, M, s_pitch, S)
     part = partials[:M * n_tiles * 2].view(M, n_tiles, 2).to(F64)
     pm, ps = part[..., 0], part[..., 1]
     m = pm.amax(1, keepdim=True)

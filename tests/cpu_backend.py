@@ -1,17 +1,26 @@
-"""TEST-ONLY CPU stand-in for libb200gen.so: every C-ABI entry point re-implemented with numpy/torch on HOST pointers,
-following include/b200gen.h literally.  Installing it lets the `-m "not gpu"` suite drive the real host code
-(generativemodels_b200: modules, weight packing, schedulers, inferers, ctypes marshalling) end to end on a machine
-without a GPU.  It is never importable from the product package and proves nothing about the CUDA kernels — those are
-covered by the -m gpu tests against the oracle."""
+"""TEST-ONLY CPU stand-in for libb200gen.so: every C-ABI entry point on HOST pointers, so that the `-m "not gpu"` suite
+drives the real host code (generativemodels_b200: modules, weight packing, schedulers, inferers, ctypes marshalling) end
+to end on a machine without a GPU.  It is never importable from the product package.
+
+The stand-in is marshalling: each method views its pointers as flat host tensors, calls the float64 reading of the
+entry point that the GPU contract tests hold the kernels to (tests/{igemm,norm,attention,elementwise}_emulator.py) and
+stores that reading's rounded result.  Only the entry points or outputs those readings do not cover are restated
+here: the GEMV of rows_linear, the pooling, interpolation and BatchNorm-fold entry points of the discriminator, SPADE
+and rescaler networks, weight repacking, the position counter of advance_i32 and the host queries."""
 import ctypes as C
-import math
 
 import numpy as np
 import torch
 import torch.nn.functional as F
 
 from generativemodels_b200 import _lib, ops
+from tests import attention_emulator as A
+from tests import elementwise_emulator as W
 from tests import igemm_emulator as E
+from tests import norm_emulator as N
+from tests.rescaler_oracle import header_interpolate
+
+F64 = torch.float64
 
 
 def _obj(ref):
@@ -41,21 +50,50 @@ def rows16(ptr, n_rows, pitch, cols):
     return torch.as_strided(flat, (n_rows, cols), (pitch, 1))
 
 
+def dense16(ptr, n_rows, pitch, cols):
+    """rows16 copied to a flat buffer of `cols`-element rows (pass `cols` as the pitch)."""
+    return rows16(ptr, n_rows, pitch, cols).reshape(-1)
+
+
 def i64(ptr, count):
     a = _np(ptr, count, C.c_int64)
     return None if a is None else torch.from_numpy(a)
 
 
-def _act(x, a):
-    if a == _lib.ACT_LEAKYRELU:
-        return F.leaky_relu(x, 0.01)
-    if a == _lib.ACT_GELU:
-        return F.gelu(x)
-    if a == _lib.ACT_TANH:
-        return torch.tanh(x)
-    if a == _lib.ACT_SIGMOID:
-        return torch.sigmoid(x)
-    return F.relu(x) if a == _lib.ACT_RELU else F.silu(x) if a == _lib.ACT_SILU else x
+def store16(ptr, value):
+    bf16(ptr, value.numel()).copy_(value.reshape(-1).to(ops.H16))
+
+
+def store32(ptr, value):
+    f32(ptr, value.numel()).copy_(value.reshape(-1).to(torch.float32))
+
+
+def _sources(p):
+    """The two channels-last sources of a GroupNorm / SPADE parameter block as the norm reading takes them."""
+    rows = p.N * p.spatial
+    C1 = p.x_C[1] if p.x_ptr[1] else 0
+    x1 = bf16(p.x_ptr[1], rows * p.x_pitch[1]) if C1 else None
+    return bf16(p.x_ptr[0], rows * p.x_pitch[0]), x1, p.x_C[0], C1, p.x_pitch[0], p.x_pitch[1]
+
+
+def _store_table(ptr, t):
+    f32(ptr, t.a.numel() * 2).view(*t.a.shape, 2).copy_(torch.stack([t.a, t.b], -1))
+
+
+def _table_affine(tab):
+    """A [N, C, 2] affine table read from memory as the norm reading's Affine (one group per channel, no error)."""
+    a, b = tab[..., 0].to(F64), tab[..., 1].to(F64)
+    z = torch.zeros_like(a)
+    return N.Affine(a, b, z, z, z, z, z, z, z[:1])
+
+
+def _strided(ptr, dt, strides, shape):
+    count = 1 + sum((s - 1) * st for s, st in zip(shape, strides))
+    return torch.as_strided((bf16 if dt == _lib.DT_H16 else f32)(ptr, count), shape, strides)
+
+
+def _pos(pos_dev):
+    return int(_np(pos_dev, 1, C.c_int32)[0]) if pos_dev else None
 
 
 class FakeLib:
@@ -63,139 +101,109 @@ class FakeLib:
         E.emulate(_obj(p))
         return 0
 
-    def b200_groupnorm_workspace_bytes(self, N, spatial, C_):
+    def b200_groupnorm_workspace_bytes(self, N_, spatial, C_):
         return 16
 
-    def b200_nchw_to_nhwc(self, x, N, C_, sp, y, pitch, stream):
-        src = f32(x, N * C_ * sp).view(N, C_, sp)
-        dst = bf16(y, N * sp * pitch).view(N, sp, pitch)
-        dst.zero_()
-        dst[:, :, :C_] = src.transpose(1, 2).to(ops.H16)
+    def b200_nchw_to_nhwc(self, x, N_, C_, sp, y, pitch, stream):
+        store16(y, W.nchw_to_nhwc(f32(x, N_ * C_ * sp), N_, C_, sp, pitch).out)
         return 0
 
-    def b200_nhwc_to_nchw(self, x, dt, N, C_, sp, pitch, y, stream):
-        src = (bf16 if dt == _lib.DT_H16 else f32)(x, N * sp * pitch).view(N, sp, pitch)
-        f32(y, N * C_ * sp).view(N, C_, sp).copy_(src[:, :, :C_].float().transpose(1, 2))
+    def b200_nhwc_to_nchw(self, x, dt, N_, C_, sp, pitch, y, stream):
+        src = (bf16 if dt == _lib.DT_H16 else f32)(x, N_ * sp * pitch)
+        store32(y, W.nhwc_to_nchw(src, N_, C_, sp, pitch).out)
         return 0
-
-    def _gather_src(self, p):
-        xs = []
-        for i in range(2):
-            if p.x_ptr[i]:
-                xs.append(bf16(p.x_ptr[i], p.N * p.spatial * p.x_pitch[i]).view(p.N, p.spatial, p.x_pitch[i])
-                          [:, :, : p.x_C[i]].float())
-        return torch.cat(xs, 2)
 
     def b200_groupnorm_stats(self, p, stream):
         p = _obj(p)
-        x = self._gather_src(p)                       # [N, S, C]
-        N, S, Cc = x.shape
-        g = x.view(N, S, p.groups, Cc // p.groups)
-        mean = g.mean(dim=(1, 3), keepdim=True)
-        var = g.var(dim=(1, 3), unbiased=False, keepdim=True)
-        rstd = (var + p.eps).rsqrt()
-        gamma, beta = f32(p.gamma, Cc), f32(p.beta, Cc)
-        a = (rstd.expand(N, 1, p.groups, Cc // p.groups).reshape(N, Cc)) * gamma
-        b = beta - (mean.expand(N, 1, p.groups, Cc // p.groups).reshape(N, Cc)) * a
-        f32(p.affine, N * Cc * 2).view(N, Cc, 2).copy_(torch.stack([a, b], -1))
+        Cc = p.x_C[0] + (p.x_C[1] if p.x_ptr[1] else 0)
+        t = N.gn_stats(*_sources(p), p.N, p.spatial, p.groups, p.eps, f32(p.gamma, Cc), f32(p.beta, Cc))
+        _store_table(p.affine, t)
         return 0
 
     def b200_groupnorm_fused(self, sp, ap, stream):
         sp, ap = _obj(sp), _obj(ap)
         Cc = sp.x_C[0] + (sp.x_C[1] if sp.x_ptr[1] else 0)
         assert Cc % sp.groups == 0 and (not sp.x_ptr[1] or sp.x_C[0] % (Cc // sp.groups) == 0)
-        table = torch.empty(sp.N * Cc * 2, dtype=torch.float32)          # the fused kernel keeps this in registers
-        sp.affine, ap.affine = table.data_ptr(), table.data_ptr()
-        try:
-            self.b200_groupnorm_stats(C.byref(sp), stream)
-            return self.b200_groupnorm_apply(C.byref(ap), stream)
-        finally:
-            sp.affine, ap.affine = None, None
-
-    def b200_groupnorm_from_partials(self, p, partial, slots, stream):
-        return self.b200_groupnorm_from_partials_ex(p, partial, slots, None, stream)
+        r, _ = N.groupnorm(*_sources(sp), sp.N, sp.spatial, sp.groups, sp.eps, f32(sp.gamma, Cc), f32(sp.beta, Cc),
+                           ap.act, ap.y_pitch)
+        store16(ap.y_ptr, r.out)
+        return 0
 
     def b200_groupnorm_from_partials_ex(self, p, partial, slots, group, stream):
         p = _obj(p)
-        ptrs = [int(v) if v else 0 for v in partial]
+        Cs = [p.x_C[0], p.x_C[1] if partial[1] else 0]
         sl = [int(v) for v in slots]
         gws = [(int(v) or 8) for v in group] if group is not None else [8, 8]
-        N, G = p.N, p.groups
-        Cs = [p.x_C[0]] + ([p.x_C[1]] if ptrs[1] else [])
-        Cc = sum(Cs)
-        cpg = Cc // G
-        assert all(cpg % gw == 0 and gw in (8, 4) for gw in gws[:len(Cs)]) and Cs[0] % cpg == 0
-        sums = []
-        for ptr, nslot, Ci, gw in zip(ptrs, sl, Cs, gws):
-            part = f32(ptr, N * nslot * (Ci // gw) * 2).view(N, nslot, Ci // gw, 2).double().sum(1)   # [N, Ci/gw, 2]
-            sums.append(part.view(N, Ci // cpg, cpg // gw, 2).sum(2))
-        tot = torch.cat(sums, 1)                                                                      # [N, G, 2]
-        cnt = float(p.spatial) * cpg
-        mean = tot[..., 0] / cnt
-        var = (tot[..., 1] / cnt - mean * mean).clamp_min(0)
-        rstd = (var + p.eps).rsqrt()
-        gamma, beta = f32(p.gamma, Cc), f32(p.beta, Cc)
-        a = rstd.float().repeat_interleave(cpg, 1) * gamma
-        b = beta - mean.float().repeat_interleave(cpg, 1) * a
-        f32(p.affine, N * Cc * 2).view(N, Cc, 2).copy_(torch.stack([a, b], -1))
+        cpg = sum(Cs) // p.groups
+        assert all(cpg % gw == 0 and gw in (8, 4) for gw, Ci in zip(gws, Cs) if Ci) and Cs[0] % cpg == 0
+        parts = [f32(partial[i], p.N * sl[i] * (Cs[i] // gws[i]) * 2) if Cs[i] else None for i in range(2)]
+        t = N.gn_from_partials(parts, sl, gws, *Cs, p.N, p.spatial, p.groups, p.eps, f32(p.gamma, sum(Cs)),
+                               f32(p.beta, sum(Cs)))
+        _store_table(p.affine, t)
         return 0
 
     def b200_spade_apply(self, p, gb, gb_pitch, gb_affine, stream):
         p = _obj(p)
-        x = self._gather_src(p)                        # [N, S, C]
-        N, S, Cc = x.shape
-        ab = f32(p.affine, N * Cc * 2).view(N, 1, Cc, 2)
-        g = bf16(gb, N * S * gb_pitch).view(N, S, gb_pitch)[:, :, :2 * Cc].float()
-        gab = f32(gb_affine, N * 2 * Cc * 2).view(N, 1, 2 * Cc, 2)
-        g = g * gab[..., 0] + gab[..., 1]
-        y = _act((x * ab[..., 0] + ab[..., 1]) * (1 + g[..., :Cc]) + g[..., Cc:], p.act)
-        dst = bf16(p.y_ptr, N * S * p.y_pitch).view(N, S, p.y_pitch)
-        dst.zero_()
-        dst[:, :, :Cc] = y.to(ops.H16)
+        src = _sources(p)
+        Cc, S = src[2] + src[3], p.N * p.spatial
+        ax = f32(p.affine, p.N * Cc * 2).view(p.N, Cc, 2)
+        gba = f32(gb_affine, p.N * 2 * Cc * 2).view(p.N, 2 * Cc, 2)
+        r = N.spade(*src, p.N, p.spatial, ax, bf16(gb, S * gb_pitch), gb_pitch, gba, p.act, p.y_pitch)
+        store16(p.y_ptr, r.out)
         return 0
 
-    def b200_resize_nearest(self, x, N, D, H, W, pitch, y, OD, OH, OW, stream):
-        src = bf16(x, N * D * H * W * pitch).view(N, D, H, W, pitch).float().permute(0, 4, 1, 2, 3)
-        out = F.interpolate(src, size=(OD, OH, OW), mode="nearest").permute(0, 2, 3, 4, 1)
-        bf16(y, N * OD * OH * OW * pitch).view(N, OD, OH, OW, pitch).copy_(out.to(ops.H16))
+    def b200_resize_nearest(self, x, N_, D, H, W_, pitch, y, OD, OH, OW, stream):
+        store16(y, N.resize_nearest(bf16(x, N_ * D * H * W_ * pitch), N_, D, H, W_, pitch, OD, OH, OW))
         return 0
 
     def b200_groupnorm_apply(self, p, stream):
         p = _obj(p)
-        x = self._gather_src(p)
-        N, S, Cc = x.shape
-        ab = f32(p.affine, N * Cc * 2).view(N, 1, Cc, 2)
-        y = _act(x * ab[..., 0] + ab[..., 1], p.act)
-        dst = bf16(p.y_ptr, N * S * p.y_pitch).view(N, S, p.y_pitch)
-        dst.zero_()
-        dst[:, :, :Cc] = y.to(ops.H16)
+        src = _sources(p)
+        Cc = src[2] + src[3]
+        X = N.concat(*src, p.N, p.spatial)
+        tab = f32(p.affine, p.N * Cc * 2).view(p.N, Cc, 2)
+        store16(p.y_ptr, N.gn_output(X, _table_affine(tab), p.act, p.y_pitch).out)
         return 0
 
     def b200_layernorm(self, x, M, C_, xp, g, b, eps, y, yp, stream):
-        src = bf16(x, M * xp).view(M, xp)[:, :C_].float()
-        out = F.layer_norm(src, (C_,), f32(g, C_), f32(b, C_), eps)
-        dst = bf16(y, M * yp).view(M, yp)
-        dst.zero_()
-        dst[:, :C_] = out.to(ops.H16)
+        store16(y, N.layernorm(bf16(x, M * xp), M, C_, xp, f32(g, C_), f32(b, C_), eps, yp).out)
         return 0
 
-    def b200_upsample_nearest2x(self, x, N, D, H, W, pitch, dims, y, stream):
-        src = bf16(x, N * D * H * W * pitch).view(N, D, H, W, pitch)
-        o = src.repeat_interleave(2, 2).repeat_interleave(2, 3)
-        if dims == 3:
-            o = o.repeat_interleave(2, 1)
-        bf16(y, o.numel()).view(o.shape).copy_(o)
+    def b200_upsample_nearest2x(self, x, N_, D, H, W_, pitch, dims, y, stream):
+        store16(y, W.upsample_nearest2x(bf16(x, N_ * D * H * W_ * pitch), N_, D, H, W_, pitch, dims).out)
         return 0
 
-    def b200_avgpool2(self, x, N, D, H, W, pitch, dims, y, stream):
-        src = bf16(x, N * D * H * W * pitch).view(N, D, H, W, pitch).float().permute(0, 4, 1, 2, 3)
-        o = F.avg_pool3d(src, (2, 2, 2) if dims == 3 else (1, 2, 2)).permute(0, 2, 3, 4, 1).contiguous()
-        bf16(y, o.numel()).view(o.shape).copy_(o.to(ops.H16))
+    def b200_upsample2x_interp(self, x, N_, H, W_, pitch, mode, y, stream):
+        src = bf16(x, N_ * H * W_ * pitch).view(N_, H, W_, pitch).float().permute(0, 3, 1, 2)
+        m = "bilinear" if mode == _lib.INTERP_BILINEAR else "bicubic"
+        out = F.interpolate(src, scale_factor=2, mode=m).permute(0, 2, 3, 1)
+        store16(y, out)
+        return 0
+
+    def b200_avgpool2(self, x, N_, D, H, W_, pitch, dims, y, stream):
+        store16(y, W.avgpool2(bf16(x, N_ * D * H * W_ * pitch), N_, D, H, W_, pitch, dims).out)
+        return 0
+
+    def b200_pool_s2(self, x, N_, D, H, W_, pitch, dims, k, pad, mode, y, stream):
+        src = bf16(x, N_ * D * H * W_ * pitch).view(N_, D, H, W_, pitch).float().permute(0, 4, 1, 2, 3)
+        kk, pp, ss = ((k, k, k), (pad, pad, pad), 2) if dims == 3 else ((1, k, k), (0, pad, pad), (1, 2, 2))
+        if mode == _lib.POOL_AVG:
+            o = F.avg_pool3d(src, kk, ss, pp, count_include_pad=True)
+        else:
+            o = F.max_pool3d(src, kk, ss, pp)
+        store16(y, o.permute(0, 2, 3, 4, 1))
+        return 0
+
+    def b200_interpolate(self, x, xdt, xs, y, ydt, ys, N_, C_, D, H, W_, OD, OH, OW, dims, mode, rd, rh, rw, stream):
+        xs, ys = [int(v) for v in xs[:5]], [int(v) for v in ys[:5]]
+        src = _strided(x, xdt, xs, (N_, C_, D, H, W_)).float().reshape(N_, C_, *(D, H, W_)[3 - dims:])
+        out = header_interpolate(src, (OD, OH, OW)[3 - dims:], (rd, rh, rw)[3 - dims:], mode)
+        dst = _strided(y, ydt, ys, (N_, C_, OD, OH, OW))
+        dst.copy_(out.reshape(N_, C_, OD, OH, OW).to(dst.dtype))
         return 0
 
     def b200_axpy_h16(self, a, b, alpha, y, n, stream):
-        out = (bf16(a, n).float() + alpha * bf16(b, n).float()).to(ops.H16)
-        bf16(y, n).copy_(out)
+        store16(y, W.axpy_h16(bf16(a, n), bf16(b, n), alpha, n).out)
         return 0
 
     @staticmethod
@@ -203,69 +211,28 @@ class FakeLib:
         return [int(v) for v in (g if not hasattr(g, "_obj") else g._obj)][:16]
 
     def b200_tap_gather(self, x, C_, xp, geom, out, op, stream):
-        N, D, H, W, OD, OH, OW, kd, kh, kw, sd, sh, sw, pd, ph, pw = self._geom(geom)
-        src = bf16(x, N * D * H * W * xp).view(N, D, H, W, xp)[..., :C_].float()
-        big = F.pad(src, (0, 0, pw, kw + sw * OW, ph, kh + sh * OH, pd, kd + sd * OD))     # generous high-side zeros
-        dst = bf16(out, N * OD * OH * OW * op).view(N, OD, OH, OW, op)
-        dst.zero_()
-        tap = 0
-        for a in range(kd):
-            for b in range(kh):
-                for c in range(kw):
-                    win = big[:, a:a + sd * OD:sd, b:b + sh * OH:sh, c:c + sw * OW:sw, :]
-                    dst[..., tap * C_:(tap + 1) * C_] = win.to(ops.H16)
-                    tap += 1
+        g = self._geom(geom)
+        store16(out, W.tap_gather(bf16(x, g[0] * g[1] * g[2] * g[3] * xp), C_, xp, g, op).out)
         return 0
 
     def b200_tap_sum(self, y, yp, geom, cout, bias, out, op, odt, stream):
-        N, D, H, W, OD, OH, OW, kd, kh, kw, sd, sh, sw, pd, ph, pw = self._geom(geom)
-        yy = f32(y, N * D * H * W * yp).view(N, D, H, W, yp)
-        big = F.pad(yy, (0, 0, pw, kw + OW, ph, kh + OH, pd, kd + OD))
-        acc = torch.zeros(N, OD, OH, OW, cout)
-        if bias:
-            acc += f32(bias, cout)
-        tap = 0
-        for a in range(kd):
-            for b in range(kh):
-                for c in range(kw):
-                    acc += big[:, a:a + OD, b:b + OH, c:c + OW, tap * cout:(tap + 1) * cout]
-                    tap += 1
-        if odt == _lib.DT_H16:
-            dst = bf16(out, N * OD * OH * OW * op).view(N, OD, OH, OW, op)
-            dst.zero_()
-            dst[..., :cout] = acc.to(ops.H16)
-        else:
-            dst = f32(out, N * OD * OH * OW * op).view(N, OD, OH, OW, op)
-            dst.zero_()
-            dst[..., :cout] = acc
+        g = self._geom(geom)
+        r = W.tap_sum(f32(y, g[0] * g[1] * g[2] * g[3] * yp), yp, g, cout, f32(bias, cout), op, odt == _lib.DT_H16)
+        (store16 if odt == _lib.DT_H16 else store32)(out, r.out)
         return 0
 
     def b200_copy_channels(self, src, C_, sp, dst, dp, off, rows, stream):
-        bf16(dst, rows * dp).view(rows, dp)[:, off:off + C_] = bf16(src, rows * sp).view(rows, sp)[:, :C_]
+        out = W.copy_channels(bf16(src, rows * sp), C_, sp, rows).out
+        bf16(dst, rows * dp).view(rows, dp)[:, off:off + C_] = out.to(ops.H16)
         return 0
 
     def b200_geglu(self, x, M, H, xp, y, yp, stream):
-        src = bf16(x, M * xp).view(M, xp).float()
-        out = src[:, :H] * F.gelu(src[:, H:2 * H])
-        dst = bf16(y, M * yp).view(M, yp)
-        dst[:, :H] = out.to(ops.H16)
-        return 0
-
-    def b200_softmax_rows(self, s, M, S, sp, p, pp, stream):
-        sc = f32(s, M * sp).view(M, sp)[:, :S]
-        dst = bf16(p, M * pp).view(M, pp)
-        dst.zero_()
-        dst[:, :S] = torch.softmax(sc, -1).to(ops.H16)
+        rows16(y, M, yp, H).copy_(W.geglu(bf16(x, M * xp), M, H, xp).out.to(ops.H16))
         return 0
 
     def b200_softmax_rows_partials(self, s, M, S, sp, part, n_tiles, p, pp, stream):
-        sc = f32(s, M * sp).view(M, sp)[:, :S]
-        pt = f32(part, M * n_tiles * 2).view(M, n_tiles, 2)
-        mx = pt[:, :, 0].max(1)[0]
-        den = (pt[:, :, 1] * torch.exp(pt[:, :, 0] - mx[:, None])).nan_to_num(0.0).sum(1)
-        dst = bf16(p, M * pp).view(M, pp)
-        dst.zero_()
-        dst[:, :S] = (torch.exp(sc - mx[:, None]) / den[:, None]).to(ops.H16)
+        r = A.softmax_rows_partials(f32(s, M * sp), M, S, sp, f32(part, M * n_tiles * 2), n_tiles, pp)
+        store16(p, r.out)
         return 0
 
     def b200_sm_count(self):
@@ -279,61 +246,51 @@ class FakeLib:
 
     def b200_attention_flash(self, a, stream):
         a = _obj(a)
-        B, T, S, heads, dh = a.B, a.T, a.S, a.heads, a.dh
-        Cc = heads * dh
-        qq = rows16(a.q, B * T, a.q_pitch, Cc).float().view(B, T, heads, dh).transpose(1, 2)
-        kk = rows16(a.k, B * S, a.k_pitch, Cc).float().view(B, S, heads, dh).transpose(1, 2)
-        vv = bf16(a.vt, B * Cc * a.vt_pitch).view(B, Cc, a.vt_pitch)[:, :, :S].float().transpose(1, 2)
-        vv = vv.reshape(B, S, heads, dh).transpose(1, 2)
-        out = (torch.softmax(a.scale * qq @ kk.transpose(-1, -2), -1) @ vv).transpose(1, 2).reshape(B, T, Cc)
-        if a.res:
-            out = out + bf16(a.res, B * T * a.res_pitch).view(B, T, a.res_pitch)[:, :, :Cc].float()
-        bf16(a.out, B * T * a.out_pitch).view(B, T, a.out_pitch)[:, :, :Cc] = out.to(ops.H16)
+        B, T, S, Cc = a.B, a.T, a.S, a.heads * a.dh
+        res = dense16(a.res, B * T, a.res_pitch, Cc) if a.res else None
+        r = A.flash(dense16(a.q, B * T, a.q_pitch, Cc), dense16(a.k, B * S, a.k_pitch, Cc),
+                    dense16(a.vt, B * Cc, a.vt_pitch, S), res, B, T, S, a.heads, a.dh, Cc, Cc, S, Cc, a.scale)
+        rows16(a.out, B * T, a.out_pitch, Cc).copy_(r.out.view(B * T, Cc).to(ops.H16))
         return 0
 
     def b200_attention_small_ex(self, q, k, v, o, B, T, S, heads, dh, qp, kp, vp, op, scale, kv_rows, causal, q_pos0,
                                 pos_dev, stream):
-        if pos_dev:
-            q_pos0 = int(_np(pos_dev, 1, C.c_int32)[0])
-            S = q_pos0 + T
         Cc = heads * dh
-        qq = rows16(q, B * T, qp, Cc).float().view(B, T, heads, dh).transpose(1, 2)
-        kk = rows16(k, B * kv_rows, kp, Cc).float().view(B, kv_rows, Cc)[:, :S].reshape(B, S, heads, dh).transpose(1, 2)
-        vv = bf16(v, B * kv_rows * vp).view(B, kv_rows, vp)[:, :S, :Cc].float().view(B, S, heads, dh).transpose(1, 2)
-        sc = scale * qq @ kk.transpose(-1, -2)
-        if causal:
-            allowed = torch.arange(S)[None, :] <= (q_pos0 + torch.arange(T))[:, None]
-            sc = sc.masked_fill(~allowed, float("-inf"))
-        out = (torch.softmax(sc, -1) @ vv).transpose(1, 2).reshape(B, T, Cc)
-        bf16(o, B * T * op).view(B, T, op)[:, :, :Cc] = out.to(ops.H16)
+        r = A.small(dense16(q, B * T, qp, Cc), dense16(k, B * kv_rows, kp, Cc), dense16(v, B * kv_rows, vp, Cc), B, T,
+                    S, heads, dh, Cc, Cc, Cc, scale, kv_rows, causal, q_pos0, _pos(pos_dev))
+        rows16(o, B * T, op, Cc).copy_(r.out.view(B * T, Cc).to(ops.H16))
+        return 0
+
+    def b200_attention_small(self, q, k, v, o, B, T, S, heads, dh, qp, kp, vp, op, scale, stream):
+        return self.b200_attention_small_ex(q, k, v, o, B, T, S, heads, dh, qp, kp, vp, op, scale, S, 0, 0, None,
+                                            stream)
+
+    def b200_attention_decode(self, q, k, v, o, B, S, heads, dh, qp, kp, vp, op, scale, kv_rows, pos_dev, stream):
+        Cc = heads * dh
+        r = A.decode(dense16(q, B, qp, Cc), dense16(k, B * kv_rows, kp, Cc), dense16(v, B * kv_rows, vp, Cc), B, S,
+                     heads, dh, Cc, Cc, Cc, scale, kv_rows, _pos(pos_dev))
+        rows16(o, B, op, Cc).copy_(r.out.to(ops.H16))
         return 0
 
     def b200_rows_linear(self, x, xp, M, K, g, b, eps, w, wp, O, bias, act, res, rp, out, op, odt, stream):
-        xs = bf16(x, M * xp).view(M, xp)[:, :K].float()
-        if g:
-            xs = F.layer_norm(xs, (K,), f32(g, K), f32(b, K), eps).to(ops.H16).float()
-        W = bf16(w, O * wp).view(O, wp)[:, :K].float()
-        y = xs @ W.t()
+        """The LayerNorm prologue is the norm reading's; the GEMV is restated in float64."""
+        xs = dense16(x, M, xp, K)
+        xs = N.rows_linear_ln(xs, M, K, K, f32(g, K), f32(b, K), eps).out if g else xs.view(M, K).to(F64)
+        y = xs @ rows16(w, O, wp, K).to(F64).t()
         if bias:
-            y = y + f32(bias, O)
-        y = _act(y, act)
+            y = y + f32(bias, O).to(F64)
+        y = W.act(y, torch.zeros_like(y), act)[0]
         if res:
-            y = y + bf16(res, M * rp).view(M, rp)[:, :O].float()
+            y = y + rows16(res, M, rp, O).to(F64)
         if odt == _lib.DT_F32:
-            f32(out, M * op).view(M, op)[:, :O] = y
+            f32(out, M * op).view(M, op)[:, :O] = y.to(torch.float32)
         else:
-            bf16(out, M * op).view(M, op)[:, :O] = y.to(ops.H16)
+            rows16(out, M, op, O).copy_(N.h16(y).to(ops.H16))
         return 0
 
-    def b200_attention_decode(self, q, k, v, o, B, S, heads, dh, qp, kp, vp, op, scale, kv_rows, pos_dev, stream):
-        if pos_dev:
-            S = int(_np(pos_dev, 1, C.c_int32)[0]) + 1
-        return self.b200_attention_small_ex(q, k, v, o, B, 1, S, heads, dh, qp, kp, vp, op, scale, kv_rows, 0, 0, None,
-                                            stream)
-
     def b200_cache_append(self, src, cache, B, T, L, pitch, pos_dev, stream):
-        pos = int(_np(pos_dev, 1, C.c_int32)[0])
-        bf16(cache, B * L * pitch).view(B, L, pitch)[:, pos:pos + T] = bf16(src, B * T * pitch).view(B, T, pitch)
+        r = W.cache_append(bf16(src, B * T * pitch), bf16(cache, B * L * pitch), B, T, L, pitch, _pos(pos_dev))
+        store16(cache, r.out)
         return 0
 
     def b200_advance_i32(self, p, delta, stream):
@@ -342,162 +299,90 @@ class FakeLib:
 
     def b200_embed_tokens(self, tokens, M, seq_len, pos0, tok_emb, pos_emb, C_, out, pitch, pos_dev, stream):
         if pos_dev:
-            pos0 = int(_np(pos_dev, 1, C.c_int32)[0])
+            pos0 = _pos(pos_dev)
         tk = i64(tokens, M)
         V, Lmax = int(tk.max()) + 1, pos0 + seq_len
-        te = f32(tok_emb, V * C_).view(V, C_)
-        pe = f32(pos_emb, Lmax * C_).view(Lmax, C_)
-        pos = pos0 + torch.arange(M) % seq_len
-        dst = bf16(out, M * pitch).view(M, pitch)
-        dst.zero_()
-        dst[:, :C_] = (te[tk] + pe[pos]).to(ops.H16)
+        r = W.embed_tokens(tk, M, seq_len, pos0, f32(tok_emb, V * C_), f32(pos_emb, Lmax * C_), C_, pitch)
+        store16(out, r.out)
         return 0
 
-    def b200_attention_small(self, q, k, v, o, B, T, S, heads, dh, qp, kp, vp, op, scale, stream):
-        Cc = heads * dh
-        qq = bf16(q, B * T * qp).view(B, T, qp)[:, :, :Cc].float().view(B, T, heads, dh).transpose(1, 2)
-        kk = bf16(k, B * S * kp).view(B, S, kp)[:, :, :Cc].float().view(B, S, heads, dh).transpose(1, 2)
-        vv = bf16(v, B * S * vp).view(B, S, vp)[:, :, :Cc].float().view(B, S, heads, dh).transpose(1, 2)
-        out = (torch.softmax(scale * qq @ kk.transpose(-1, -2), -1) @ vv).transpose(1, 2).reshape(B, T, Cc)
-        bf16(o, B * T * op).view(B, T, op)[:, :, :Cc] = out.to(ops.H16)
+    def b200_timestep_embedding(self, t, N_, dim, max_period, emb, stream):
+        store32(emb, W.timestep_embedding(f32(t, N_), N_, dim, max_period).out)
         return 0
 
-    def b200_timestep_embedding(self, t, N, dim, max_period, emb, stream):
-        half = dim // 2
-        tt = f32(t, N)
-        exponent = -math.log(max_period) * torch.arange(0, half, dtype=torch.float32)
-        args = tt[:, None] * torch.exp(exponent / half)[None]
-        e = torch.cat([torch.cos(args), torch.sin(args)], -1)
-        if dim % 2:
-            e = F.pad(e, (0, 1))
-        f32(emb, N * dim).view(N, dim).copy_(e)
-        return 0
-
-    def b200_small_linear(self, x, M, K, W, b, O_, act_in, act_out, y, stream):
-        out = F.linear(_act(f32(x, M * K).view(M, K), act_in), f32(W, O_ * K).view(O_, K), f32(b, O_))
-        f32(y, M * O_).view(M, O_).copy_(_act(out, act_out))
+    def b200_small_linear(self, x, M, K, W_, b, O_, act_in, act_out, y, stream):
+        r = W.small_linear(f32(x, M * K), M, K, f32(W_, O_ * K), f32(b, O_), O_, act_in, act_out)
+        store32(y, r.out)
         return 0
 
     def b200_ddim_step(self, m, s, nz, c, prev, x0o, n, stream):
-        c = _obj(c)
-        mm, ss = f32(m, n), f32(s, n)
-        if c.prediction_type == _lib.PRED_EPSILON:
-            x0, eps = (ss - c.sqrt_beta_prod_t * mm) / c.sqrt_alpha_prod_t, mm
-        elif c.prediction_type == _lib.PRED_SAMPLE:
-            x0 = mm
-            eps = (ss - c.sqrt_alpha_prod_t * x0) / c.sqrt_beta_prod_t
-        else:
-            x0 = c.sqrt_alpha_prod_t * ss - c.sqrt_beta_prod_t * mm
-            eps = c.sqrt_alpha_prod_t * mm + c.sqrt_beta_prod_t * ss
-        if c.clip:
-            x0 = x0.clamp(c.clip_min, c.clip_max)
-        p = c.sqrt_alpha_prod_prev * x0 + c.dir_coef * eps
-        if nz:
-            p = p + c.sigma * f32(nz, n)
-        f32(prev, n).copy_(p)
+        rp, rx = W.ddim_step(f32(m, n), f32(s, n), f32(nz, n), _obj(c), n)
+        store32(prev, rp.out)
         if x0o:
-            f32(x0o, n).copy_(x0)
+            store32(x0o, rx.out)
         return 0
 
     def b200_ddpm_step(self, m, s, nz, pv, c, prev, x0o, n, stream):
-        c = _obj(c)
-        mm, ss = f32(m, n), f32(s, n)
-        if c.prediction_type == _lib.PRED_EPSILON:
-            x0 = (ss - c.sqrt_beta_prod_t * mm) / c.sqrt_alpha_prod_t
-        elif c.prediction_type == _lib.PRED_SAMPLE:
-            x0 = mm
-        else:
-            x0 = c.sqrt_alpha_prod_t * ss - c.sqrt_beta_prod_t * mm
-        if c.clip:
-            x0 = x0.clamp(c.clip_min, c.clip_max)
-        p = c.coef_x0 * x0 + c.coef_xt * ss
-        if nz:
-            sig = c.sigma
-            if c.var_mode == 1:
-                sig = f32(pv, n).sqrt()
-            elif c.var_mode == 2:
-                frac = (f32(pv, n) + 1) / 2
-                sig = (frac * c.max_log + (1 - frac) * c.min_log).sqrt()
-            p = p + sig * f32(nz, n)
-        f32(prev, n).copy_(p)
+        rp, rx = W.ddpm_step(f32(m, n), f32(s, n), f32(nz, n), f32(pv, n), _obj(c), n)
+        store32(prev, rp.out)
         if x0o:
-            f32(x0o, n).copy_(x0)
+            store32(x0o, rx.out)
         return 0
 
-    def b200_ddpm_kl(self, x0, xt, mo, c, kl_out, ssum, N, per, stream):
-        from oracle import torch_oracle as O
-        c = _obj(c)
-        a, s_, m = (f32(p, N * per).view(N, per) for p in (x0, xt, mo))
-        if c.prediction_type == _lib.PRED_EPSILON:
-            p0 = (s_ - c.sqrt_beta_prod_t * m) / c.sqrt_alpha_prod_t
-        elif c.prediction_type == _lib.PRED_SAMPLE:
-            p0 = m
-        else:
-            p0 = c.sqrt_alpha_prod_t * s_ - c.sqrt_beta_prod_t * m
-        if c.clip:
-            p0 = p0.clamp(-1, 1)
-        pred = c.coef_x0 * p0 + c.coef_xt * s_
-        if c.is_t0:
-            bw = c.bin_width
-            kl = -O.decoder_log_likelihood(a, pred, torch.tensor(0.5 * c.log_pred_var), (0, 1), (0, bw))
-        else:
-            post = c.coef_x0 * a + c.coef_xt * s_
-            kl = 0.5 * (-1.0 + c.log_pred_var - c.log_post_var + math.exp(c.log_post_var - c.log_pred_var)
-                        + (post - pred) ** 2 * math.exp(-c.log_pred_var))
+    def b200_ddpm_kl(self, x0, xt, mo, c, kl_out, ssum, N_, per, stream):
+        r, sums, _ = W.ddpm_kl(*(f32(p, N_ * per) for p in (x0, xt, mo)), _obj(c), N_, per)
         if kl_out:
-            f32(kl_out, N * per).view(N, per).copy_(kl)
-        _np(ssum, N, C.c_double)[:] += kl.double().sum(1).numpy()
+            store32(kl_out, r.out)
+        _np(ssum, N_, C.c_double)[:] += sums.numpy()
         return 0
 
     def b200_pndm_step(self, hist, s, c, prev, eps_out, n, stream):
         c = _obj(c)
-        e = torch.zeros(n)
-        for k in range(c.n_hist):
-            e = e + c.w[k] * f32(hist[k], n)
+        rp, re = W.pndm_step([f32(hist[k], n) for k in range(c.n_hist)], f32(s, n) if prev else None, c, n)
         if eps_out:
-            f32(eps_out, n).copy_(e)
+            store32(eps_out, re.out)
         if prev:
-            ss = f32(s, n)
-            if c.prediction_type == _lib.PRED_V:
-                e = c.v_alpha * e + c.v_beta * ss
-            f32(prev, n).copy_(c.sample_coeff * ss - c.eps_coeff * e)
+            store32(prev, rp.out)
         return 0
 
-    def b200_add_noise(self, x0, nz, ca, cb, sign_b, N, per, out, stream):
-        a, b = f32(ca, N)[:, None], f32(cb, N)[:, None] * sign_b
-        f32(out, N * per).view(N, per).copy_(a * f32(x0, N * per).view(N, per) + b * f32(nz, N * per).view(N, per))
+    def b200_add_noise(self, x0, nz, ca, cb, sign_b, N_, per, out, stream):
+        r = W.add_noise(f32(x0, N_ * per), f32(nz, N_ * per), f32(ca, N_), f32(cb, N_), sign_b, N_, per)
+        store32(out, r.out)
         return 0
 
     def b200_exp_half_clamped(self, x, lo, hi, y, n, stream):
-        f32(y, n).copy_(torch.exp(f32(x, n).clamp(lo, hi) / 2))
+        store32(y, W.exp_half_clamped(f32(x, n), lo, hi, n).out)
         return 0
 
     def b200_fma_f32(self, a, b, c, y, n, stream):
-        f32(y, n).copy_(f32(a, n) + f32(b, n) * f32(c, n))
+        store32(y, W.fma_f32(f32(a, n), f32(b, n), f32(c, n), n).out)
         return 0
 
     def b200_scale_f32(self, x, mul, div, y, n, stream):
-        f32(y, n).copy_(f32(x, n) * mul / div)
+        store32(y, W.scale_f32(f32(x, n), mul, div, n).out)
+        return 0
+
+    def b200_vae_reparam_kld(self, mu, lv, eps, z, kld, n, stream):
+        rz, rk = W.vae_reparam_kld(f32(mu, n), f32(lv, n), f32(eps, n), n)
+        store32(z, rz.out)
+        store32(kld, rk.out)
         return 0
 
     def b200_vq_argmin_gather(self, x, M, D, xp, cb, K, idx, q16, qp, q32, ste, sq, hist, stream):
-        xx = f32(x, M * xp).view(M, xp)[:, :D]
-        cbk = f32(cb, K * D).view(K, D)
-        d = (xx ** 2).sum(1, keepdim=True) + (cbk.t() ** 2).sum(0, keepdim=True) - 2 * xx @ cbk.t()
-        ii = torch.max(-d, 1)[1]
-        i64(idx, M).copy_(ii)
-        qv = cbk[ii]
+        v = W.vq_argmin_gather(f32(x, M * xp), M, D, xp, f32(cb, K * D), K, qp, ste)
+        i64(idx, M).copy_(v.idx)
         if q16:
-            dst = bf16(q16, M * qp).view(M, qp)
-            dst.zero_()
-            dst[:, :D] = qv.to(ops.H16)
+            store16(q16, v.q16)
         if q32:
-            f32(q32, M * D).view(M, D).copy_(xx + (qv - xx) if ste else qv)
+            store32(q32, v.q32)
         if sq:
-            _np(sq, 1, C.c_double)[0] += float(((qv - xx).double() ** 2).sum())
+            _np(sq, 1, C.c_double)[0] += v.sqerr
         if hist:
-            h = _np(hist, K, C.c_int32)
-            h += np.bincount(ii.numpy(), minlength=K).astype(np.int32)
+            _np(hist, K, C.c_int32)[:] += v.hist.numpy().astype(np.int32)
+        return 0
+
+    def b200_vq_gather(self, idx, M, cb, K, D, q16, qp, stream):
+        store16(q16, W.vq_gather(i64(idx, M), M, f32(cb, K * D), K, D, qp).out)
         return 0
 
     def b200_repack_weight(self, src, cout, cin, taps, transposed, mode, blocks, n_blocks, dst, rows_pad, pitch, stream):
@@ -521,10 +406,12 @@ class FakeLib:
         bf16(dst, rows_pad * pitch).view(rows_pad, pitch).copy_(out.to(ops.H16))
         return 0
 
-    def b200_vq_gather(self, idx, M, cb, K, D, q16, qp, stream):
-        dst = bf16(q16, M * qp).view(M, qp)
-        dst.zero_()
-        dst[:, :D] = f32(cb, K * D).view(K, D)[i64(idx, M)].to(ops.H16)
+    def b200_batchnorm_fold(self, w, b, gamma, beta, mean, var, eps, cout, per, w_out, b_out, stream):
+        s = f32(gamma, cout).double() / (f32(var, cout).double() + eps).sqrt()
+        ww = f32(w, cout * per).view(cout, per).double()
+        bb = f32(b, cout).double() if b else torch.zeros(cout, dtype=torch.float64)
+        f32(w_out, cout * per).view(cout, per).copy_(ww * s[:, None])
+        f32(b_out, cout).copy_(f32(beta, cout).double() + (bb - f32(mean, cout).double()) * s)
         return 0
 
 
@@ -535,15 +422,18 @@ def install(monkeypatch):
     monkeypatch.setattr(ops, "_stream", lambda: 0)
     monkeypatch.setattr(ops, "igemm_raw", E.emulate)
     import generativemodels_b200.networks._holders as H
-    import generativemodels_b200.networks.nets.autoencoderkl as A
+    import generativemodels_b200.networks.blocks.encoder_modules as EM
+    import generativemodels_b200.networks.nets.autoencoderkl as AK
     import generativemodels_b200.networks.nets.controlnet as CN
     import generativemodels_b200.networks.nets.diffusion_model_unet as U
+    import generativemodels_b200.networks.nets.patchgan_discriminator as PG
+    import generativemodels_b200.networks.nets.spade_network as SN
     import generativemodels_b200.networks.nets.vqvae as V
     import generativemodels_b200.networks.schedulers.scheduler as S
     import generativemodels_b200.networks.schedulers.ddim as S1
     import generativemodels_b200.networks.schedulers.ddpm as S2
     import generativemodels_b200.networks.schedulers.pndm as S3
-    for mod in (H, A, CN, U, V):
+    for mod in (H, AK, CN, U, V, PG, SN, EM):
         monkeypatch.setattr(mod, "require_cuda", lambda x, m: None, raising=False)
 
     def prep(*tensors):

@@ -6,8 +6,8 @@ import ctypes as C
 
 import numpy as np
 
-from generativemodels_b200._lib import (ACT_DTYPE, ACT_GEGLU, ACT_GELU, ACT_LEAKYRELU, ACT_RELU, ACT_SIGMOID, ACT_SILU, ACT_TANH,
-                                         DT_H16, IgemmParams)
+from generativemodels_b200._lib import (ACT_DTYPE, ACT_GEGLU, ACT_GELU, ACT_LEAKYRELU, ACT_LEAKYRELU02, ACT_RELU, ACT_SIGMOID,
+                                         ACT_SILU, ACT_TANH, DT_H16, IgemmParams)
 
 
 def _bf16_view(ptr, count):
@@ -44,6 +44,8 @@ def _act(x, a):
         return x / (1 + np.exp(-x))
     if a == ACT_LEAKYRELU:
         return np.where(x > 0, x, np.float32(0.01) * x)
+    if a == ACT_LEAKYRELU02:
+        return np.where(x > 0, x, np.float32(0.2) * x)
     if a == ACT_TANH:
         return np.tanh(x)
     if a == ACT_SIGMOID:

@@ -4,16 +4,13 @@ F.conv, F.batch_norm with the running statistics, F.instance_norm, F.avg_pool / 
 against the unmodified reference and the committed fixture (tests/golden/g_patchgan.pt) by tests/test_patchgan_cpu.py;
 the CUDA path is checked against both.
 
-Also the name-seeded weights the fixture uses (:func:`seeded_weights`) and a CPU stand-in for the two library entry
-points the discriminators add (:func:`install`)."""
+Also the name-seeded weights the fixture uses (:func:`seeded_weights`)."""
 from __future__ import annotations
 
 import zlib
 
 import torch
 import torch.nn.functional as F
-
-from generativemodels_b200 import _lib
 
 LEAKY02 = ("LEAKYRELU", {"negative_slope": 0.2})
 
@@ -121,36 +118,3 @@ def input_of(rec):
         x = x.repeat_interleave(rec["repeat"], d)
     return x
 
-
-# ---------------------------------------------------------------------------------------------------------------------
-# CPU stand-in for the new entry points (tests only)
-# ---------------------------------------------------------------------------------------------------------------------
-def install(monkeypatch):
-    """tests/cpu_backend.install plus b200_pool_s2 and b200_batchnorm_fold, restated from include/b200gen.h."""
-    from tests import cpu_backend as CB
-    import generativemodels_b200.networks.nets.patchgan_discriminator as PG
-    from tests import spadenet_oracle as SO
-    fake = SO.install(monkeypatch)                       # LeakyReLU(0.2) in the stand-in and the igemm emulator
-
-    def pool_s2(x, N, D, H, W, pitch, dims, k, pad, mode, y, stream):
-        src = CB.bf16(x, N * D * H * W * pitch).view(N, D, H, W, pitch).float().permute(0, 4, 1, 2, 3)
-        kk, pp, ss = ((k, k, k), (pad, pad, pad), 2) if dims == 3 else ((1, k, k), (0, pad, pad), (1, 2, 2))
-        if mode == _lib.POOL_AVG:
-            o = F.avg_pool3d(src, kk, ss, pp, count_include_pad=True)
-        else:
-            o = F.max_pool3d(src, kk, ss, pp)
-        o = o.permute(0, 2, 3, 4, 1).contiguous()
-        CB.bf16(y, o.numel()).view(o.shape).copy_(o.to(CB.ops.H16))
-        return 0
-
-    def batchnorm_fold(w, b, gamma, beta, mean, var, eps, cout, per, w_out, b_out, stream):
-        s = CB.f32(gamma, cout).double() / (CB.f32(var, cout).double() + eps).sqrt()
-        ww = CB.f32(w, cout * per).view(cout, per).double()
-        bb = CB.f32(b, cout).double() if b else torch.zeros(cout, dtype=torch.float64)
-        CB.f32(w_out, cout * per).view(cout, per).copy_(ww * s[:, None])
-        CB.f32(b_out, cout).copy_(CB.f32(beta, cout).double() + (bb - CB.f32(mean, cout).double()) * s)
-        return 0
-    fake.b200_pool_s2 = pool_s2
-    fake.b200_batchnorm_fold = batchnorm_fold
-    monkeypatch.setattr(PG, "require_cuda", lambda x, m: None)
-    return fake

@@ -2,8 +2,8 @@
 
 ``header_interpolate`` evaluates include/b200gen.h's b200_interpolate rules literally (per-axis fp32 coordinates, then
 one dense weight matrix per resampled axis, applied in float64): tests/test_spatial_rescaler_cpu.py pins it against
-F.interpolate, which pins the documented rules to ATen's.  ``install`` makes it the CPU stand-in of the entry point
-(extending tests/cpu_backend.py), so the module's host code runs end to end without a GPU.  ``rescaler`` is the module
+F.interpolate, which pins the documented rules to ATen's; tests/cpu_backend.py stands it in for the entry point, so
+the module's host code runs end to end without a GPU.  ``rescaler`` is the module
 itself in plain PyTorch, from a ``state_dict`` and the constructor arguments.  Test infrastructure only."""
 from __future__ import annotations
 
@@ -73,32 +73,6 @@ def header_interpolate(x: torch.Tensor, out_sizes, ratios, mode: int) -> torch.T
         m = torch.from_numpy(axis_weights(mode, x.shape[2 + a], out_sizes[a], ratios[a]))
         y = torch.movedim(torch.tensordot(y, m, dims=([2 + a], [1])), -1, 2 + a)
     return y.float()
-
-
-def _strided(ptr, dt, strides, shape):
-    from tests import cpu_backend as CB
-    count = 1 + sum((s - 1) * st for s, st in zip(shape, strides))
-    flat = (CB.bf16 if dt == _lib.DT_H16 else CB.f32)(ptr, count)
-    return torch.as_strided(flat, shape, strides)
-
-
-def install(monkeypatch):
-    """tests/cpu_backend.install plus b200_interpolate (header_interpolate on the strided host buffers) and the
-    encoder_modules CUDA guard lifted."""
-    from tests import cpu_backend as CB
-    import generativemodels_b200.networks.blocks.encoder_modules as EM
-    fake = CB.install(monkeypatch)
-
-    def interpolate(x, xdt, xs, y, ydt, ys, N, C_, D, H, W, OD, OH, OW, dims, mode, rd, rh, rw, stream):
-        xs, ys = [int(v) for v in xs[:5]], [int(v) for v in ys[:5]]
-        src = _strided(x, xdt, xs, (N, C_, D, H, W)).float().reshape(N, C_, *(D, H, W)[3 - dims:])
-        out = header_interpolate(src, (OD, OH, OW)[3 - dims:], (rd, rh, rw)[3 - dims:], mode)
-        dst = _strided(y, ydt, ys, (N, C_, OD, OH, OW))
-        dst.copy_(out.reshape(N, C_, OD, OH, OW).to(dst.dtype))
-        return 0
-    fake.b200_interpolate = interpolate
-    monkeypatch.setattr(EM, "require_cuda", lambda x, m: None)
-    return fake
 
 
 def rescaler(sd: dict, x: torch.Tensor, n_stages: int = 1, size=None, method: str = "bilinear",

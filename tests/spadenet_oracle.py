@@ -1,17 +1,11 @@
 """Plain-PyTorch restatement of SPADENet (generative/networks/nets/spade_network.py) from a ``state_dict`` and the
 constructor arguments, pinned against the unmodified reference by tests/test_spadenet_cpu.py.  Test infrastructure: the
-CUDA path is checked against this and against the committed fixture tests/golden/g_spadenet.pt.
-
-Also a CPU stand-in for the library's SPADENet entry points (:func:`install`), extending tests/cpu_backend.py with
-``B200_ACT_LEAKYRELU02``, ``b200_upsample2x_interp`` and ``b200_vae_reparam_kld`` so that the host code of the module
-(weight permutations, shapes, the GAN path) runs end to end without a GPU."""
+CUDA path is checked against this and against the committed fixture tests/golden/g_spadenet.pt."""
 from __future__ import annotations
 
 import numpy as np
 import torch
 import torch.nn.functional as F
-
-from generativemodels_b200 import _lib
 
 
 def _conv(sd, p, x, stride=1, padding=None):
@@ -81,51 +75,6 @@ def spadenet_vae(sd, seg, x, eps, depth, upsampling_mode="nearest", last_act=0.2
     latent = [s // 2 ** depth for s in x.shape[2:]]
     img = decoder(sd, seg, z, c0, latent, depth, False, upsampling_mode, last_act)
     return img, kld(mu, logvar), mu, logvar, z
-
-
-# ---------------------------------------------------------------------------------------------------------------------
-# CPU stand-in for the new entry points (tests only)
-# ---------------------------------------------------------------------------------------------------------------------
-def patch_emulator(monkeypatch):
-    """Teach tests/igemm_emulator.py's activation table B200_ACT_LEAKYRELU02 (x > 0 ? x : 0.2 x, in float32 like its
-    LeakyReLU(0.01)) for the duration of one test; every other code keeps the emulator's own arithmetic."""
-    from tests import igemm_emulator as E
-    plain = E._act
-
-    def act(x, a):
-        return np.where(x > 0, x, np.float32(0.2) * x) if a == _lib.ACT_LEAKYRELU02 else plain(x, a)
-    monkeypatch.setattr(E, "_act", act)
-
-
-def install(monkeypatch):
-    """tests/cpu_backend.install plus the SPADENet entry points and activation code (in the CPU stand-in and in the
-    igemm emulator it routes b200_igemm to)."""
-    from tests import cpu_backend as CB
-    import generativemodels_b200.networks.nets.spade_network as SN
-    fake = CB.install(monkeypatch)
-    plain_act = CB._act
-
-    def act(x, a):
-        return F.leaky_relu(x, 0.2) if a == _lib.ACT_LEAKYRELU02 else plain_act(x, a)
-    monkeypatch.setattr(CB, "_act", act)
-
-    def upsample2x_interp(x, N, H, W, pitch, mode, y, stream):
-        src = CB.bf16(x, N * H * W * pitch).view(N, H, W, pitch).float().permute(0, 3, 1, 2)
-        m = "bilinear" if mode == _lib.INTERP_BILINEAR else "bicubic"
-        out = F.interpolate(src, scale_factor=2, mode=m).permute(0, 2, 3, 1)
-        CB.bf16(y, out.numel()).view(out.shape).copy_(out.to(CB.ops.H16))
-        return 0
-
-    def vae_reparam_kld(mu, lv, eps, z, out, n, stream):
-        m, l, e = CB.f32(mu, n), CB.f32(lv, n), CB.f32(eps, n)
-        CB.f32(z, n).copy_(e * torch.exp(0.5 * l) + m)
-        CB.f32(out, 1)[0] = float(-0.5 * (1 + l.double() - m.double() ** 2 - l.double().exp()).sum())
-        return 0
-    patch_emulator(monkeypatch)
-    fake.b200_upsample2x_interp = upsample2x_interp
-    fake.b200_vae_reparam_kld = vae_reparam_kld
-    monkeypatch.setattr(SN, "require_cuda", lambda x, m: None)
-    return fake
 
 
 def randomize(module, seed=0):

@@ -23,6 +23,16 @@ def test_library_exports_every_declared_symbol():
     assert lib.b200_version() >= 100
 
 
+def test_cpu_stand_in_covers_every_entry_point():
+    """tests/cpu_backend.FakeLib has a method for every entry point the host code can call, so the CPU suite never
+    needs a per-network extension of it; the host queries (version, errors, ABI, planning) are the exception."""
+    from tests.cpu_backend import FakeLib
+    host_queries = {"b200_version", "b200_last_error_string", "b200_act_dtype", "b200_device_check", "b200_abi_sizeof",
+                    "b200_igemm_plan"}
+    missing = sorted(n for n in set(_lib.SIGNATURES) - host_queries if not callable(getattr(FakeLib, n, None)))
+    assert not missing, missing
+
+
 def test_struct_sizes_match():
     lib = _lib.load()
     import ctypes as C

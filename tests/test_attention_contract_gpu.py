@@ -416,7 +416,7 @@ def test_attention_decode_matches_emulator(cuda_device, lib, case):
 
 
 # ------------------------------------------------------------------------------------------------------------------
-# b200_softmax_rows and b200_softmax_rows_partials
+# b200_softmax_rows_partials
 # ------------------------------------------------------------------------------------------------------------------
 @dataclass(frozen=True)
 class Softmax:
@@ -425,21 +425,15 @@ class Softmax:
     S: int
     s_pitch: int
     p_pitch: int
-    partials: bool = False
     s_off: int = 0                # element offset of the score pointer (misaligned: the scalar path)
 
 
 SOFTMAX = [
-    Softmax("rows_S1_M20", 20, 1, 1, 8),
-    Softmax("rows_S3_M37_multiblock", 37, 3, 5, 4),
-    Softmax("rows_S1024_narrow_kernel", 19, 1024, 1024, 1032),
-    Softmax("rows_S1025_wide_kernel", 5, 1025, 1027, 1025),
-    Softmax("rows_S5000_wide_kernel", 3, 5000, 5000, 5008),
-    Softmax("partials_float4_S1001_tail", 9, 1001, 1004, 1008, partials=True),
-    Softmax("partials_float4_S7_M300", 300, 7, 8, 8, partials=True),
-    Softmax("partials_scalar_odd_s_pitch", 10, 130, 131, 136, partials=True),
-    Softmax("partials_scalar_p_pitch_not_4", 4, 257, 260, 258, partials=True),
-    Softmax("partials_scalar_misaligned_scores", 6, 203, 204, 208, partials=True, s_off=1),
+    Softmax("partials_float4_S1001_tail", 9, 1001, 1004, 1008),
+    Softmax("partials_float4_S7_M300", 300, 7, 8, 8),
+    Softmax("partials_scalar_odd_s_pitch", 10, 130, 131, 136),
+    Softmax("partials_scalar_p_pitch_not_4", 4, 257, 260, 258),
+    Softmax("partials_scalar_misaligned_scores", 6, 203, 204, 208, s_off=1),
 ]
 
 
@@ -451,32 +445,26 @@ def softmax_operands(c: Softmax):
         x[1] = torch.where(torch.arange(c.S) % 3 == 0, 1e4, -1e4)
     s = torch.full((c.s_off + (c.M + 1) * c.s_pitch,), NAN)
     s[c.s_off:c.s_off + c.M * c.s_pitch].view(c.M, c.s_pitch)[:, :c.S] = x
-    t = {"s": s, "out": sentinel((c.M + 2) * c.p_pitch)}
-    if c.partials:
-        # the igemm stat_ptr contract: (max, sum exp(v - max)) per 128-column tile of the fp32 row, plus a trailing
-        # tile without columns, (-inf, 0)
-        nt = (c.S + 127) // 128 + 1
-        part = torch.zeros(c.M, nt, 2)
-        xd = x.double()
-        for i in range(nt):
-            seg = xd[:, i * 128:min((i + 1) * 128, c.S)]
-            if seg.shape[1] == 0:
-                part[:, i, 0], part[:, i, 1] = -math.inf, 0.0
-                continue
-            mx = seg.amax(1)
-            part[:, i, 0], part[:, i, 1] = mx.float(), torch.exp(seg - mx[:, None]).sum(1).float()
-        t["part"] = part.reshape(-1)
-    return t
+    # the igemm stat_ptr contract: (max, sum exp(v - max)) per 128-column tile of the fp32 row, plus a trailing tile
+    # without columns, (-inf, 0)
+    nt = (c.S + 127) // 128 + 1
+    part = torch.zeros(c.M, nt, 2)
+    xd = x.double()
+    for i in range(nt):
+        seg = xd[:, i * 128:min((i + 1) * 128, c.S)]
+        if seg.shape[1] == 0:
+            part[:, i, 0], part[:, i, 1] = -math.inf, 0.0
+            continue
+        mx = seg.amax(1)
+        part[:, i, 0], part[:, i, 1] = mx.float(), torch.exp(seg - mx[:, None]).sum(1).float()
+    return {"s": s, "out": sentinel((c.M + 2) * c.p_pitch), "part": part.reshape(-1)}
 
 
 def softmax_call(lib, c, t):
     d = {k: v.cuda() for k, v in t.items()}
     sp = d["s"].data_ptr() + 4 * c.s_off
-    if c.partials:
-        rc = lib.b200_softmax_rows_partials(sp, c.M, c.S, c.s_pitch, d["part"].data_ptr(), d["part"].numel() // (2 * c.M),
-                                            d["out"].data_ptr(), c.p_pitch, ops._stream())
-    else:
-        rc = lib.b200_softmax_rows(sp, c.M, c.S, c.s_pitch, d["out"].data_ptr(), c.p_pitch, ops._stream())
+    rc = lib.b200_softmax_rows_partials(sp, c.M, c.S, c.s_pitch, d["part"].data_ptr(), d["part"].numel() // (2 * c.M),
+                                        d["out"].data_ptr(), c.p_pitch, ops._stream())
     torch.cuda.synchronize()
     assert rc == 0, _lib.last_error()
     return d["out"].cpu()
@@ -486,18 +474,14 @@ def softmax_call(lib, c, t):
 def test_softmax_rows_match_emulator(cuda_device, lib, case):
     c = case
     t = softmax_operands(c)
-    s = t["s"][c.s_off:]
-    if c.partials:
-        nt = t["part"].numel() // (2 * c.M)
-        want = E.softmax_rows_partials(s, c.M, c.S, c.s_pitch, t["part"], nt, c.p_pitch)
-    else:
-        want = E.softmax_rows(s, c.M, c.S, c.s_pitch, c.p_pitch)
+    nt = t["part"].numel() // (2 * c.M)
+    want = E.softmax_rows_partials(t["s"][c.s_off:], c.M, c.S, c.s_pitch, t["part"], nt, c.p_pitch)
     out = softmax_call(lib, c, t)
     ob = bits(out).view(-1, c.p_pitch)
     assert (ob[c.M:] == SENT16).all(), f"{c.name}: stores past row M"
     assert (ob[:c.M, c.S:] == 0).all(), f"{c.name}: pad columns are not +0"
     got = out.view(-1, c.p_pitch)[:c.M].double()
-    ratio_report("partials" if c.partials else "softmax_rows", c.name, check_values(c.name, want, got))
+    ratio_report("partials", c.name, check_values(c.name, want, got))
     assert torch.equal(bits(softmax_call(lib, c, t)), bits(out)), f"{c.name}: a second call stores different bits"
 
 

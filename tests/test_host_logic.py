@@ -103,7 +103,7 @@ def test_tap_reformulations_host_logic(monkeypatch, sd, Cin, Cout, sp, k, s, p, 
 
 def test_groupnorm_from_conv_partials_host_logic(monkeypatch):
     """GroupNorm statistics taken from the partial sums the producing convolutions leave behind (b200_igemm gn_partial
-    -> b200_groupnorm_from_partials) against the ordinary two-pass GroupNorm: single source, virtual concat of two
+    -> b200_groupnorm_from_partials_ex) against the ordinary two-pass GroupNorm: single source, virtual concat of two
     producers with different channel counts (groups of 24 = 3 producer groups), the 8-phase upsample convolution,
     and invalidation by an in-place update."""
     from tests import cpu_backend
@@ -257,17 +257,6 @@ def test_attention_tc_host_logic(monkeypatch):
         def b200_softmax_rows_partials(self, s, M, S, sp, part, n_tiles, p, pp, stream):
             from tests.cpu_backend import FakeLib as F2
             return F2().b200_softmax_rows_partials(s, M, S, sp, part, n_tiles, p, pp, stream)
-
-        def b200_softmax_rows(self, s, M, S, sp, p, pp, stream):
-            import ctypes as C
-            import numpy as np
-            sc = np.ctypeslib.as_array(C.cast(s, C.POINTER(C.c_float)), shape=(M * sp,)).reshape(M, sp)[:, :S]
-            e = np.exp(sc - sc.max(1, keepdims=True))
-            pr = e / e.sum(1, keepdims=True)
-            dst = np.ctypeslib.as_array(C.cast(p, C.POINTER(C.c_uint16)), shape=(M * pp,)).reshape(M, pp)
-            dst[:] = 0
-            dst[:, :S] = igemm_emulator._f32_to_bf16(pr.astype(np.float32)).reshape(M, S)
-            return 0
 
     monkeypatch.setattr(ops._lib, "require_device", lambda: FakeLib())
     monkeypatch.setattr(ops, "_stream", lambda: 0)

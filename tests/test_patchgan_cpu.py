@@ -13,6 +13,7 @@ import torch
 import torch.nn as nn
 
 from tests.golden import load
+from tests import cpu_backend
 from tests import patchgan_oracle as PO
 from oracle import ref_import
 from generativemodels_b200 import ops
@@ -219,7 +220,7 @@ def test_import_through_alias():
 # ---- the host code on the CPU stand-in ---------------------------------------------------------------------------
 @pytest.fixture
 def cpu_lib(monkeypatch):
-    return PO.install(monkeypatch)
+    return cpu_backend.install(monkeypatch)
 
 
 def _run(net, x):

@@ -5,6 +5,7 @@ import pytest
 import torch
 
 from tests.golden import load
+from tests import cpu_backend
 from tests import spadenet_oracle as SO
 from oracle import ref_import
 from generativemodels_b200 import ops
@@ -139,7 +140,7 @@ def test_input_shape_errors():
 # ---- the host code on the CPU stand-in ---------------------------------------------------------------------------
 @pytest.fixture
 def cpu_lib(monkeypatch):
-    return SO.install(monkeypatch)
+    return cpu_backend.install(monkeypatch)
 
 
 @pytest.mark.parametrize("name", ["tutorial", "bilinear", "bicubic"])

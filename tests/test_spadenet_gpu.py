@@ -156,8 +156,7 @@ LEAKY_CASES = [_leaky02(c) for c in CASES if {c.act1, c.act2} - {ACT_NONE, ACT_G
 
 
 @pytest.mark.parametrize("case", LEAKY_CASES, ids=[c.name for c in LEAKY_CASES])
-def test_igemm_leakyrelu02_matches_emulator(cuda_device, lib, case, monkeypatch):  # noqa: F811
-    SO.patch_emulator(monkeypatch)
+def test_igemm_leakyrelu02_matches_emulator(cuda_device, lib, case):  # noqa: F811
     run_case(lib, case)
 
 

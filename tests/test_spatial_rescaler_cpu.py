@@ -8,6 +8,7 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+from tests import cpu_backend
 from tests import rescaler_oracle as RO
 from tests.golden import load
 from oracle import ref_import
@@ -33,7 +34,7 @@ def ref():
 
 @pytest.fixture
 def cpu_lib(monkeypatch):
-    return RO.install(monkeypatch)
+    return cpu_backend.install(monkeypatch)
 
 
 def _rescaler(kw, seed=0):
