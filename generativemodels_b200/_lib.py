@@ -24,6 +24,8 @@ LIB_PATH = _HERE / "lib" / ("libb200gen.so" if ACT_DTYPE == "fp16" else "libb200
 
 B200_OK, B200_EINVAL, B200_ENOTSUP, B200_ECUDA, B200_ENODEV = 0, -1, -2, -3, -4
 DT_H16, DT_F32 = 0, 1
+DT_F64, DT_FP16, DT_BF16 = 2, 3, 4      # metric inputs only (b200_ssim, b200_avgpool2_f32, b200_mmd)
+SSIM_MAX_K, SSIM_MAX_SCALES = 128, 32
 H16_FP16, H16_BF16 = 0, 1
 ACT_NONE, ACT_RELU, ACT_SILU, ACT_LEAKYRELU, ACT_GELU, ACT_TANH, ACT_SIGMOID = 0, 1, 2, 3, 4, 5, 6
 ACT_GEGLU = 7        # b200_igemm act1 only: [32 a | 32 gate] column groups -> a * gelu(gate), half as many output channels
@@ -118,6 +120,23 @@ class RepackBlock(C.Structure):
                 ("tap", C.c_int16 * 8)]
 
 
+class SsimParams(C.Structure):
+    _fields_ = [("x", C.c_void_p), ("y", C.c_void_p), ("x_dtype", C.c_int32), ("y_dtype", C.c_int32),
+                ("x_strides", C.c_int64 * 5), ("y_strides", C.c_int64 * 5),
+                ("N", C.c_int32), ("C", C.c_int32), ("D", C.c_int32), ("H", C.c_int32), ("W", C.c_int32),
+                ("kd", C.c_int32), ("kh", C.c_int32), ("kw", C.c_int32),
+                ("taps_d", C.c_float * SSIM_MAX_K), ("taps_h", C.c_float * SSIM_MAX_K),
+                ("taps_w", C.c_float * SSIM_MAX_K), ("scale", C.c_float), ("c1", C.c_float), ("c2", C.c_float),
+                ("ssim_map", C.c_void_p), ("cs_map", C.c_void_p), ("partials", C.c_void_p)]
+
+
+class SsimCombineParams(C.Structure):
+    _fields_ = [("partials", C.c_void_p * SSIM_MAX_SCALES), ("slots", C.c_int32 * SSIM_MAX_SCALES),
+                ("count", C.c_int64 * SSIM_MAX_SCALES), ("weights", C.c_float * SSIM_MAX_SCALES),
+                ("N", C.c_int32), ("n_scales", C.c_int32),
+                ("ssim_mean", C.c_void_p), ("cs_mean", C.c_void_p), ("ms_ssim", C.c_void_p)]
+
+
 REPACK_BLOCKS, REPACK_TAP_IN, REPACK_TAP_OUT = 0, 1, 2
 
 _P, _I32, _I64, _F = C.c_void_p, C.c_int32, C.c_int64, C.c_float
@@ -181,8 +200,18 @@ SIGNATURES = {
     "b200_repack_weight": [_P, _I32, _I32, _I32, _I32, _I32, C.POINTER(RepackBlock), _I32, _P, _I32, _I32, _P],
     "b200_batchnorm_fold": [_P, _P, _P, _P, _P, _P, _F, _I32, _I64, _P, _P, _P],
 }
+# the sample-quality metrics' entry points; mirrors include/b200gen_metrics.h exactly
+METRIC_SIGNATURES = {
+    "b200_ssim_workspace_bytes": [C.POINTER(SsimParams)],
+    "b200_ssim": [C.POINTER(SsimParams), _P],
+    "b200_ssim_combine": [C.POINTER(SsimCombineParams), _P],
+    "b200_avgpool2_f32": [_P, _I32, _P, _I32, _I32, _I32, _I32, _I32, _I32, _P, _P],
+    "b200_mmd_workspace_bytes": [_P],
+    "b200_mmd": [_P, _I32, _P, _P, _I32, _P, _P, _P, _P, _P],
+}
 _RESTYPES = {"b200_last_error_string": C.c_char_p, "b200_groupnorm_workspace_bytes": C.c_int64,
-             "b200_attention_flash_workspace_bytes": C.c_int64, "b200_igemm_split_workspace_bytes": C.c_int64}
+             "b200_attention_flash_workspace_bytes": C.c_int64, "b200_igemm_split_workspace_bytes": C.c_int64,
+             "b200_ssim_workspace_bytes": C.c_int64, "b200_mmd_workspace_bytes": C.c_int64}
 
 _lib = None
 _device_ok = False
@@ -198,12 +227,12 @@ def load():
             f"{LIB_PATH} is missing: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
             "(generativemodels_b200/csrc/build.sh). There is no fallback path.")
     lib = C.CDLL(str(LIB_PATH))
-    for name, argtypes in SIGNATURES.items():
+    for name, argtypes in {**SIGNATURES, **METRIC_SIGNATURES}.items():
         fn = getattr(lib, name)  # AttributeError if the .so does not export it
         fn.argtypes = argtypes
         fn.restype = _RESTYPES.get(name, C.c_int)
     for which, struct in enumerate((IgemmParams, GnStatsParams, GnApplyParams, DdimCoef, DdpmCoef, PndmCoef, IgemmSeg,
-                                    FlashParams, KlCoef, RepackBlock)):
+                                    FlashParams, KlCoef, RepackBlock, SsimParams, SsimCombineParams)):
         c_size = lib.b200_abi_sizeof(which)
         if c_size != C.sizeof(struct):
             raise B200Error(f"ABI mismatch: {struct.__name__} is {C.sizeof(struct)} bytes in Python but {c_size} in "

@@ -1,5 +1,6 @@
 // Error reporting, version and device checks for libb200gen.so.
 #include "common.cuh"
+#include "../../include/b200gen_metrics.h"
 
 namespace b200 {
 
@@ -69,6 +70,8 @@ extern "C" int b200_abi_sizeof(int which) {
     case 7: return (int)sizeof(b200_flash_params);
     case 8: return (int)sizeof(b200_kl_coef);
     case 9: return (int)sizeof(b200_repack_block);
+    case 10: return (int)sizeof(b200_ssim_params);
+    case 11: return (int)sizeof(b200_ssim_combine_params);
     default: return -1;
   }
 }

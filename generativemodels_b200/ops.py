@@ -1337,3 +1337,106 @@ def small_linear(x: torch.Tensor, weight: torch.Tensor, bias: torch.Tensor | Non
     check(lib.b200_small_linear(x.data_ptr(), M, K, w.data_ptr(), _ptr(b), O, act_in, act_out, y.data_ptr(), _stream()),
           "b200_small_linear")
     return y
+
+
+# ------------------------------------------------------------------------------------------------
+# Sample-quality metrics (generativemodels_b200.metrics).  Inputs are planar [N, C, D, H, W] views of any strides in
+# fp32 / fp64 / fp16 / bf16, read in place; everything the kernels compute is fp32 with fp64 sums.
+# ------------------------------------------------------------------------------------------------
+_METRIC_DT = {torch.float32: _lib.DT_F32, torch.float64: _lib.DT_F64, torch.float16: _lib.DT_FP16,
+              torch.bfloat16: _lib.DT_BF16}
+
+
+def _metric_dt(t: torch.Tensor) -> int:
+    if t.dtype not in _METRIC_DT:
+        raise TypeError(f"metrics read fp32, fp64, fp16 or bf16 tensors, got {t.dtype}")
+    return _METRIC_DT[t.dtype]
+
+
+@dataclass
+class SsimScale:
+    """What one b200_ssim pass leaves for b200_ssim_combine: per-CTA fp64 sums [N, slots, 2] and the voxel count per
+    item (C * OD * OH * OW) that turns them into means."""
+    partials: torch.Tensor
+    slots: int
+    count: int
+
+
+def ssim_pass(x: torch.Tensor, y: torch.Tensor, taps: Sequence[Sequence[float]], scale: float, c1: float, c2: float,
+              maps: bool = False) -> tuple[SsimScale, torch.Tensor | None, torch.Tensor | None]:
+    """One fused SSIM / CS pass over 5-D [N, C, D, H, W] views x (= y_pred) and y with the separable kernel
+    ``taps = (taps_d, taps_h, taps_w)``; with ``maps`` also the fp32 SSIM and CS maps [N, C, OD, OH, OW]."""
+    lib = _lib.require_device()
+    p = _lib.SsimParams()
+    p.x, p.y = x.data_ptr(), y.data_ptr()
+    p.x_dtype, p.y_dtype = _metric_dt(x), _metric_dt(y)
+    p.x_strides[:], p.y_strides[:] = x.stride(), y.stride()
+    p.N, p.C, p.D, p.H, p.W = x.shape
+    p.kd, p.kh, p.kw = (len(t) for t in taps)
+    if max(p.kd, p.kh, p.kw) > _lib.SSIM_MAX_K:
+        raise NotImplementedError(f"SSIM kernels are at most {_lib.SSIM_MAX_K} taps per axis, got {p.kd, p.kh, p.kw}")
+    for dst, t in zip((p.taps_d, p.taps_h, p.taps_w), taps):
+        dst[:len(t)] = list(t)
+    p.scale, p.c1, p.c2 = scale, c1, c2
+    nbytes = lib.b200_ssim_workspace_bytes(C.byref(p))
+    if nbytes < 0:
+        raise NotImplementedError(f"no SSIM kernel for a {p.kd} x {p.kh} x {p.kw} kernel on a {p.D} x {p.H} x {p.W} "
+                                  "input (the tile does not fit in shared memory)")
+    part = torch.empty(nbytes // 8, dtype=torch.float64, device=x.device)
+    out_shape = (p.N, p.C, p.D - p.kd + 1, p.H - p.kh + 1, p.W - p.kw + 1)
+    ssim_map = cs_map = None
+    if maps:
+        ssim_map = torch.empty(out_shape, dtype=torch.float32, device=x.device)
+        cs_map = torch.empty(out_shape, dtype=torch.float32, device=x.device)
+    p.ssim_map, p.cs_map, p.partials = _ptr(ssim_map), _ptr(cs_map), part.data_ptr()
+    check(lib.b200_ssim(C.byref(p), _stream()), "b200_ssim")
+    count = out_shape[1] * out_shape[2] * out_shape[3] * out_shape[4]
+    return SsimScale(part, nbytes // (16 * p.N), count), ssim_map, cs_map
+
+
+def ssim_combine(scales: Sequence[SsimScale], N: int, weights: Sequence[float] | None = None):
+    """Per-item means of SSIM and CS per scale (fp32 [S, N] each) and, with ``weights`` (one per scale), MS-SSIM
+    prod_s relu(v_s) ** w_s (fp32 [N]; v_s = the CS mean, the SSIM mean at the last scale)."""
+    lib = _lib.require_device()
+    if not 1 <= len(scales) <= _lib.SSIM_MAX_SCALES:
+        raise NotImplementedError(f"MS-SSIM takes 1 to {_lib.SSIM_MAX_SCALES} scales, got {len(scales)}")
+    dev = scales[0].partials.device
+    p = _lib.SsimCombineParams()
+    for i, s in enumerate(scales):
+        p.partials[i], p.slots[i], p.count[i] = s.partials.data_ptr(), s.slots, s.count
+        p.weights[i] = float(weights[i]) if weights is not None else 0.0
+    p.N, p.n_scales = N, len(scales)
+    ssim = torch.empty((len(scales), N), dtype=torch.float32, device=dev)
+    cs = torch.empty((len(scales), N), dtype=torch.float32, device=dev)
+    ms = torch.empty(N, dtype=torch.float32, device=dev) if weights is not None else None
+    p.ssim_mean, p.cs_mean, p.ms_ssim = ssim.data_ptr(), cs.data_ptr(), _ptr(ms)
+    check(lib.b200_ssim_combine(C.byref(p), _stream()), "b200_ssim_combine")
+    return ssim, cs, ms
+
+
+def avgpool2_f32(x: torch.Tensor, dims: int) -> torch.Tensor:
+    """F.avg_pool{dims}d(x, kernel_size=2) in fp32 on a 5-D [N, C, D, H, W] view (2-D: D == 1, not pooled); a
+    contiguous fp32 result."""
+    lib = _lib.require_device()
+    N_, C_, D, H, W = x.shape
+    y = torch.empty((N_, C_, D // 2 if dims == 3 else D, H // 2, W // 2), dtype=torch.float32, device=x.device)
+    check(lib.b200_avgpool2_f32(x.data_ptr(), _metric_dt(x), (C.c_int64 * 5)(*x.stride()), N_, C_, D, H, W, dims,
+                                y.data_ptr(), _stream()), "b200_avgpool2_f32")
+    return y
+
+
+def mmd(y: torch.Tensor, y_pred: torch.Tensor) -> torch.Tensor:
+    """mean(Y Y^T) + mean(P P^T) - 2 mean(P Y^T) of MMDMetric's linear kernel over the flattened [B, V] rows, as the
+    column reduction sum_v (ybar_v - pbar_v)^2 / V; y and y_pred of equal shape, 1 to 5 dims.  fp32 0-dim result."""
+    lib = _lib.require_device()
+    if y.dim() > 5:
+        y, y_pred = y.reshape(y.shape[0], -1), y_pred.reshape(y_pred.shape[0], -1)
+    pad = 5 - y.dim()
+    shape = (C.c_int64 * 5)(*y.shape, *(1,) * pad)
+    ys = (C.c_int64 * 5)(*y.stride(), *(1,) * pad)
+    ps = (C.c_int64 * 5)(*y_pred.stride(), *(1,) * pad)
+    ws = torch.empty(lib.b200_mmd_workspace_bytes(shape) // 8, dtype=torch.float64, device=y.device)
+    out = torch.empty((), dtype=torch.float32, device=y.device)
+    check(lib.b200_mmd(y.data_ptr(), _metric_dt(y), ys, y_pred.data_ptr(), _metric_dt(y_pred), ps, shape,
+                       ws.data_ptr(), out.data_ptr(), _stream()), "b200_mmd")
+    return out
