@@ -24,7 +24,7 @@ LIB_PATH = _HERE / "lib" / ("libb200gen.so" if ACT_DTYPE == "fp16" else "libb200
 
 B200_OK, B200_EINVAL, B200_ENOTSUP, B200_ECUDA, B200_ENODEV = 0, -1, -2, -3, -4
 DT_H16, DT_F32 = 0, 1
-DT_F64, DT_FP16, DT_BF16 = 2, 3, 4      # metric inputs only (b200_ssim, b200_avgpool2_f32, b200_mmd)
+DT_F64, DT_FP16, DT_BF16 = 2, 3, 4      # inputs only (b200_interpolate's x, b200_ssim, b200_mmd)
 SSIM_MAX_K, SSIM_MAX_SCALES = 128, 32
 H16_FP16, H16_BF16 = 0, 1
 ACT_NONE, ACT_RELU, ACT_SILU, ACT_LEAKYRELU, ACT_GELU, ACT_TANH, ACT_SIGMOID = 0, 1, 2, 3, 4, 5, 6
@@ -154,15 +154,12 @@ SIGNATURES = {
     "b200_groupnorm_stats": [C.POINTER(GnStatsParams), _P],
     "b200_groupnorm_from_partials_ex": [C.POINTER(GnStatsParams), _P, _P, _P, _P],
     "b200_spade_apply": [C.POINTER(GnApplyParams), _P, _I32, _P, _P],
-    "b200_resize_nearest": [_P, _I32, _I32, _I32, _I32, _I32, _P, _I32, _I32, _I32, _P],
     "b200_groupnorm_apply": [C.POINTER(GnApplyParams), _P],
     "b200_groupnorm_fused": [C.POINTER(GnStatsParams), C.POINTER(GnApplyParams), _P],
     "b200_layernorm": [_P, _I64, _I32, _I32, _P, _P, _F, _P, _I32, _P],
     "b200_nchw_to_nhwc": [_P, _I32, _I32, _I64, _P, _I32, _P],
     "b200_nhwc_to_nchw": [_P, _I32, _I32, _I32, _I64, _I32, _P, _P],
-    "b200_upsample_nearest2x": [_P, _I32, _I32, _I32, _I32, _I32, _I32, _P, _P],
     "b200_upsample2x_interp": [_P, _I32, _I32, _I32, _I32, _I32, _P, _P],
-    "b200_avgpool2": [_P, _I32, _I32, _I32, _I32, _I32, _I32, _P, _P],
     "b200_pool_s2": [_P, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _P, _P],
     "b200_interpolate": [_P, _I32, _P, _P, _I32, _P, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _F, _F,
                          _F, _P],
@@ -205,7 +202,6 @@ METRIC_SIGNATURES = {
     "b200_ssim_workspace_bytes": [C.POINTER(SsimParams)],
     "b200_ssim": [C.POINTER(SsimParams), _P],
     "b200_ssim_combine": [C.POINTER(SsimCombineParams), _P],
-    "b200_avgpool2_f32": [_P, _I32, _P, _I32, _I32, _I32, _I32, _I32, _I32, _P, _P],
     "b200_mmd_workspace_bytes": [_P],
     "b200_mmd": [_P, _I32, _P, _P, _I32, _P, _P, _P, _P, _P],
 }

@@ -127,6 +127,16 @@ __device__ __forceinline__ uint4 pack8(const float* f) {
   return v;
 }
 
+// element i of an fp32 / fp64 / IEEE fp16 / bf16 array (B200_DT_F32 / _F64 / _FP16 / _BF16) as fp32
+__device__ __forceinline__ float load_any(const void* p, int dt, int64_t i) {
+  switch (dt) {
+    case B200_DT_F32: return static_cast<const float*>(p)[i];
+    case B200_DT_F64: return static_cast<float>(static_cast<const double*>(p)[i]);
+    case B200_DT_FP16: return __half2float(static_cast<const __half*>(p)[i]);
+    default: return __bfloat162float(static_cast<const __nv_bfloat16*>(p)[i]);
+  }
+}
+
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);

@@ -58,26 +58,6 @@ __global__ void nhwc_to_nchw_kernel(const T* __restrict__ x, int C, long long sp
 }
 
 // ------------------------------------------------------------------------------------------------
-// nearest x2 upsample / 2x average pool on channels-last bf16; one thread per (output voxel, 8 channels)
-// ------------------------------------------------------------------------------------------------
-__global__ void upsample2x_kernel(const uint4* __restrict__ x, int N, int D, int H, int W, int pv, int dims,
-                                  uint4* __restrict__ y) {
-  const int OD = dims == 3 ? 2 * D : D, OH = 2 * H, OW = 2 * W;
-  const long long total = (long long)N * OD * OH * OW * pv;
-  for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < total;
-       idx += (long long)gridDim.x * blockDim.x) {
-    long long t = idx;
-    const int v = (int)(t % pv); t /= pv;
-    const int ow = (int)(t % OW); t /= OW;
-    const int oh = (int)(t % OH); t /= OH;
-    const int od = (int)(t % OD); t /= OD;
-    const int n = (int)t;
-    const int id = dims == 3 ? od >> 1 : od;
-    y[idx] = __ldg(x + ((((long long)n * D + id) * H + (oh >> 1)) * W + (ow >> 1)) * pv + v);
-  }
-}
-
-// ------------------------------------------------------------------------------------------------
 // x2 bilinear / bicubic upsample of a 2-D channels-last tensor (align_corners=False); one thread per (output pixel,
 // 8 channels).  Output o = 2i + parity reads source coordinate s = i - 0.25 (even) or i + 0.25 (odd), so each axis has
 // two sets of taps and weights, picked by parity.
@@ -146,39 +126,6 @@ __global__ void upsample2x_interp_kernel(const uint4* __restrict__ x, int N, int
       for (int c = 0; c < 8; ++c) out[c] = fmaf(row[c], hw[a], out[c]);
     }
     y[idx] = pack8(out);
-  }
-}
-
-__global__ void avgpool2_kernel(const uint4* __restrict__ x, int N, int D, int H, int W, int pv, int dims,
-                                uint4* __restrict__ y) {
-  const int OD = dims == 3 ? D / 2 : D, OH = H / 2, OW = W / 2;
-  const int kd = dims == 3 ? 2 : 1;
-  const float inv = 1.0f / (float)(kd * 4);
-  const long long total = (long long)N * OD * OH * OW * pv;
-  for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < total;
-       idx += (long long)gridDim.x * blockDim.x) {
-    long long t = idx;
-    const int v = (int)(t % pv); t /= pv;
-    const int ow = (int)(t % OW); t /= OW;
-    const int oh = (int)(t % OH); t /= OH;
-    const int od = (int)(t % OD); t /= OD;
-    const int n = (int)t;
-    float acc[8];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) acc[j] = 0.f;
-    for (int a = 0; a < kd; ++a)
-      for (int b = 0; b < 2; ++b)
-        for (int c = 0; c < 2; ++c) {
-          const int id = dims == 3 ? od * 2 + a : od;
-          uint4 q = __ldg(x + ((((long long)n * D + id) * H + (oh * 2 + b)) * W + (ow * 2 + c)) * pv + v);
-          float f[8];
-          unpack8(q, f);
-#pragma unroll
-          for (int j = 0; j < 8; ++j) acc[j] += f[j];
-        }
-#pragma unroll
-    for (int j = 0; j < 8; ++j) acc[j] *= inv;
-    y[idx] = pack8(acc);
   }
 }
 
@@ -264,7 +211,9 @@ __device__ __forceinline__ void interp_load(const void* x, int dt, long long off
       f[4] = b.x; f[5] = b.y; f[6] = b.z; f[7] = b.w;
     }
   } else {
-    f[0] = dt == B200_DT_H16 ? h2f(reinterpret_cast<const h16*>(x)[off]) : __ldg(reinterpret_cast<const float*>(x) + off);
+    f[0] = dt == B200_DT_H16   ? h2f(reinterpret_cast<const h16*>(x)[off])
+           : dt == B200_DT_F32 ? __ldg(reinterpret_cast<const float*>(x) + off)
+                               : load_any(x, dt, off);
   }
 }
 
@@ -943,19 +892,6 @@ extern "C" int b200_nhwc_to_nchw(const void* x, int32_t x_dtype, int32_t N, int3
   return B200_OK;
 }
 
-extern "C" int b200_upsample_nearest2x(const void* x, int32_t N, int32_t D, int32_t H, int32_t W, int32_t pitch,
-                                       int32_t dims, void* y, void* stream_v) {
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
-  B200_CHECK_ARG(x && y && N >= 1 && D >= 1 && H >= 1 && W >= 1 && pitch >= 8 && pitch % 8 == 0 &&
-                 (dims == 2 || dims == 3) && (uintptr_t)x % 16 == 0 && (uintptr_t)y % 16 == 0,
-                 "upsample2x: bad arguments");
-  const long long total = (long long)N * (dims == 3 ? 2 * D : D) * 2 * H * 2 * W * (pitch / 8);
-  B200_CUDA(b200::launch_kernel(upsample2x_kernel, grid_for(total), 256, 0, stream, reinterpret_cast<const uint4*>(x), N, D, H, W, pitch / 8, dims,
-                                                        reinterpret_cast<uint4*>(y)));
-  B200_LAUNCH_CHECK("upsample2x_kernel");
-  return B200_OK;
-}
-
 extern "C" int b200_upsample2x_interp(const void* x, int32_t N, int32_t H, int32_t W, int32_t pitch, int32_t mode,
                                       void* y, void* stream_v) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
@@ -979,20 +915,6 @@ extern "C" int b200_vae_reparam_kld(const float* mu, const float* logvar, const 
   B200_CHECK_ARG(mu && logvar && eps && z && kld && n >= 1, "vae_reparam_kld: bad arguments");
   B200_CUDA(b200::launch_kernel(vae_reparam_kld_kernel, 1, 256, 0, stream, mu, logvar, eps, z, kld, (long long)n));
   B200_LAUNCH_CHECK("vae_reparam_kld_kernel");
-  return B200_OK;
-}
-
-extern "C" int b200_avgpool2(const void* x, int32_t N, int32_t D, int32_t H, int32_t W, int32_t pitch, int32_t dims,
-                             void* y, void* stream_v) {
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
-  B200_CHECK_ARG(x && y && N >= 1 && D >= 1 && H >= 1 && W >= 1 && pitch >= 8 && pitch % 8 == 0 &&
-                 (dims == 2 || dims == 3) && (uintptr_t)x % 16 == 0 && (uintptr_t)y % 16 == 0,
-                 "avgpool2: bad arguments");
-  const long long total = (long long)N * (dims == 3 ? D / 2 : D) * (H / 2) * (W / 2) * (pitch / 8);
-  if (total == 0) return B200_OK;
-  B200_CUDA(b200::launch_kernel(avgpool2_kernel, grid_for(total), 256, 0, stream, reinterpret_cast<const uint4*>(x), N, D, H, W, pitch / 8, dims,
-                                                      reinterpret_cast<uint4*>(y)));
-  B200_LAUNCH_CHECK("avgpool2_kernel");
   return B200_OK;
 }
 
@@ -1035,7 +957,7 @@ extern "C" int b200_interpolate(const void* x, int32_t x_dtype, const int64_t* x
                                 float ratio_h, float ratio_w, void* stream_v) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
   B200_CHECK_ARG(x && y && x_strides && y_strides, "interpolate: null pointer");
-  B200_CHECK_ARG((x_dtype == B200_DT_H16 || x_dtype == B200_DT_F32) && (y_dtype == B200_DT_H16 || y_dtype == B200_DT_F32),
+  B200_CHECK_ARG(x_dtype >= B200_DT_H16 && x_dtype <= B200_DT_BF16 && (y_dtype == B200_DT_H16 || y_dtype == B200_DT_F32),
                  "interpolate: unknown dtype %d / %d", x_dtype, y_dtype);
   const bool dims_ok = (mode == B200_INTERPOLATE_NEAREST || mode == B200_INTERPOLATE_AREA) ? (dims >= 1 && dims <= 3)
                        : mode == B200_INTERPOLATE_LINEAR                                 ? dims == 1
@@ -1073,11 +995,11 @@ extern "C" int b200_interpolate(const void* x, int32_t x_dtype, const int64_t* x
   a.rd = dims == 3 ? ratio_d : 1.f;
   a.rh = dims >= 2 ? ratio_h : 1.f;
   a.rw = ratio_w;
-  // 16-byte vectors across channels: channel stride 1 and every other stride a multiple of 8 elements on both sides,
-  // 16-byte aligned pointers, and a voxel stride that leaves room for round_up(C, 8) channels
+  // 16-byte vectors across channels: an h16 or fp32 input, channel stride 1 and every other stride a multiple of 8
+  // elements on both sides, 16-byte aligned pointers, and a voxel stride that leaves room for round_up(C, 8) channels
   const long long c8 = (C + 7) / 8 * 8;
-  bool vec = x_strides[1] == 1 && y_strides[1] == 1 && (uintptr_t)x % 16 == 0 && (uintptr_t)y % 16 == 0 &&
-             x_strides[4] >= c8 && y_strides[4] >= c8;
+  bool vec = x_dtype <= B200_DT_F32 && x_strides[1] == 1 && y_strides[1] == 1 && (uintptr_t)x % 16 == 0 &&
+             (uintptr_t)y % 16 == 0 && x_strides[4] >= c8 && y_strides[4] >= c8;
   for (int i : {0, 2, 3, 4}) vec = vec && x_strides[i] % 8 == 0 && y_strides[i] % 8 == 0;
   cudaError_t e;
   switch (mode) {

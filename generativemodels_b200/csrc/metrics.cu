@@ -1,6 +1,6 @@
 // Sample-quality metrics (generative/metrics/{ssim,ms_ssim,mmd}.py of the reference): SSIM / CS partial sums in one
-// separable pass per scale, the fp32 2x average pooling between MS-SSIM scales, the per-item finish of SSIM and
-// MS-SSIM, and MMD with the linear kernel as one column reduction.  Contracts: include/b200gen_metrics.h.
+// separable pass per scale, the per-item finish of SSIM and MS-SSIM, and MMD with the linear kernel as one column
+// reduction (the pooling between MS-SSIM scales is b200_interpolate's).  Contracts: include/b200gen_metrics.h.
 #include "common.cuh"
 #include "../../include/b200gen_metrics.h"
 
@@ -10,15 +10,6 @@ namespace {
 constexpr int kTW = 32;          // output tile width (one warp across W)
 constexpr int kThreads = 256;
 constexpr int kMaxSmem = 224 * 1024;  // dynamic; block_sum2 adds 128 static bytes
-
-__device__ __forceinline__ float load_any(const void* p, int dt, int64_t i) {
-  switch (dt) {
-    case B200_DT_F32: return static_cast<const float*>(p)[i];
-    case B200_DT_F64: return static_cast<float>(static_cast<const double*>(p)[i]);
-    case B200_DT_FP16: return __half2float(static_cast<const __half*>(p)[i]);
-    default: return __bfloat162float(static_cast<const __nv_bfloat16*>(p)[i]);
-  }
-}
 
 // Sum of (a, b) over the block in a fixed order: warp butterflies, then warp 0 over the per-warp sums.
 __device__ __forceinline__ double2 block_sum2(double a, double b) {
@@ -205,29 +196,6 @@ __global__ void __launch_bounds__(kThreads) ssim_combine_kernel(const b200_ssim_
   if (threadIdx.x == 0 && p.ms_ssim) p.ms_ssim[n] = ms;
 }
 
-__global__ void avgpool2_f32_kernel(const void* x, int dt, int64_t s0, int64_t s1, int64_t s2, int64_t s3, int64_t s4, int N, int C, int OD, int OH, int OW, int pd,
-                                    float* y) {
-  const int64_t total = (int64_t)N * C * OD * OH * OW;
-  const float div = pd == 2 ? 8.f : 4.f;
-  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
-    int64_t t = i;
-    const int ow = t % OW;
-    t /= OW;
-    const int oh = t % OH;
-    t /= OH;
-    const int od = t % OD;
-    t /= OD;
-    const int c = t % C;
-    const int n = t / C;
-    const int64_t base = n * s0 + c * s1 + (int64_t)od * pd * s2 + (int64_t)oh * 2 * s3 + (int64_t)ow * 2 * s4;
-    float sum = 0.f;
-    for (int dd = 0; dd < pd; ++dd)
-      for (int hh = 0; hh < 2; ++hh)
-        for (int ww = 0; ww < 2; ++ww) sum += load_any(x, dt, base + dd * s2 + hh * s3 + ww * s4);
-    y[i] = sum / div;
-  }
-}
-
 struct MmdArgs {
   const void* y;
   const void* p;
@@ -324,24 +292,6 @@ extern "C" int b200_ssim_combine(const b200_ssim_combine_params* p, void* stream
     B200_CHECK_ARG(p->partials[s] && p->slots[s] >= 1 && p->count[s] >= 1, "ssim_combine: scale %d has no partials", s);
   B200_CUDA(b200::launch_kernel(b200::ssim_combine_kernel, dim3(p->N), dim3(b200::kThreads), 0, stream, *p));
   B200_LAUNCH_CHECK("ssim_combine_kernel");
-  return B200_OK;
-}
-
-extern "C" int b200_avgpool2_f32(const void* x, int32_t x_dtype, const int64_t* x_strides, int32_t N, int32_t C,
-                                 int32_t D, int32_t H, int32_t W, int32_t dims, float* y, void* stream_v) {
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
-  B200_CHECK_ARG(x && y && x_strides, "avgpool2_f32: null pointer");
-  B200_CHECK_ARG(b200::metric_dtype_ok(x_dtype), "avgpool2_f32: unknown dtype %d", x_dtype);
-  B200_CHECK_ARG(dims == 2 || dims == 3, "avgpool2_f32: dims must be 2 or 3, got %d", dims);
-  B200_CHECK_ARG(dims == 3 || D == 1, "avgpool2_f32: a 2-D pooling needs D == 1");
-  const int OD = dims == 3 ? D / 2 : 1, OH = H / 2, OW = W / 2;
-  B200_CHECK_ARG(N >= 1 && C >= 1 && OD >= 1 && OH >= 1 && OW >= 1, "avgpool2_f32: output would be empty");
-  const int64_t total = (int64_t)N * C * OD * OH * OW;
-  const int blocks = (int)((total + 255) / 256 < 65536 ? (total + 255) / 256 : 65536);
-  B200_CUDA(b200::launch_kernel(b200::avgpool2_f32_kernel, dim3(blocks), dim3(256), 0, stream, x, x_dtype,
-                                x_strides[0], x_strides[1], x_strides[2], x_strides[3], x_strides[4], N, C, OD, OH, OW,
-                                dims == 3 ? 2 : 1, y));
-  B200_LAUNCH_CHECK("avgpool2_f32_kernel");
   return B200_OK;
 }
 

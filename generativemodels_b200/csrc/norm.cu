@@ -552,24 +552,6 @@ __global__ void spade_apply_kernel(const h16* __restrict__ x0, const h16* __rest
   }
 }
 
-__global__ void resize_nearest_kernel(const h16* __restrict__ x, int N, int D, int H, int W, int pitch,
-                                      h16* __restrict__ y, int OD, int OH, int OW) {
-  const long long total = (long long)N * OD * OH * OW * pitch;
-  const float sd = (float)D / OD, sh = (float)H / OH, sw = (float)W / OW;
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total;
-       i += (long long)gridDim.x * blockDim.x) {
-    const int c = (int)(i % pitch);
-    long long t = i / pitch;
-    const int ow = (int)(t % OW); t /= OW;
-    const int oh = (int)(t % OH); t /= OH;
-    const int od = (int)(t % OD);
-    const int n = (int)(t / OD);
-    const int iw = min((int)floorf(ow * sw), W - 1), ih = min((int)floorf(oh * sh), H - 1),
-              id = min((int)floorf(od * sd), D - 1);
-    y[i] = x[((((long long)n * D + id) * H + ih) * W + iw) * pitch + c];
-  }
-}
-
 // ---- LayerNorm: one warp per row ----------------------------------------------------------------
 __global__ void layernorm_kernel(const h16* __restrict__ x, long long M, int C, int x_pitch,
                                  const float* __restrict__ gamma, const float* __restrict__ beta, float eps,
@@ -859,20 +841,6 @@ extern "C" int b200_spade_apply(const b200_gn_apply_params* p, const void* gb, i
     B200_CUDA(b200::launch_kernel(zero_pad_channels_kernel, (unsigned)zb, 256, 0, stream, y, rows, C, p->y_pitch));
     B200_LAUNCH_CHECK("zero_pad_channels_kernel");
   }
-  return B200_OK;
-}
-
-extern "C" int b200_resize_nearest(const void* x, int32_t N, int32_t D, int32_t H, int32_t W, int32_t pitch, void* y,
-                                   int32_t OD, int32_t OH, int32_t OW, void* stream_v) {
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
-  B200_CHECK_ARG(x && y && N >= 1 && D >= 1 && H >= 1 && W >= 1 && OD >= 1 && OH >= 1 && OW >= 1 && pitch >= 1,
-                 "resize_nearest: bad arguments");
-  const long long total = (long long)N * OD * OH * OW * pitch;
-  long long blocks = (total + 255) / 256;
-  if (blocks > 16ll * sm_count()) blocks = 16ll * sm_count();
-  B200_CUDA(b200::launch_kernel(resize_nearest_kernel, (unsigned)blocks, 256, 0, stream, reinterpret_cast<const h16*>(x), N, D, H, W, pitch,
-                                                             reinterpret_cast<h16*>(y), OD, OH, OW));
-  B200_LAUNCH_CHECK("resize_nearest_kernel");
   return B200_OK;
 }
 

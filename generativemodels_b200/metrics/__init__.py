@@ -1,6 +1,6 @@
 """Sample-quality metrics of the reference's ``generative.metrics`` on the CUDA path: SSIM, MS-SSIM and MMD.
 
-Every per-voxel operation runs in libb200gen.so (b200_ssim, b200_avgpool2_f32, b200_ssim_combine, b200_mmd); the
+Every per-voxel operation runs in libb200gen.so (b200_ssim, b200_interpolate, b200_ssim_combine, b200_mmd); the
 classes here restate MONAI's metric bookkeeping (a buffer of per-item values, ``aggregate`` / ``reset``) on the host.
 FID is not provided: its cost is a dense matrix square root, which the reference itself computes with scipy."""
 from .metric import Cumulative, CumulativeIterationMetric, IterationMetric, Metric, MetricReduction, RegressionMetric

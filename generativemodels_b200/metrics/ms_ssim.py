@@ -1,6 +1,7 @@
 """MultiScaleSSIMMetric (reference: generative/metrics/ms_ssim.py): per scale one b200_ssim pass, an fp32 2x average
-pooling (b200_avgpool2_f32, floor) between scales, and one b200_ssim_combine for prod_s relu(cs_s) ** w_s with the
-last scale's SSIM in place of its CS: 3 * len(weights) - 1 launches per call, no host synchronisation."""
+pooling (b200_interpolate's AREA over the even part of each extent, floor) between scales, and one b200_ssim_combine
+for prod_s relu(cs_s) ** w_s with the last scale's SSIM in place of its CS: 3 * len(weights) - 1 launches per call, no
+host synchronisation."""
 from __future__ import annotations
 
 from collections.abc import Sequence

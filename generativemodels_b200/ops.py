@@ -760,16 +760,12 @@ def spade_modulate(srcs: CL | Sequence[CL], affine: torch.Tensor, gb: CL, gb_aff
 
 def resize_nearest(x: CL, dims: Sequence[int]) -> CL:
     """F.interpolate(x, size=dims, mode="nearest") on a channels-last tensor."""
-    lib = _lib.require_device()
     d = tuple(int(v) for v in dims)
     if len(d) == 2:
         d = (1, *d)
     if d == (x.D, x.H, x.W):
         return x
-    out = x.like(dims=d)
-    check(lib.b200_resize_nearest(x.t.data_ptr(), x.N, x.D, x.H, x.W, x.pitch, out.t.data_ptr(), *d, _stream()),
-          "b200_resize_nearest")
-    return out
+    return _resample(x, d, _lib.INTERPOLATE_NEAREST)
 
 
 def layernorm(x: CL, gamma: torch.Tensor, beta: torch.Tensor, eps: float) -> CL:
@@ -785,13 +781,9 @@ def layernorm(x: CL, gamma: torch.Tensor, beta: torch.Tensor, eps: float) -> CL:
 # resampling / elementwise
 # --------------------------------------------------------------------------------------------------
 def upsample_nearest2x(x: CL) -> CL:
-    lib = _lib.require_device()
+    """F.interpolate(x, scale_factor=2, mode="nearest"); a 2-D tensor keeps its D slices."""
     sd = x.spatial_dims
-    dims = (x.D * 2 if sd == 3 else x.D, x.H * 2, x.W * 2)
-    out = x.like(dims=dims)
-    check(lib.b200_upsample_nearest2x(x.t.data_ptr(), x.N, x.D, x.H, x.W, x.pitch, sd, out.t.data_ptr(), _stream()),
-          "b200_upsample_nearest2x")
-    return out
+    return _resample(x, (x.D * 2 if sd == 3 else x.D, x.H * 2, x.W * 2), _lib.INTERPOLATE_NEAREST)
 
 
 _INTERP_MODES = {"bilinear": _lib.INTERP_BILINEAR, "bicubic": _lib.INTERP_BICUBIC}
@@ -825,13 +817,33 @@ def vae_reparam_kld(mu: torch.Tensor, logvar: torch.Tensor, eps: torch.Tensor) -
 
 
 def avgpool2(x: CL) -> CL:
-    lib = _lib.require_device()
+    """nn.AvgPool{2,3}d(2, 2): floor extents; a 2-D tensor keeps its D slices."""
     sd = x.spatial_dims
     dims = (x.D // 2 if sd == 3 else x.D, x.H // 2, x.W // 2)
-    out = x.like(dims=dims)
-    check(lib.b200_avgpool2(x.t.data_ptr(), x.N, x.D, x.H, x.W, x.pitch, sd, out.t.data_ptr(), _stream()),
-          "b200_avgpool2")
-    return out
+    return _resample(x, dims, _lib.INTERPOLATE_AREA, src=(dims[0] * 2 if sd == 3 else x.D, dims[1] * 2, dims[2] * 2))
+
+
+def _resample(x: CL, dims: Sequence[int], mode: int, src: Sequence[int] | None = None,
+              y: torch.Tensor | None = None) -> CL:
+    """One b200_interpolate launch (``mode`` B200_INTERPOLATE_NEAREST or _AREA) from x's first ``src`` voxels per axis
+    (all of them by default) to extents ``dims``, into ``y`` ([N, *dims, pitch] of x's storage type; a new tensor by
+    default).  All three axes are resampled, so a 2-D tensor's D slices are kept as they are, and all ``pitch``
+    channels, so the output's pad channels come from the input's (zeros stay zeros).  The ratios are fp32(in / out)
+    per axis, interpolate_plan's rule for a size.  AREA over even extents halved is AvgPool(2, 2)."""
+    lib = _lib.require_device()
+    t = x.t
+    N_, D, H, W, P = t.shape
+    OD, OH, OW = dims
+    if src is not None:
+        D, H, W = src
+    if y is None:
+        y = torch.empty((N_, OD, OH, OW, P), dtype=t.dtype, device=t.device)
+    xs, ys = t.stride(), y.stride()
+    # the ratios are rounded to fp32 by the c_float arguments
+    check(lib.b200_interpolate(t.data_ptr(), DT_H16, (C.c_int64 * 5)(xs[0], 1, xs[1], xs[2], xs[3]), y.data_ptr(),
+                               DT_H16, (C.c_int64 * 5)(ys[0], 1, ys[1], ys[2], ys[3]), N_, P, D, H, W, OD, OH, OW, 3,
+                               mode, D / OD, H / OH, W / OW, _stream()), "b200_interpolate")
+    return CL(y, x.C, x.spatial_dims)
 
 
 _POOL_MODES = {"avg": _lib.POOL_AVG, "max": _lib.POOL_MAX}
@@ -1416,12 +1428,16 @@ def ssim_combine(scales: Sequence[SsimScale], N: int, weights: Sequence[float] |
 
 def avgpool2_f32(x: torch.Tensor, dims: int) -> torch.Tensor:
     """F.avg_pool{dims}d(x, kernel_size=2) in fp32 on a 5-D [N, C, D, H, W] view (2-D: D == 1, not pooled); a
-    contiguous fp32 result."""
+    contiguous fp32 result.  b200_interpolate's AREA over the even part of each pooled extent."""
     lib = _lib.require_device()
     N_, C_, D, H, W = x.shape
     y = torch.empty((N_, C_, D // 2 if dims == 3 else D, H // 2, W // 2), dtype=torch.float32, device=x.device)
-    check(lib.b200_avgpool2_f32(x.data_ptr(), _metric_dt(x), (C.c_int64 * 5)(*x.stride()), N_, C_, D, H, W, dims,
-                                y.data_ptr(), _stream()), "b200_avgpool2_f32")
+    src = [2 * v for v in y.shape[2:]]
+    if dims == 2:
+        src[0] = D
+    check(lib.b200_interpolate(x.data_ptr(), _metric_dt(x), (C.c_int64 * 5)(*x.stride()), y.data_ptr(), DT_F32,
+                               (C.c_int64 * 5)(*y.stride()), N_, C_, *src, *y.shape[2:], dims,
+                               _lib.INTERPOLATE_AREA, 1.0, 1.0, 1.0, _stream()), "b200_interpolate")
     return y
 
 

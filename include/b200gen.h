@@ -32,6 +32,11 @@ extern "C" {
  * flavour built with -DB200_H16_IS_BF16.  b200_act_dtype() reports which one a loaded library computes in. */
 #define B200_DT_H16  0
 #define B200_DT_F32  1
+/* input-only formats: b200_interpolate's x (on its one-element-per-thread path) and the metric inputs of
+ * b200gen_metrics.h, converted to fp32 on load */
+#define B200_DT_F64  2
+#define B200_DT_FP16 3   /* IEEE half, whichever 16-bit format the library stores activations in */
+#define B200_DT_BF16 4
 #define B200_H16_FP16 0
 #define B200_H16_BF16 1
 
@@ -246,11 +251,6 @@ int b200_groupnorm_fused(const b200_gn_stats_params* s, const b200_gn_apply_para
  * input pad channels are not read; output pad channels [C, y_pitch) are written +0. */
 int b200_spade_apply(const b200_gn_apply_params* p, const void* gb, int32_t gb_pitch, const float* gb_affine,
                      void* stream);
-/* F.interpolate(mode="nearest", size=...) on NDHWC h16: src index = min(floor(dst * fp32(in / out)), in - 1) per axis,
- * the product rounded to fp32 as PyTorch does for fp16 / bf16 / fp32 tensors (it differs from the exact-rational
- * floor(dst * in / out) for some sizes, e.g. 26 -> 22, 6 -> 74, 14 -> 46).  Copies all `pitch` channels of a voxel. */
-int b200_resize_nearest(const void* x, int32_t N, int32_t D, int32_t H, int32_t W, int32_t pitch, void* y, int32_t OD,
-                        int32_t OH, int32_t OW, void* stream);
 
 /* nn.LayerNorm over the last dim of a h16 [M, C] matrix (diffusion_model_unet.py:221-223): two fp32 passes (mean, then
  * the mean square of x - mean), one warp per row; with u = 2^-24 (C / 32 + 8) and s = sqrt(var + eps),
@@ -268,11 +268,6 @@ int b200_nchw_to_nhwc(const float* x, int32_t N, int32_t C, int64_t spatial, voi
                       void* stream);
 int b200_nhwc_to_nchw(const void* x, int32_t x_dtype, int32_t N, int32_t C, int64_t spatial,
                       int32_t pitch, float* y, void* stream);
-/* F.interpolate(scale_factor=2, mode="nearest") (diffusion_model_unet.py:578; autoencoderkl.py:84): a copy of every
- * `pitch` channel of x [N][D][H][W][pitch] into y [N][OD][2H][2W][pitch] (OD = 2D for dims == 3, D slices for dims == 2).
- * N, D, H, W >= 1, pitch a positive multiple of 8, x and y 16-byte aligned (B200_EINVAL otherwise). */
-int b200_upsample_nearest2x(const void* x, int32_t N, int32_t D, int32_t H, int32_t W, int32_t pitch,
-                            int32_t dims /*2 or 3*/, void* y, void* stream);
 /* nn.Upsample(scale_factor=2, mode="bilinear" | "bicubic") on a 2-D NHWC h16 tensor [N][H][W][pitch] -> [N][2H][2W][pitch]
  * (SPADEDecoder's upsampling_mode, nets/spade_network.py:280,317), PyTorch's align_corners=False semantics: source
  * coordinate s = (dst + 0.5) / 2 - 0.5 per axis;
@@ -285,12 +280,6 @@ int b200_upsample_nearest2x(const void* x, int32_t N, int32_t D, int32_t H, int3
 #define B200_INTERP_BICUBIC  1
 int b200_upsample2x_interp(const void* x, int32_t N, int32_t H, int32_t W, int32_t pitch, int32_t mode, void* y,
                            void* stream);
-/* nn.AvgPool{2,3}d(kernel=2, stride=2) (diffusion_model_unet.py:522) on [N][D][H][W][pitch] -> floor(extent / 2) per
- * pooled axis (dims == 2 pools H and W of every D slice): the 4 (8) taps added in fp32 in d, h, w order, then scaled by
- * 1/4 (1/8), one rounding on the store.  Every `pitch` channel is processed, so input pad channels must be finite (zeros
- * stay zeros).  N, D, H, W >= 1, pitch a positive multiple of 8, x and y 16-byte aligned (B200_EINVAL otherwise). */
-int b200_avgpool2(const void* x, int32_t N, int32_t D, int32_t H, int32_t W, int32_t pitch,
-                  int32_t dims, void* y, void* stream);
 /* nn.AvgPool{2,3}d / nn.MaxPool{2,3}d(kernel_size=kernel, stride=2, padding=padding) on NDHWC h16 [N][D][H][W][pitch]
  * (MultiScalePatchDiscriminator's input pyramid, nets/patchgan_discriminator.py:89-92): dims == 2 pools H and W of
  * every D slice, dims == 3 all three.  Output extent per pooled axis floor((in + 2 * padding - kernel) / 2) + 1
@@ -304,10 +293,14 @@ int b200_avgpool2(const void* x, int32_t N, int32_t D, int32_t H, int32_t W, int
 int b200_pool_s2(const void* x, int32_t N, int32_t D, int32_t H, int32_t W, int32_t pitch, int32_t dims,
                  int32_t kernel, int32_t padding, int32_t mode, void* y, void* stream);
 /* F.interpolate(x, size=... | scale_factor=..., mode=..., align_corners=False, antialias=False) at any size or scale
- * (SpatialRescaler, blocks/encoder_modules.py:60,78).  x is [N][C][D][H][W] and y [N][C][OD][OH][OW] with arbitrary
- * element strides {n, c, d, h, w} (host arrays x_strides / y_strides) and their own dtypes (B200_DT_H16 / B200_DT_F32),
- * so one entry point reads and writes planar NC[D]HW fp32, channels-last fp32 and channels-last h16.  `dims` is the
- * number of resampled axes, the last ones: dims == 2 needs D == OD == 1, dims == 1 also H == OH == 1.
+ * (SpatialRescaler, blocks/encoder_modules.py:60,78), and the library's other resampling on a grid: nearest x2
+ * (diffusion_model_unet.py:578; autoencoderkl.py:84), nearest to a size (SPADE's segmentation map,
+ * blocks/spade_norm.py:89), nn.AvgPool{2,3}d(2, 2) (diffusion_model_unet.py:522) and MS-SSIM's pooling between scales
+ * (ms_ssim.py:130-131), the last two as AREA over the even part of each extent.  x is [N][C][D][H][W] and
+ * y [N][C][OD][OH][OW] with arbitrary element strides {n, c, d, h, w} (host arrays x_strides / y_strides) and their own
+ * dtypes (B200_DT_H16 / B200_DT_F32; x also B200_DT_F64 / _FP16 / _BF16, which only the one-element-per-thread path
+ * below reads), so one entry point reads and writes planar NC[D]HW fp32, channels-last fp32 and channels-last h16.
+ * `dims` is the number of resampled axes, the last ones: dims == 2 needs D == OD == 1, dims == 1 also H == OH == 1.
  * Modes and the dims they take (anything else is B200_EINVAL):
  *   B200_INTERPOLATE_NEAREST 1, 2, 3 | _LINEAR 1 | _BILINEAR 2 | _BICUBIC 2 | _TRILINEAR 3 | _AREA 1, 2, 3.
  * Coordinates follow ATen (ATen/native/UpSample.h and AdaptivePooling.h) per resampled axis, with the fp32 ratio r the
@@ -325,10 +318,12 @@ int b200_pool_s2(const void* x, int32_t N, int32_t D, int32_t H, int32_t W, int3
  *              a fused multiply-add;
  *   AREA     : adaptive average pooling, window [floor(o * in / out), ceil((o + 1) * in / out)) per axis in integer
  *              arithmetic (the ratios are ignored).
- * Numerics: fp32 arithmetic, one rounding on the store (fp16 stores saturate).  NEAREST is a copy (bit-exact when the
- * dtypes match).  The separable modes interpolate along W within each source row first, then along H, then along D;
+ * Numerics: fp32 arithmetic, one rounding on the store (fp16 stores saturate).  NEAREST is a copy (bit-exact on finite
+ * values when the dtypes match).  The separable modes interpolate along W within each source row first, then along H, then along D;
  * each 1-D step is sum_k x_k * w_k over its taps in order, products and sums rounded separately.  AREA sums the window
- * in d, h, w order (w innermost) and divides by the window's D, H and W extents in turn.
+ * in d, h, w order (w innermost) and divides by the window's D, H and W extents in turn, as ATen does; on 2 x 2 (x 2)
+ * windows that equals one scaling by 1/4 (1/8) except through double rounding when the mean is fp32-subnormal (a window
+ * sum below 2^-124 in magnitude), which no fp16 input can give (every fp16 value is a multiple of 2^-24).
  * Threads: with channel stride 1 on both sides, every other stride a multiple of 8 elements, x and y 16-byte aligned
  * and w strides >= round_up(C, 8), one thread moves 8 channels as 16-byte vectors; these also write channels
  * [C, round_up(C, 8)) of every output voxel (a channels-last buffer's pad channels, interpolated from the input's

@@ -14,13 +14,11 @@ extern "C" {
 /* ------------------------------------------------------------------------------------------------
  * Sample-quality metrics (generative/metrics/ssim.py, ms_ssim.py, mmd.py).  Inputs are planar tensors read in place
  * through element strides, in any of four formats; every value is converted to fp32 on load (the reference computes
- * in fp32 after convert_data_type(dtype=float)).  The B200_DT_* codes below are metric inputs only.
+ * in fp32 after convert_data_type(dtype=float)): B200_DT_F32, _F64, _FP16 and _BF16 of b200gen.h.
  * The conventions of b200gen.h hold (return codes, no allocation, no synchronisation, work enqueued on `stream`).
  * The ABI size query of b200gen.h answers 10 with sizeof(b200_ssim_params), 11 with sizeof(b200_ssim_combine_params).
+ * The 2x average pooling between MS-SSIM scales is b200_interpolate's AREA mode over the even part of each extent.
  * ------------------------------------------------------------------------------------------------ */
-#define B200_DT_F64  2
-#define B200_DT_FP16 3   /* IEEE half, whichever 16-bit format the library stores activations in */
-#define B200_DT_BF16 4
 #define B200_SSIM_MAX_K 128
 #define B200_SSIM_MAX_SCALES 32
 
@@ -71,11 +69,6 @@ typedef struct {
   float* ms_ssim;
 } b200_ssim_combine_params;
 int b200_ssim_combine(const b200_ssim_combine_params* p, void* stream);
-/* F.avg_pool{2,3}d(x, kernel_size=2) between MS-SSIM scales (ms_ssim.py:130-131) in fp32: x [N][C][D][H][W] with element
- * strides, any metric dtype; y contiguous fp32 [N][C][OD][H / 2][W / 2] (floor), OD = D / 2 for dims == 3, D (== 1)
- * for dims == 2.  Each output is the fp32 sum of its window in d, h, w order (w innermost), divided by 4 or 8. */
-int b200_avgpool2_f32(const void* x, int32_t x_dtype, const int64_t* x_strides, int32_t N, int32_t C, int32_t D,
-                      int32_t H, int32_t W, int32_t dims, float* y, void* stream);
 /* MMDMetric (mmd.py:36-70) with its linear kernel, beta = 1, gamma = 2: mean(Y Y^T) + mean(P P^T) - 2 mean(P Y^T) over
  * V = prod(shape[1..4]) equals sum_v (ybar_v - pbar_v)^2 / V, ybar and pbar the means over the batch, so one pass
  * reads each element once and no GEMM is formed.  y and y_pred are [shape[0]][shape[1]]..[shape[4]] with their own

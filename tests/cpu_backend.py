@@ -87,9 +87,18 @@ def _table_affine(tab):
     return N.Affine(a, b, z, z, z, z, z, z, z[:1])
 
 
+_CTYPES = {_lib.DT_F32: (C.c_float, np.float32, None), _lib.DT_F64: (C.c_double, np.float64, None),
+           _lib.DT_FP16: (C.c_uint16, np.int16, torch.float16), _lib.DT_BF16: (C.c_uint16, np.int16, torch.bfloat16)}
+
+
 def _strided(ptr, dt, strides, shape):
+    """A strided host view of a B200_DT_* buffer: h16 (the flavour's 16-bit type), fp32, fp64, fp16 or bf16."""
     count = 1 + sum((s - 1) * st for s, st in zip(shape, strides))
-    return torch.as_strided((bf16 if dt == _lib.DT_H16 else f32)(ptr, count), shape, strides)
+    if dt == _lib.DT_H16:
+        return torch.as_strided(bf16(ptr, count), tuple(shape), tuple(strides))
+    ctype, npt, as_dtype = _CTYPES[dt]
+    flat = torch.from_numpy(_np(ptr, count, ctype).view(npt))
+    return torch.as_strided(flat.view(as_dtype) if as_dtype else flat, tuple(shape), tuple(strides))
 
 
 def _pos(pos_dev):
@@ -152,10 +161,6 @@ class FakeLib:
         store16(p.y_ptr, r.out)
         return 0
 
-    def b200_resize_nearest(self, x, N_, D, H, W_, pitch, y, OD, OH, OW, stream):
-        store16(y, N.resize_nearest(bf16(x, N_ * D * H * W_ * pitch), N_, D, H, W_, pitch, OD, OH, OW))
-        return 0
-
     def b200_groupnorm_apply(self, p, stream):
         p = _obj(p)
         src = _sources(p)
@@ -169,19 +174,11 @@ class FakeLib:
         store16(y, N.layernorm(bf16(x, M * xp), M, C_, xp, f32(g, C_), f32(b, C_), eps, yp).out)
         return 0
 
-    def b200_upsample_nearest2x(self, x, N_, D, H, W_, pitch, dims, y, stream):
-        store16(y, W.upsample_nearest2x(bf16(x, N_ * D * H * W_ * pitch), N_, D, H, W_, pitch, dims).out)
-        return 0
-
     def b200_upsample2x_interp(self, x, N_, H, W_, pitch, mode, y, stream):
         src = bf16(x, N_ * H * W_ * pitch).view(N_, H, W_, pitch).float().permute(0, 3, 1, 2)
         m = "bilinear" if mode == _lib.INTERP_BILINEAR else "bicubic"
         out = F.interpolate(src, scale_factor=2, mode=m).permute(0, 2, 3, 1)
         store16(y, out)
-        return 0
-
-    def b200_avgpool2(self, x, N_, D, H, W_, pitch, dims, y, stream):
-        store16(y, W.avgpool2(bf16(x, N_ * D * H * W_ * pitch), N_, D, H, W_, pitch, dims).out)
         return 0
 
     def b200_pool_s2(self, x, N_, D, H, W_, pitch, dims, k, pad, mode, y, stream):
@@ -196,7 +193,7 @@ class FakeLib:
 
     def b200_interpolate(self, x, xdt, xs, y, ydt, ys, N_, C_, D, H, W_, OD, OH, OW, dims, mode, rd, rh, rw, stream):
         xs, ys = [int(v) for v in xs[:5]], [int(v) for v in ys[:5]]
-        src = _strided(x, xdt, xs, (N_, C_, D, H, W_)).float().reshape(N_, C_, *(D, H, W_)[3 - dims:])
+        src = _strided(x, xdt, xs, (N_, C_, D, H, W_)).reshape(N_, C_, *(D, H, W_)[3 - dims:])
         out = header_interpolate(src, (OD, OH, OW)[3 - dims:], (rd, rh, rw)[3 - dims:], mode)
         dst = _strided(y, ydt, ys, (N_, C_, OD, OH, OW))
         dst.copy_(out.reshape(N_, C_, OD, OH, OW).to(dst.dtype))

@@ -6,9 +6,9 @@ the float64 value before the final rounding (`exact`), the value as the entry po
 as float64) and the accuracy term of the bound (`err`), one per element of the written region.  `kind` says how the
 bound reads:
 
-  copy   the kernel moves data, or runs an fp32 sequence the emulator reproduces exactly (avgpool2's in-order adds and
-         power-of-two scale, embed_tokens' one fp32 add): the bound is zero and the GPU test compares bits.  16-bit
-         stores are fp32 -> 16-bit RN; fp16 saturates at +-65504 (cvt.rn.satfinite), which is part of the rounding.
+  copy   the kernel moves data, or runs an fp32 sequence the emulator reproduces exactly (embed_tokens' one fp32
+         add): the bound is zero and the GPU test compares bits.  16-bit stores are fp32 -> 16-bit RN; fp16
+         saturates at +-65504 (cvt.rn.satfinite), which is part of the rounding.
   h16    |got - out| <= ulp16(max(|got|, |out|)) + err;
   f32    |got - out| <= ulp32(max(|got|, |out|)) + err.
 
@@ -109,30 +109,6 @@ def nhwc_to_nchw(x, n, C, spatial, pitch):
     """rows [N * spatial][pitch] (h16 or fp32) -> [N][C][spatial] fp32: columns [C, pitch) not read."""
     X = rows_of(x, n * spatial, pitch, C).view(n, spatial, C)
     return copy(X.permute(0, 2, 1).reshape(-1))
-
-
-def upsample_nearest2x(x, n, D, H, W, pitch, dims):
-    """[N][D][H][W][pitch] -> [N][OD][2H][2W][pitch], OD = 2D (dims 3) or D: every channel copied."""
-    X = x[:n * D * H * W * pitch].view(n, D, H, W, pitch).to(F64)
-    X = X.repeat_interleave(2, 2).repeat_interleave(2, 3)
-    if dims == 3:
-        X = X.repeat_interleave(2, 1)
-    return copy(X.reshape(-1))
-
-
-def avgpool2(x, n, D, H, W, pitch, dims):
-    """fp32 adds in d, h, w order from 0, times 1/4 (1/8): exact in fp32 emulation; floor extents."""
-    X = x[:n * D * H * W * pitch].view(n, D, H, W, pitch).float()
-    kd = 2 if dims == 3 else 1
-    OD, OH, OW = D // kd, H // 2, W // 2
-    acc = torch.zeros(n, OD, OH, OW, pitch, dtype=torch.float32)
-    for a in range(kd):
-        for b in range(2):
-            for c in range(2):
-                dsl = slice(a, a + kd * OD, kd) if dims == 3 else slice(0, D)
-                acc = acc + X[:, dsl, b:b + 2 * OH:2, c:c + 2 * OW:2]
-    acc = acc * (1.0 / (4 * kd))
-    return copy(h16(acc.to(F64)).reshape(-1))
 
 
 def axpy_h16(a, b, alpha, n):

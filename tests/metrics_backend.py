@@ -1,27 +1,17 @@
 """TEST-ONLY CPU stand-in for the metric entry points of libb200gen.so (include/b200gen_metrics.h), on HOST pointers:
 tests/cpu_backend.FakeLib extended by one method per metric symbol, each viewing its pointers as host tensors and
-storing what the float64 reading of the contract (tests/metrics_emulator.py) computes.  install() routes the product's
+storing what the float64 reading of the contract (tests/metrics_emulator.py) computes; the pooling between MS-SSIM
+scales is cpu_backend's b200_interpolate.  install() routes the product's
 C-ABI calls, the sampling path's included, to it."""
 import ctypes as C
 
-import numpy as np
 import torch
 
 from generativemodels_b200 import _lib
 from tests import cpu_backend
 from tests import metrics_emulator as M
 from tests.cpu_backend import _np, _obj, store32
-
-_CTYPES = {_lib.DT_F32: (C.c_float, np.float32, None), _lib.DT_F64: (C.c_double, np.float64, None),
-           _lib.DT_FP16: (C.c_uint16, np.int16, torch.float16), _lib.DT_BF16: (C.c_uint16, np.int16, torch.bfloat16)}
-
-
-def view(ptr, dt, strides, shape):
-    """A strided host view of a metric input in any of its four formats."""
-    ctype, npt, as_dtype = _CTYPES[dt]
-    count = 1 + sum((s - 1) * st for s, st in zip(shape, strides))
-    flat = torch.from_numpy(_np(ptr, count, ctype).view(npt))
-    return torch.as_strided(flat.view(as_dtype) if as_dtype else flat, tuple(shape), tuple(strides))
+from tests.cpu_backend import _strided as view
 
 
 class MetricsFakeLib(cpu_backend.FakeLib):
@@ -56,10 +46,6 @@ class MetricsFakeLib(cpu_backend.FakeLib):
             store32(p.cs_mean, cs)
         if p.ms_ssim:
             store32(p.ms_ssim, M.combine(ssim, cs, list(p.weights[:S])))
-        return 0
-
-    def b200_avgpool2_f32(self, x, dt, xs, N_, C_, D, H, W_, dims, y, stream):
-        store32(y, M.avgpool2(view(x, dt, [int(v) for v in xs[:5]], (N_, C_, D, H, W_)), dims))
         return 0
 
     def b200_mmd_workspace_bytes(self, shape):

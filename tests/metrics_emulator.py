@@ -1,9 +1,12 @@
-"""Float64 reading of the metric entry points of include/b200gen_metrics.h (b200_ssim, b200_ssim_combine, b200_avgpool2_f32,
-b200_mmd), the contract the GPU tests hold the kernels to and the CPU stand-in computes with.  Inputs are converted to
-fp32 first, as the kernels load them; the filters, moments and sums are then float64, so a kernel's fp32 arithmetic
-shows up as its difference from this reading.  The pooling is restated exactly (fp32 sums in d, h, w order)."""
+"""Float64 reading of the metric entry points of include/b200gen_metrics.h (b200_ssim, b200_ssim_combine, b200_mmd),
+the contract the GPU tests hold the kernels to and the CPU stand-in computes with.  Inputs are converted to fp32 first,
+as the kernels load them; the filters, moments and sums are then float64, so a kernel's fp32 arithmetic shows up as its
+difference from this reading.  The pooling between MS-SSIM scales is b200_interpolate's: ``pool`` reads it with
+tests/rescaler_oracle.py, exactly."""
 import torch
 import torch.nn.functional as F
+
+from tests import rescaler_oracle as R
 
 F64 = torch.float64
 
@@ -39,18 +42,13 @@ def combine(ssim_means, cs_means, weights):
     return torch.prod(v.to(F64).clamp_min(0) ** w, dim=0)
 
 
-def avgpool2(x, dims):
-    """b200_avgpool2_f32: fp32 window sums in d, h, w order, divided by 4 or 8, floor extents."""
-    x = x.float()
+def pool(x, dims):
+    """ops.avgpool2_f32 of a 5-D [N, C, D, H, W] tensor (2-D: D == 1, not pooled): AREA over the even part of each
+    pooled extent, fp32."""
     N, C, D, H, W = x.shape
-    OD = D // 2 if dims == 3 else D
-    pd = 2 if dims == 3 else 1
-    s = torch.zeros(N, C, OD, H // 2, W // 2)
-    for dd in range(pd):
-        for hh in range(2):
-            for ww in range(2):
-                s = s + x[:, :, dd:dd + pd * OD:pd, hh:hh + 2 * (H // 2):2, ww:ww + 2 * (W // 2):2]
-    return s / (8.0 if dims == 3 else 4.0)
+    out = (D // 2 if dims == 3 else D, H // 2, W // 2)
+    src = (2 * out[0] if dims == 3 else D, 2 * out[1], 2 * out[2])
+    return R.header_interpolate(x[:, :, :src[0], :src[1], :src[2]], out, (1.0, 1.0, 1.0), R.AREA)
 
 
 def mmd(y, y_pred):

@@ -13,7 +13,6 @@ the arithmetic its kernel documents:
   GroupNorm out   h16(act(fma(x, a, b))); SiLU as x / (1 + e^-x) within the error of __expf / __fdividef.
   SPADE out       h16(act(fma(nx, 1 + gg, tt))), nx = fma(x, ax, bx), gg = fma(g, ag, bg), tt = fma(t, at, bt).
   LayerNorm out   h16((x - mean) rstd gamma + beta); the rows_linear prologue stages the same h16 row.
-  resize_nearest  src = min(floor(dst * fp32(in / out)), in - 1) per axis, the product in fp32: F.interpolate's index.
   pads            output channels [C, y_pitch) are +0.
 
 16-bit rounding goes through fp32 (the kernels round their fp32 values with RN); fp16 stores saturate at +-65504.
@@ -39,7 +38,6 @@ import contextlib
 import math
 from dataclasses import dataclass
 
-import numpy as np
 import torch
 
 from generativemodels_b200._lib import ACT_DTYPE
@@ -315,20 +313,3 @@ def layernorm(x, M, C, x_pitch, gamma, beta, eps, y_pitch):
 def rows_linear_ln(x, M, K, x_pitch, gamma, beta, eps):
     """The LayerNorm prologue of b200_rows_linear: the staged h16 row [M, K] (what an identity weight returns)."""
     return layernorm(x, M, K, x_pitch, gamma, beta, eps, K)
-
-
-# ----------------------------------------------------------------------------------------------------------------
-# resize_nearest
-# ----------------------------------------------------------------------------------------------------------------
-def nearest_index(n_in, n_out):
-    """min(floor(dst * fp32(in / out)), in - 1) with the product rounded to fp32, as the kernel and F.interpolate."""
-    scale = np.float32(n_in) / np.float32(n_out)
-    dst = np.arange(n_out, dtype=np.float32)
-    return torch.from_numpy(np.minimum(np.floor(dst * scale).astype(np.int64), n_in - 1))
-
-
-def resize_nearest(x, N, D, H, W, pitch, OD, OH, OW):
-    """b200_resize_nearest: [N][OD][OH][OW][pitch] gathered from [N][D][H][W][pitch] (every channel, pads included)."""
-    X = x[:N * D * H * W * pitch].view(N, D, H, W, pitch)
-    idd, ih, iw = nearest_index(D, OD), nearest_index(H, OH), nearest_index(W, OW)
-    return X[:, idd][:, :, ih][:, :, :, iw]

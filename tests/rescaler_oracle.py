@@ -1,12 +1,14 @@
 """Plain restatements for SpatialRescaler (generative/networks/blocks/encoder_modules.py) and b200_interpolate.
 
 ``header_interpolate`` evaluates include/b200gen.h's b200_interpolate rules literally (per-axis fp32 coordinates, then
-one dense weight matrix per resampled axis, applied in float64): tests/test_spatial_rescaler_cpu.py pins it against
-F.interpolate, which pins the documented rules to ATen's; tests/cpu_backend.py stands it in for the entry point, so
-the module's host code runs end to end without a GPU.  ``rescaler`` is the module
+one dense weight matrix per resampled axis, applied in float64; AREA as the header's fp32 sequence, exactly):
+tests/test_spatial_rescaler_cpu.py pins it against F.interpolate, which pins the documented rules to ATen's;
+tests/cpu_backend.py stands it in for the entry point, so the module's host code runs end to end without a GPU.
+``resample_cl`` is the channels-last call ops makes for nearest x2, nearest resizing and the 2x average pool.  ``rescaler`` is the module
 itself in plain PyTorch, from a ``state_dict`` and the constructor arguments.  Test infrastructure only."""
 from __future__ import annotations
 
+import itertools
 import math
 import zlib
 
@@ -66,13 +68,43 @@ def axis_weights(mode: int, n_in: int, n_out: int, ratio: float) -> np.ndarray:
 
 
 def header_interpolate(x: torch.Tensor, out_sizes, ratios, mode: int) -> torch.Tensor:
-    """b200_interpolate of a planar [N, C, *spatial] tensor (1 to 3 resampled axes), as float32."""
+    """b200_interpolate of a planar [N, C, *spatial] tensor (1 to 3 resampled axes, any input dtype: values are
+    converted to fp32 on load), as float32."""
+    x = x.float()
+    if mode == AREA:
+        return _area(x, out_sizes)
     y = x.double()
     dims = x.dim() - 2
     for a in range(dims):
         m = torch.from_numpy(axis_weights(mode, x.shape[2 + a], out_sizes[a], ratios[a]))
         y = torch.movedim(torch.tensordot(y, m, dims=([2 + a], [1])), -1, 2 + a)
     return y.float()
+
+
+def _area(x: torch.Tensor, out_sizes) -> torch.Tensor:
+    """AREA in fp32: each window summed from 0 in d, h, w order (the last axis innermost), then divided by the
+    window's extent along each axis in turn."""
+    wins = [[(o * n // m, -(-(o + 1) * n // m)) for o in range(m)] for n, m in zip(x.shape[2:], out_sizes)]
+    starts = [torch.tensor([s for s, _ in w]) for w in wins]
+    ext = [torch.tensor([e - s for s, e in w]) for w in wins]
+    shape = lambda a: [-1 if b == a else 1 for b in range(len(wins))]
+    acc = torch.zeros(*x.shape[:2], *out_sizes)
+    for taps in itertools.product(*(range(int(e.max())) for e in ext)):
+        idx = [(s + t).clamp_max(n - 1).view(shape(a)) for a, (s, t, n) in enumerate(zip(starts, taps, x.shape[2:]))]
+        ok = math.prod((t < e).view(shape(a)) for a, (t, e) in enumerate(zip(taps, ext)))
+        acc = acc + torch.where(ok.bool(), x[(slice(None), slice(None), *idx)], 0.0)
+    for a, e in enumerate(ext):
+        acc = acc / e.float().view(shape(a))
+    return acc
+
+
+def resample_cl(x: torch.Tensor, dims, mode: int, src=None) -> torch.Tensor:
+    """ops' channels-last resampling: [N, D, H, W, pitch] (its first ``src`` voxels per axis) -> [N, *dims, pitch]
+    float32, every channel, all three axes resampled with ratios fp32(in / out)."""
+    src = tuple(src or x.shape[1:4])
+    planar = x[:, :src[0], :src[1], :src[2]].permute(0, 4, 1, 2, 3)
+    ratios = [float(np.float32(i) / np.float32(o)) for i, o in zip(src, dims)]
+    return header_interpolate(planar, dims, ratios, mode).permute(0, 2, 3, 4, 1)
 
 
 def rescaler(sd: dict, x: torch.Tensor, n_stages: int = 1, size=None, method: str = "bilinear",

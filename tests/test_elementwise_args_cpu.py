@@ -41,30 +41,16 @@ def ddpm(var_mode=0):
 
 HIST = (C.c_void_p * 4)(P, Q, R, P)
 HIST_NULL = (C.c_void_p * 4)(P, None, R, P)
+ST = (C.c_int64 * 5)(64, 16, 16, 16, 1)                      # planar strides: the one-element-per-thread path
+INTERP = (1, 1, 1, 1, 8, 1, 1, 4, 1, _lib.INTERPOLATE_LINEAR, 1.0, 1.0, 2.0, None)
 
 # entry point, arguments outside the contract, the same call inside it
 CASES = {
     "nchw_to_nhwc_pitch_below_C": ("b200_nchw_to_nhwc", (P, 1, 8, 64, Q, 7, None), (P, 1, 8, 64, Q, 8, None)),
     "nchw_to_nhwc_N_above_65535": ("b200_nchw_to_nhwc", (P, 65536, 8, 64, Q, 8, None), (P, 65535, 8, 64, Q, 8, None)),
     "nhwc_to_nchw_spatial_0": ("b200_nhwc_to_nchw", (P, 0, 1, 8, 0, 8, Q, None), (P, 0, 1, 8, 1, 8, Q, None)),
-    "upsample_x_misaligned": ("b200_upsample_nearest2x", (P + 2, 1, 1, 4, 4, 8, 2, Q, None),
-                              (P, 1, 1, 4, 4, 8, 2, Q, None)),
-    "upsample_y_misaligned": ("b200_upsample_nearest2x", (P, 1, 1, 4, 4, 8, 2, Q + 8, None),
-                              (P, 1, 1, 4, 4, 8, 2, Q, None)),
-    "upsample_pitch_0": ("b200_upsample_nearest2x", (P, 1, 1, 4, 4, 0, 2, Q, None), (P, 1, 1, 4, 4, 8, 2, Q, None)),
-    "upsample_pitch_not_multiple_of_8": ("b200_upsample_nearest2x", (P, 1, 1, 4, 4, 12, 2, Q, None),
-                                         (P, 1, 1, 4, 4, 16, 2, Q, None)),
-    "upsample_N_0": ("b200_upsample_nearest2x", (P, 0, 1, 4, 4, 8, 2, Q, None), (P, 1, 1, 4, 4, 8, 2, Q, None)),
-    "upsample_D_0": ("b200_upsample_nearest2x", (P, 1, 0, 4, 4, 8, 3, Q, None), (P, 1, 1, 4, 4, 8, 3, Q, None)),
-    "upsample_H_negative": ("b200_upsample_nearest2x", (P, 1, 1, -4, 4, 8, 2, Q, None), (P, 1, 1, 4, 4, 8, 2, Q, None)),
-    "upsample_W_0": ("b200_upsample_nearest2x", (P, 1, 1, 4, 0, 8, 2, Q, None), (P, 1, 1, 4, 1, 8, 2, Q, None)),
-    "upsample_dims_1": ("b200_upsample_nearest2x", (P, 1, 1, 4, 4, 8, 1, Q, None), (P, 1, 1, 4, 4, 8, 2, Q, None)),
-    "avgpool_x_misaligned": ("b200_avgpool2", (P + 4, 1, 2, 4, 4, 8, 3, Q, None), (P, 1, 2, 4, 4, 8, 3, Q, None)),
-    "avgpool_y_misaligned": ("b200_avgpool2", (P, 1, 2, 4, 4, 8, 3, Q + 2, None), (P, 1, 2, 4, 4, 8, 3, Q, None)),
-    "avgpool_pitch_0": ("b200_avgpool2", (P, 1, 2, 4, 4, 0, 3, Q, None), (P, 1, 2, 4, 4, 8, 3, Q, None)),
-    "avgpool_N_negative": ("b200_avgpool2", (P, -1, 2, 4, 4, 8, 3, Q, None), (P, 1, 2, 4, 4, 8, 3, Q, None)),
-    "avgpool_D_0": ("b200_avgpool2", (P, 1, 0, 4, 4, 8, 2, Q, None), (P, 1, 1, 4, 4, 8, 2, Q, None)),
-    "avgpool_H_0": ("b200_avgpool2", (P, 1, 2, 0, 4, 8, 3, Q, None), (P, 1, 2, 4, 4, 8, 3, Q, None)),
+    "interpolate_y_dtype_f64": ("b200_interpolate", (P, 2, ST, Q, 2, ST, *INTERP), (P, 2, ST, Q, 1, ST, *INTERP)),
+    "interpolate_x_dtype_5": ("b200_interpolate", (P, 5, ST, Q, 1, ST, *INTERP), (P, 4, ST, Q, 1, ST, *INTERP)),
     "axpy_a_misaligned": ("b200_axpy_h16", (P + 2, Q, 1.0, R, 64, None), (P, Q, 1.0, R, 64, None)),
     "axpy_b_misaligned": ("b200_axpy_h16", (P, Q + 8, 1.0, R, 64, None), (P, Q, 1.0, R, 64, None)),
     "axpy_y_misaligned": ("b200_axpy_h16", (P, Q, 1.0, R + 4, 64, None), (P, Q, 1.0, R, 64, None)),

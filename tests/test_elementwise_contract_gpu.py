@@ -149,7 +149,7 @@ def test_layout_conversion_bit_exact(cuda_device, lib, name, n, Cc, S, pitch, sc
 
 
 # ------------------------------------------------------------------------------------------------------------------
-# upsample_nearest2x, avgpool2, axpy_h16
+# nearest x2 and the 2x average pool (b200_interpolate as ops calls it), axpy_h16
 # ------------------------------------------------------------------------------------------------------------------
 RESAMPLE = [  # name, N, D, H, W, C, pitch, dims, scale
     ("dims2_N2_C16_5x6", 2, 1, 5, 6, 16, 16, 2, 1.0),
@@ -161,24 +161,34 @@ RESAMPLE = [  # name, N, D, H, W, C, pitch, dims, scale
 
 
 @pytest.mark.parametrize("name,n,D,H,W,Cc,pitch,dims,scale", RESAMPLE, ids=[c[0] for c in RESAMPLE])
-def test_upsample_avgpool_bit_exact(cuda_device, lib, name, n, D, H, W, Cc, pitch, dims, scale):
+def test_nearest2x_avgpool2_through_interpolate_bit_exact(cuda_device, lib, name, n, D, H, W, Cc, pitch, dims, scale):
     g = gen(name)
     X = torch.zeros(n * D * H * W, pitch)
     X[:, :Cc] = scale * torch.randn(n * D * H * W, Cc, generator=g)
-    x = h16_of(X).reshape(-1)                                 # pad channels 0: every channel is processed
-    xd = x.cuda()
-    for entry, fn, emu in (("upsample_nearest2x", lib.b200_upsample_nearest2x, E.upsample_nearest2x),
-                           ("avgpool2", lib.b200_avgpool2, E.avgpool2)):
-        want = emu(x, n, D, H, W, pitch, dims).out
+    x = h16_of(X).view(n, D, H, W, pitch)                    # pad channels 0: every channel is processed
+    xd = ops.CL(x.cuda(), Cc, dims)
+    ncd = x.double().permute(0, 4, 1, 2, 3)
+    if dims == 2:                                            # D slices, each resampled in 2-D
+        ncd = ncd.transpose(1, 2).reshape(n * D, pitch, H, W)
+    up = F.interpolate(ncd, scale_factor=2.0, mode="nearest")
+    pool = (F.avg_pool3d if dims == 3 else F.avg_pool2d)(ncd, 2, 2)
+    even = [D if dims == 2 else D // 2 * 2, H // 2 * 2, W // 2 * 2]           # AvgPool's floor windows
+    for entry, fn, want, mode, src in (("upsample_nearest2x", ops.upsample_nearest2x, up, _lib.INTERPOLATE_NEAREST, None),
+                                       ("avgpool2", ops.avgpool2, pool, _lib.INTERPOLATE_AREA, even)):
+        if dims == 2:
+            want = want.reshape(n, D, pitch, *want.shape[2:]).transpose(1, 2)
+        want = E.h16(want.permute(0, 2, 3, 4, 1))
         outs = []
         for _ in range(2):
             y = sentinel16(want.numel() + 5 * pitch).cuda()
-            sync_ok(fn(xd.data_ptr(), n, D, H, W, pitch, dims, y.data_ptr(), stream()))
+            ops._resample(xd, want.shape[1:4], mode, src, y[:want.numel()].view(want.shape))
+            torch.cuda.synchronize()
             outs.append(y.cpu())
         y = outs[0]
         assert torch.equal(bits(outs[1]), bits(y)), f"{name}: {entry} repeats differ"
         assert (bits(y[want.numel():]) == SENT16).all(), f"{name}: {entry} stores past the output"
-        assert torch.equal(bits(y[:want.numel()]), bits(want.to(H16))), f"{name}: {entry} differs"
+        assert torch.equal(bits(y[:want.numel()]), bits(want.reshape(-1).to(H16))), f"{name}: {entry} differs"
+        assert torch.equal(bits(fn(xd).t.cpu().reshape(-1)), bits(y[:want.numel()])), f"{name}: ops.{entry} differs"
         ratio_report(entry, name, 0.0)
 
 

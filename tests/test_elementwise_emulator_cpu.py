@@ -1,10 +1,11 @@
 """tests/elementwise_emulator.py against independent float64 references, and its bound against kernel-shaped mutants
 (CPU only).
 
-The emulator has to agree with F.interpolate(nearest), F.avg_pool{2,3}d, F.gelu, F.conv{2,3}d (for the tap pair),
+The emulator, and tests/rescaler_oracle.py's reading of the channels-last resampling calls, have to agree with
+F.interpolate(nearest), F.avg_pool{2,3}d, F.gelu, F.conv{2,3}d (for the tap pair),
 float64 restatements of the DDIM / DDPM / PNDM updates and of the likelihood terms, and torch.cdist's nearest codes.  Its
 bound has to reject the mistakes these kernels make: kh / kw swapped in the tap decode, tap_sum padding off by one, a
-dropped last tap, avgpool2 dividing by 4 in 3-D, the nearest index (o + 1) >> 1, GEGLU halves swapped, copy_channels
+dropped last tap, the 2x average pool dividing by 4 in 3-D, the nearest index (o + 1) >> 1, GEGLU halves swapped, copy_channels
 ignoring dst_off, v-prediction's eps with the wrong sign, DDPM learned_range interpolated in the log domain, sigma
 noise added when noise is NULL, PNDM history weights shifted by one, add_noise ignoring sign_b, the KL t = 0
 thresholds swapped, the KLD sign, VQ ties to the highest index and the VQ tiled tail written from its duplicate.  Each
@@ -21,6 +22,7 @@ import torch.nn.functional as F
 
 from oracle import torch_oracle as O
 from tests import elementwise_emulator as E
+from tests import rescaler_oracle as R
 
 F64 = torch.float64
 FLAVOURS = [torch.float16, torch.bfloat16]
@@ -64,20 +66,20 @@ def test_upsample_and_avgpool_match_torch(dt, dims):
         x = torch.zeros(n, D, H, W, pitch, dtype=E.N.H16)
         x[..., :C] = h16t(X)
         ncd = x[..., :C].to(F64).permute(0, 4, 1, 2, 3)
-        up = E.upsample_nearest2x(x.reshape(-1), n, D, H, W, pitch, dims).out
+        OD = 2 * D if dims == 3 else D
+        got = E.h16(R.resample_cl(x, (OD, 2 * H, 2 * W), R.NEAREST).to(F64))
         if dims == 3:
             want = F.interpolate(ncd, scale_factor=2.0, mode="nearest")
         else:
             want = torch.stack([F.interpolate(ncd[:, :, i], scale_factor=2.0, mode="nearest") for i in range(D)], 2)
-        OD = 2 * D if dims == 3 else D
-        got = up.view(n, OD, 2 * H, 2 * W, pitch)
         assert torch.equal(got[..., :C], want.permute(0, 2, 3, 4, 1)) and (got[..., C:] == 0).all()
-        pool = E.avgpool2(x.reshape(-1), n, D, H, W, pitch, dims).out
+        OD = D // 2 if dims == 3 else D
+        got = E.h16(R.resample_cl(x, (OD, H // 2, W // 2), R.AREA,
+                                  src=(2 * OD if dims == 3 else D, H // 2 * 2, W // 2 * 2)).to(F64))
         if dims == 3:
             want = F.avg_pool3d(ncd, 2, 2)
         else:
             want = torch.stack([F.avg_pool2d(ncd[:, :, i], 2, 2) for i in range(D)], 2)
-        got = pool.view(n, D // 2 if dims == 3 else D, H // 2, W // 2, pitch)
         assert torch.equal(got[..., :C], E.h16(want.permute(0, 2, 3, 4, 1))) and (got[..., C:] == 0).all()
 
 
@@ -396,10 +398,10 @@ def test_bound_rejects_resampling_and_copy_mutants(dt):
         g = gen("rsmut")
         n, D, H, W, p = 1, 4, 6, 6, 8
         x = h16t(torch.randn(n * D * H * W * p, generator=g) + 2).to(F64)
-        r = E.avgpool2(x, n, D, H, W, p, 3)
-        rejects("avgpool2_3d_divides_by_4", dt, r, E.h16(r.out * 2))
-        r = E.upsample_nearest2x(x, n, D, H, W, p, 3)
         X = x.view(n, D, H, W, p)
+        r = E.copy(E.h16(R.resample_cl(X, (D // 2, H // 2, W // 2), R.AREA).to(F64)).reshape(-1))
+        rejects("avgpool2_3d_divides_by_4", dt, r, E.h16(r.out * 2))
+        r = E.copy(E.h16(R.resample_cl(X, (2 * D, 2 * H, 2 * W), R.NEAREST).to(F64)).reshape(-1))
         i = lambda e: ((torch.arange(2 * e) + 1) >> 1).clamp_max(e - 1)
         m = X[:, i(D)][:, :, i(H)][:, :, :, i(W)]
         rejects("nearest_index_o_plus_1", dt, r, m.reshape(-1))

@@ -452,7 +452,7 @@ def test_layernorm_geglu(cuda_device):
 # ------------------------------------------------------------------------------------------------ resampling
 def test_resample(cuda_device):
     """Through the ops wrappers (layout conversion, pitch, allocation): the F.interpolate / avg_pool / a + alpha b
-    checks, and the contract of tests/elementwise_emulator.py on top (avgpool2 bit-exact, axpy one ulp)."""
+    checks, bit-exact for avgpool2 (b200_interpolate's AREA sums in fp32 and divides exactly)."""
     from tests import elementwise_emulator as E
     ops = _ops()
     for shape in ((2, 16, 5, 6), (1, 24, 3, 4, 5)):

@@ -102,7 +102,7 @@ def test_ms_ssim_odd_extents_match_the_contract(cuda_device, sd, shape, ks, w, d
         sm, cm = M.ssim(x, y, taps, scale, 1e-4, 9e-4)
         ss.append(M.per_item_means(sm).float())
         cc.append(M.per_item_means(cm).float())
-        x, y = M.avgpool2(x, sd), M.avgpool2(y, sd)
+        x, y = M.pool(x, sd), M.pool(y, sd)
     want = M.combine(torch.stack(ss), torch.stack(cc), w)
     err = (got.double().view(-1) - want).abs().max().item()
     print(f"ms-ssim {shape} k={ks} {dtype}: max |got - reading| = {err:.3e}")
@@ -114,7 +114,7 @@ def test_pooling_is_exact(cuda_device):
     x = torch.rand(2, 3, 9, 13, 11, device=DEV)[:, :, :, 1:, :]
     for sd, v in ((3, x), (2, x[:, :, :1])):
         got = ops.avgpool2_f32(v, sd).cpu()
-        assert torch.equal(got, M.avgpool2(v.cpu(), sd))
+        assert torch.equal(got, M.pool(v.cpu(), sd))
 
 
 @pytest.mark.parametrize("dtype", [torch.float32, torch.float16, torch.bfloat16, torch.float64])

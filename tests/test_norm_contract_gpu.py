@@ -532,30 +532,29 @@ def test_rows_linear_layernorm_prologue_matches_emulator(cuda_device, lib, M, K,
 
 
 # ------------------------------------------------------------------------------------------------------------------
-# b200_resize_nearest
+# nearest resizing (b200_interpolate as ops.resize_nearest calls it)
 # ------------------------------------------------------------------------------------------------------------------
 RESIZE = [("2d_26x6_to_22x74", 2, 1, 26, 6, 1, 22, 74, 12), ("3d_14x6x26_to_46x74x22", 1, 14, 6, 26, 46, 74, 22, 8),
           ("3d_6x14x26_to_74x46x22_pitch3", 2, 6, 14, 26, 74, 46, 22, 3)]
 
 
 @pytest.mark.parametrize("name,N,D,H,W,OD,OH,OW,pitch", RESIZE, ids=[r[0] for r in RESIZE])
-def test_resize_nearest_bit_exact(cuda_device, lib, name, N, D, H, W, OD, OH, OW, pitch):
+def test_resize_nearest_through_interpolate_bit_exact(cuda_device, lib, name, N, D, H, W, OD, OH, OW, pitch):
     g = gen(name)
     x = torch.randn(N, D, H, W, pitch, generator=g).to(H16)
     x[..., pitch - 1] = 0.0 if pitch > 4 else x[..., pitch - 1]    # a pad channel: copied as it is
-    want = E.resize_nearest(x.reshape(-1), N, D, H, W, pitch, OD, OH, OW)
     ncd = x.float().permute(0, 4, 1, 2, 3)
-    ref = F.interpolate(ncd, size=(OD, OH, OW), mode="nearest").permute(0, 2, 3, 4, 1).to(H16)
-    assert torch.equal(bits(ref), bits(want))
+    want = F.interpolate(ncd, size=(OD, OH, OW), mode="nearest").permute(0, 2, 3, 4, 1).to(H16)
     n = N * OD * OH * OW * pitch
     y = sentinel(n + 37).cuda()
-    xd = x.cuda()
-    rc = lib.b200_resize_nearest(xd.data_ptr(), N, D, H, W, pitch, y.data_ptr(), OD, OH, OW, ops._stream())
+    xd = ops.CL(x.cuda(), pitch, 3)
+    ops._resample(xd, (OD, OH, OW), _lib.INTERPOLATE_NEAREST, y=y[:n].view(N, OD, OH, OW, pitch))
     torch.cuda.synchronize()
-    assert rc == 0, _lib.last_error()
     y = y.cpu()
     assert (bits(y[n:]) == SENT16).all(), "stores past the output"
     assert torch.equal(bits(y[:n]), bits(want.reshape(-1))), f"{name}: differs from F.interpolate"
+    got = ops.resize_nearest(xd, (OD, OH, OW)).t.cpu()
+    assert torch.equal(bits(got.reshape(-1)), bits(y[:n])), f"{name}: ops.resize_nearest differs"
 
 
 # ------------------------------------------------------------------------------------------------------------------

@@ -10,11 +10,13 @@ Each mutant prints its excess factor (max err / tol) in both storage flavours.
 import math
 import zlib
 
+import numpy as np
 import pytest
 import torch
 import torch.nn.functional as F
 
 from tests import norm_emulator as E
+from tests import rescaler_oracle as R
 
 F64 = torch.float64
 FLAVOURS = [torch.float16, torch.bfloat16]
@@ -132,7 +134,8 @@ def test_nearest_index_is_f_interpolates_for_every_pair_up_to_79():
         src = torch.arange(n_in, dtype=torch.float32).view(1, 1, n_in)
         for n_out in range(1, 80):
             got = F.interpolate(src, size=n_out, mode="nearest").view(-1).long()
-            assert torch.equal(E.nearest_index(n_in, n_out), got), (n_in, n_out)
+            index = R.axis_weights(R.NEAREST, n_in, n_out, np.float32(n_in) / np.float32(n_out)).argmax(1)
+            assert torch.equal(torch.from_numpy(index), got), (n_in, n_out)
 
 
 @pytest.mark.parametrize("dims", [2, 3])
@@ -141,7 +144,7 @@ def test_resize_nearest_emulator_matches_f_interpolate(dims):
     N, pitch = 2, 8
     D, H, W, OD, OH, OW = (1, 26, 6, 1, 22, 74) if dims == 2 else (14, 6, 26, 46, 74, 22)
     x = torch.randn(N, D, H, W, pitch, generator=g)
-    got = E.resize_nearest(x.reshape(-1), N, D, H, W, pitch, OD, OH, OW)
+    got = R.resample_cl(x, (OD, OH, OW), R.NEAREST)
     ncd = x.permute(0, 4, 1, 2, 3)
     if dims == 2:
         want = F.interpolate(ncd[:, :, 0], size=(OH, OW), mode="nearest")[:, :, None]
@@ -250,7 +253,8 @@ def test_bound_rejects_partial_slot_read_off_by_one(dt):
 def test_exact_rational_nearest_index_differs():
     for n_in, n_out in ((26, 22), (6, 74), (14, 46)):
         rational = torch.minimum(torch.arange(n_out) * n_in // n_out, torch.tensor(n_in - 1))
-        bad = int((rational != E.nearest_index(n_in, n_out)).sum())
+        index = R.axis_weights(R.NEAREST, n_in, n_out, np.float32(n_in) / np.float32(n_out)).argmax(1)
+        bad = int((rational != torch.from_numpy(index)).sum())
         print(f"\nMUTANT exact_rational_nearest {n_in}->{n_out} differs at {bad} of {n_out} indices")
         assert bad > 0
 

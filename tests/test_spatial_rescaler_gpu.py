@@ -138,10 +138,10 @@ def test_vector_path_writes_pad_channels_from_the_input(cuda_device):
 
 
 # ---- argument checks ------------------------------------------------------------------------------------------------
-def _call(lib, x, y, mode, dims, ext_in, ext_out, ratios=(1.0, 1.0, 0.5), xs=None, dt=_lib.DT_F32):
+def _call(lib, x, y, mode, dims, ext_in, ext_out, ratios=(1.0, 1.0, 0.5), xs=None, dt=_lib.DT_F32, ydt=None):
     st = (C.c_int64 * 5)(*(xs or (64, 16, 16, 16, 1)))
-    return lib.b200_interpolate(x, dt, st, y, dt, (C.c_int64 * 5)(64, 16, 16, 16, 1), 1, 1, *ext_in, *ext_out, dims,
-                                mode, *ratios, ops._stream())
+    return lib.b200_interpolate(x, dt, st, y, dt if ydt is None else ydt, (C.c_int64 * 5)(64, 16, 16, 16, 1), 1, 1,
+                                *ext_in, *ext_out, dims, mode, *ratios, ops._stream())
 
 
 def test_einval(cuda_device):
@@ -172,6 +172,12 @@ def test_einval(cuda_device):
     assert _call(lib, xp, yp, _lib.INTERPOLATE_LINEAR, 1, (1, 1, 8), (1, 1, 4), xs=(64, 16, 16, 16, -1)) == \
         _lib.B200_EINVAL
     assert _call(lib, xp, yp, _lib.INTERPOLATE_LINEAR, 1, (1, 1, 8), (1, 1, 4), dt=2) == _lib.B200_EINVAL
+    # fp64 / fp16 / bf16 inputs are read on the scalar path; the output stays h16 or fp32
+    for dt in (_lib.DT_F64, _lib.DT_FP16, _lib.DT_BF16):
+        assert _call(lib, xp, yp, _lib.INTERPOLATE_AREA, 1, (1, 1, 8), (1, 1, 4), dt=dt, ydt=_lib.DT_F32) == _lib.B200_OK
+        assert _call(lib, xp, yp, _lib.INTERPOLATE_AREA, 1, (1, 1, 8), (1, 1, 4), dt=_lib.DT_F32, ydt=dt) == \
+            _lib.B200_EINVAL
+    assert _call(lib, xp, yp, _lib.INTERPOLATE_AREA, 1, (1, 1, 8), (1, 1, 4), dt=5, ydt=_lib.DT_F32) == _lib.B200_EINVAL
     torch.cuda.synchronize()
 
 
