@@ -24,8 +24,9 @@ LIB_PATH = _HERE / "lib" / ("libb200gen.so" if ACT_DTYPE == "fp16" else "libb200
 
 B200_OK, B200_EINVAL, B200_ENOTSUP, B200_ECUDA, B200_ENODEV = 0, -1, -2, -3, -4
 DT_H16, DT_F32 = 0, 1
-DT_F64, DT_FP16, DT_BF16 = 2, 3, 4      # inputs only (b200_interpolate's x, b200_ssim, b200_mmd)
+DT_F64, DT_FP16, DT_BF16 = 2, 3, 4      # inputs only (b200_interpolate's x, b200_ssim, b200_mmd, b200_fid_moments)
 SSIM_MAX_K, SSIM_MAX_SCALES = 128, 32
+FID_MAX_F = 32768
 H16_FP16, H16_BF16 = 0, 1
 ACT_NONE, ACT_RELU, ACT_SILU, ACT_LEAKYRELU, ACT_GELU, ACT_TANH, ACT_SIGMOID = 0, 1, 2, 3, 4, 5, 6
 ACT_GEGLU = 7        # b200_igemm act1 only: [32 a | 32 gate] column groups -> a * gelu(gate), half as many output channels
@@ -137,6 +138,17 @@ class SsimCombineParams(C.Structure):
                 ("ssim_mean", C.c_void_p), ("cs_mean", C.c_void_p), ("ms_ssim", C.c_void_p)]
 
 
+class FidMomentsParams(C.Structure):
+    _fields_ = [("x", C.c_void_p), ("x_dtype", C.c_int32), ("F", C.c_int32), ("n", C.c_int64),
+                ("x_strides", C.c_int64 * 2), ("mu", C.c_void_p), ("sigma", C.c_void_p)]
+
+
+class FrechetParams(C.Structure):
+    _fields_ = [("mu_x", C.c_void_p), ("sigma_x", C.c_void_p), ("mu_y", C.c_void_p), ("sigma_y", C.c_void_p),
+                ("F", C.c_int32), ("reserved", C.c_int32), ("workspace", C.c_void_p), ("out", C.c_void_p),
+                ("eigvals", C.c_void_p), ("rank", C.c_void_p)]
+
+
 REPACK_BLOCKS, REPACK_TAP_IN, REPACK_TAP_OUT = 0, 1, 2
 
 _P, _I32, _I64, _F = C.c_void_p, C.c_int32, C.c_int64, C.c_float
@@ -205,9 +217,16 @@ METRIC_SIGNATURES = {
     "b200_mmd_workspace_bytes": [_P],
     "b200_mmd": [_P, _I32, _P, _P, _I32, _P, _P, _P, _P, _P],
 }
+# FID's entry points; mirrors include/b200gen_fid.h exactly
+FID_SIGNATURES = {
+    "b200_fid_moments": [C.POINTER(FidMomentsParams), _P],
+    "b200_frechet_workspace_bytes": [_I32],
+    "b200_frechet": [C.POINTER(FrechetParams), _P],
+}
 _RESTYPES = {"b200_last_error_string": C.c_char_p, "b200_groupnorm_workspace_bytes": C.c_int64,
              "b200_attention_flash_workspace_bytes": C.c_int64, "b200_igemm_split_workspace_bytes": C.c_int64,
-             "b200_ssim_workspace_bytes": C.c_int64, "b200_mmd_workspace_bytes": C.c_int64}
+             "b200_ssim_workspace_bytes": C.c_int64, "b200_mmd_workspace_bytes": C.c_int64,
+             "b200_frechet_workspace_bytes": C.c_int64}
 
 _lib = None
 _device_ok = False
@@ -223,12 +242,13 @@ def load():
             f"{LIB_PATH} is missing: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
             "(generativemodels_b200/csrc/build.sh). There is no fallback path.")
     lib = C.CDLL(str(LIB_PATH))
-    for name, argtypes in {**SIGNATURES, **METRIC_SIGNATURES}.items():
+    for name, argtypes in {**SIGNATURES, **METRIC_SIGNATURES, **FID_SIGNATURES}.items():
         fn = getattr(lib, name)  # AttributeError if the .so does not export it
         fn.argtypes = argtypes
         fn.restype = _RESTYPES.get(name, C.c_int)
     for which, struct in enumerate((IgemmParams, GnStatsParams, GnApplyParams, DdimCoef, DdpmCoef, PndmCoef, IgemmSeg,
-                                    FlashParams, KlCoef, RepackBlock, SsimParams, SsimCombineParams)):
+                                    FlashParams, KlCoef, RepackBlock, SsimParams, SsimCombineParams,
+                                    FidMomentsParams, FrechetParams)):
         c_size = lib.b200_abi_sizeof(which)
         if c_size != C.sizeof(struct):
             raise B200Error(f"ABI mismatch: {struct.__name__} is {C.sizeof(struct)} bytes in Python but {c_size} in "

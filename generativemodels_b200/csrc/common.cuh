@@ -136,6 +136,10 @@ __device__ __forceinline__ float load_any(const void* p, int dt, int64_t i) {
     default: return __bfloat162float(static_cast<const __nv_bfloat16*>(p)[i]);
   }
 }
+// the same element as fp64 (exact for every format)
+__device__ __forceinline__ double load_any_f64(const void* p, int dt, int64_t i) {
+  return dt == B200_DT_F64 ? static_cast<const double*>(p)[i] : static_cast<double>(load_any(p, dt, i));
+}
 
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll

@@ -1,6 +1,7 @@
 // Error reporting, version and device checks for libb200gen.so.
 #include "common.cuh"
 #include "../../include/b200gen_metrics.h"
+#include "../../include/b200gen_fid.h"
 
 namespace b200 {
 
@@ -72,6 +73,8 @@ extern "C" int b200_abi_sizeof(int which) {
     case 9: return (int)sizeof(b200_repack_block);
     case 10: return (int)sizeof(b200_ssim_params);
     case 11: return (int)sizeof(b200_ssim_combine_params);
+    case 12: return (int)sizeof(b200_fid_moments_params);
+    case 13: return (int)sizeof(b200_frechet_params);
     default: return -1;
   }
 }

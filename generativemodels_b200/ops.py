@@ -1456,3 +1456,40 @@ def mmd(y: torch.Tensor, y_pred: torch.Tensor) -> torch.Tensor:
     check(lib.b200_mmd(y.data_ptr(), _metric_dt(y), ys, y_pred.data_ptr(), _metric_dt(y_pred), ps, shape,
                        ws.data_ptr(), out.data_ptr(), _stream()), "b200_mmd")
     return out
+
+
+def fid_moments(x: torch.Tensor) -> tuple[torch.Tensor, torch.Tensor]:
+    """fp64 column mean [F] and covariance (X - mu)^T (X - mu) / (n - 1) [F, F] of a 2-D [n, F] view (n >= 2) of any
+    strides in fp32 / fp64 / fp16 / bf16, read in place."""
+    lib = _lib.require_device()
+    p = _lib.FidMomentsParams()
+    p.x, p.x_dtype = x.data_ptr(), _metric_dt(x)
+    p.n, p.F = x.shape
+    p.x_strides[:] = x.stride()
+    mu = torch.empty(p.F, dtype=torch.float64, device=x.device)
+    sigma = torch.empty((p.F, p.F), dtype=torch.float64, device=x.device)
+    p.mu, p.sigma = mu.data_ptr(), sigma.data_ptr()
+    check(lib.b200_fid_moments(C.byref(p), _stream()), "b200_fid_moments")
+    return mu, sigma
+
+
+def frechet(mu_x: torch.Tensor, sigma_x: torch.Tensor, mu_y: torch.Tensor, sigma_y: torch.Tensor,
+            details: bool = False):
+    """|mu_x - mu_y|^2 + tr sigma_x + tr sigma_y - 2 tr sqrt(sigma_x sigma_y) from contiguous fp64 mu [F] and symmetric
+    PSD sigma [F, F]: a 0-dim fp64 tensor; with ``details`` also the F eigenvalues of M = G^T sigma_x G (ascending, fp64)
+    and the rank of sigma_y's pivoted Cholesky factor G (0-dim int32)."""
+    lib = _lib.require_device()
+    F_ = mu_x.shape[0]
+    p = _lib.FrechetParams()
+    p.mu_x, p.sigma_x, p.mu_y, p.sigma_y = (t.data_ptr() for t in (mu_x, sigma_x, mu_y, sigma_y))
+    p.F = F_
+    nbytes = lib.b200_frechet_workspace_bytes(F_)
+    if nbytes < 0:
+        raise NotImplementedError(f"the Frechet distance takes 1 to {_lib.FID_MAX_F} features, got {F_}")
+    ws = torch.empty((nbytes + 7) // 8, dtype=torch.float64, device=mu_x.device)
+    out = torch.empty((), dtype=torch.float64, device=mu_x.device)
+    eig = torch.empty(F_, dtype=torch.float64, device=mu_x.device) if details else None
+    rank = torch.empty((), dtype=torch.int32, device=mu_x.device) if details else None
+    p.workspace, p.out, p.eigvals, p.rank = ws.data_ptr(), out.data_ptr(), _ptr(eig), _ptr(rank)
+    check(lib.b200_frechet(C.byref(p), _stream()), "b200_frechet")
+    return (out, eig, rank) if details else out

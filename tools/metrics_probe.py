@@ -3,12 +3,18 @@ reference's arithmetic (oracle/metrics_oracle.py: full-kernel F.conv{2,3}d, F.av
 card, and record the card's name and power limit from the same run.  Prints one JSON line; --out also writes it to a
 file.
 
+FID rows time FIDMetric / compute_frechet_distance against tests/fid_oracle.py (torch fp64 moments on the GPU, scipy
+sqrtm on the host; one untimed-warm-up-free call, as the host sqrtm dominates) and add a per-stage split and the launch
+count from a separate torch.profiler pass: moments, factor (pivoted Cholesky), M (the two GEMMs), tridiagonalisation,
+bisection and finish.
+
     python tools/metrics_probe.py [--iters 10] [--out results/metrics_probe.json]
 """
 import argparse
 import json
 import subprocess
 import sys
+import time
 from pathlib import Path
 
 import torch
@@ -17,7 +23,10 @@ ROOT = Path(__file__).resolve().parents[1]
 sys.path.insert(0, str(ROOT))
 
 from generativemodels_b200 import metrics as GM  # noqa: E402
+from generativemodels_b200 import ops  # noqa: E402
 from oracle import metrics_oracle as MO  # noqa: E402
+from tests import fid_oracle as FO  # noqa: E402
+from tests.golden.make_golden_fid import features  # noqa: E402
 
 BRAIN = (1, 1, 160, 224, 160)
 
@@ -39,6 +48,62 @@ def time_ms(fn, iters, warmup=2):
     end.record()
     torch.cuda.synchronize()
     return start.elapsed_time(end) / iters
+
+
+STAGES = [("moments", ("fid_colmean",)), ("factor", ("fid_chol",)), ("tridiagonalisation", ("fid_house", "fid_symv",
+           "fid_rank2", "fid_tri_tail")), ("bisection", ("fid_bisect",)), ("finish", ("fid_finish",))]
+
+
+def fid_stages(moments, frechet):
+    """Per-stage kernel time (ms) and launch count of one call, from torch.profiler: fid_dgemm is the moments' Gram
+    under `moments` and the M products under `frechet`."""
+    from torch.profiler import ProfilerActivity, profile
+    split, launches = {}, 0
+    for part, fn in (("moments", moments), ("frechet", frechet)):
+        fn()
+        torch.cuda.synchronize()
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            fn()
+            torch.cuda.synchronize()
+        for ev in prof.key_averages():
+            if ev.device_type != torch.autograd.DeviceType.CUDA or "fid_" not in ev.key:
+                continue
+            stage = "M" if "fid_dgemm" in ev.key and part == "frechet" else "moments" if "fid_dgemm" in ev.key else \
+                next((n for n, keys in STAGES if any(k in ev.key for k in keys)), "other")
+            split[stage] = round(split.get(stage, 0.0) + ev.device_time_total / 1e3, 3)
+            launches += ev.count
+    return split, launches
+
+
+def fid_rows(iters):
+    rows = {}
+    for name, (n, F) in {"fid_1000x2048_vs_1000x2048": (1000, 2048), "fid_10000x2048_vs_10000x2048": (10000, 2048),
+                         "fid_5000x4096_vs_5000x4096": (5000, 4096)}.items():
+        p, y = features(n, F, 1, shift=0.1).cuda(), features(n, F, 2).cuda()
+        stats = [ops.fid_moments(p), ops.fid_moments(y)]
+        rows[name] = (lambda p=p, y=y: GM.FIDMetric()(p, y), lambda p=p, y=y: FO.fid(p, y),
+                      lambda p=p, y=y: (ops.fid_moments(p), ops.fid_moments(y)),
+                      lambda s=stats: ops.frechet(*s[0], *s[1]))
+        if F == 2048 and n == 10000:
+            rows["compute_frechet_distance_cached_F2048"] = (
+                lambda s=stats: GM.compute_frechet_distance(*s[0], *s[1]),
+                lambda s=stats: FO.frechet_distance(*s[0], *s[1]), lambda: None,
+                lambda s=stats: ops.frechet(*s[0], *s[1]))
+    out = {}
+    for name, (ours, base, mom, fre) in rows.items():
+        o = time_ms(ours, iters)
+        torch.cuda.synchronize()
+        t0 = time.perf_counter()
+        ref = base()
+        torch.cuda.synchronize()
+        bl = (time.perf_counter() - t0) * 1e3
+        split, launches = fid_stages(mom, fre)
+        got = float(ours())
+        out[name] = {"ms": round(o, 3), "oracle_ms": round(bl, 1), "speedup": round(bl / o, 1),
+                     "stages_ms": split, "launches": launches, "fid": got,
+                     "rel_diff_vs_oracle": abs(got - float(ref)) / max(abs(float(ref)), 1e-300)}
+        print(name, out[name], flush=True)
+    return out
 
 
 def main():
@@ -73,6 +138,7 @@ def main():
             res["cases"][name] = {"ms": round(o, 4), "torch_restatement_ms": round(bl, 4),
                                   "speedup": round(bl / o, 1), "max_abs_diff_vs_restatement": diff}
             print(name, res["cases"][name], flush=True)
+    res["cases"].update(fid_rows(max(2, args.iters // 5)))
     print(json.dumps(res))
     if args.out:
         Path(args.out).parent.mkdir(parents=True, exist_ok=True)
