@@ -223,6 +223,12 @@ FID_SIGNATURES = {
     "b200_frechet_workspace_bytes": [_I32],
     "b200_frechet": [C.POINTER(FrechetParams), _P],
 }
+# the perceptual distance's entry points; mirrors include/b200gen_perceptual.h exactly
+PERCEPTUAL_SIGNATURES = {
+    "b200_perceptual_prep": [_P, _I32, _P, _P, _I32, _P, _I32, _I32, _I32, _I32, _P, _I32, _P, _P, _P],
+    "b200_perceptual_distance": [_P, _P, _I32, _I32, _I32, _I32, _I32, _P, _P, _P, _P],
+    "b200_perceptual_mean": [_P, _I32, _P, _P, _P, _P],
+}
 _RESTYPES = {"b200_last_error_string": C.c_char_p, "b200_groupnorm_workspace_bytes": C.c_int64,
              "b200_attention_flash_workspace_bytes": C.c_int64, "b200_igemm_split_workspace_bytes": C.c_int64,
              "b200_ssim_workspace_bytes": C.c_int64, "b200_mmd_workspace_bytes": C.c_int64,
@@ -242,7 +248,7 @@ def load():
             f"{LIB_PATH} is missing: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
             "(generativemodels_b200/csrc/build.sh). There is no fallback path.")
     lib = C.CDLL(str(LIB_PATH))
-    for name, argtypes in {**SIGNATURES, **METRIC_SIGNATURES, **FID_SIGNATURES}.items():
+    for name, argtypes in {**SIGNATURES, **METRIC_SIGNATURES, **FID_SIGNATURES, **PERCEPTUAL_SIGNATURES}.items():
         fn = getattr(lib, name)  # AttributeError if the .so does not export it
         fn.argtypes = argtypes
         fn.restype = _RESTYPES.get(name, C.c_int)

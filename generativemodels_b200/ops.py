@@ -462,12 +462,13 @@ _SPLIT_K = True          # tests and probes set it to False to compare split and
 _SPLIT_LAUNCHES = 0      # calls that went through the split-K pair of kernels (tests / probes read it)
 
 
-def igemm_raw(p: IgemmParams) -> None:
+def igemm_raw(p: IgemmParams, split_k: bool = True) -> None:
     """One b200_igemm launch.  Calls whose grid cannot fill the SMs (deep levels of a latent UNet, single-sample
-    linears) get the split-K workspace the library asks for; everything else is a single kernel."""
+    linears) get the split-K workspace the library asks for; everything else is a single kernel.  ``split_k=False``
+    keeps every call one pass, so a row's result does not depend on how many other rows the call has."""
     lib = _lib.require_device()
     ws = None
-    if _SPLIT_K and not p.split_ws:
+    if _SPLIT_K and split_k and not p.split_ws:
         need = int(lib.b200_igemm_split_workspace_bytes(C.byref(p)))
         if need:
             global _SPLIT_LAUNCHES
@@ -540,10 +541,11 @@ def _conv_params(srcs: Sequence[CL], w: torch.Tensor, segs, stride, out_t: torch
 
 def conv(srcs: CL | Sequence[CL], pc: PackedConv, *, rowvec: torch.Tensor | None = None, act1: int = ACT_NONE,
          scale: float = 1.0, residual: CL | None = None, act2: int = ACT_NONE, out_f32: bool = False,
-         impl: int = 0, out: CL | None = None) -> CL | torch.Tensor:
+         impl: int = 0, out: CL | None = None, gn_stats: bool = True, split_k: bool = True) -> CL | torch.Tensor:
     """Fused convolution: act2(residual + scale * act1(conv(cat(srcs)) + bias + rowvec[n])).
 
     Returns a :class:`CL` (h16) or, with ``out_f32``, an fp32 channels-last tensor ``[N, D, H, W, round_up(C, 4)]``.
+    ``gn_stats=False`` skips the GroupNorm partial sums for an output no GroupNorm reads; ``split_k``: igemm_raw.
     """
     if isinstance(srcs, CL):
         srcs = [srcs]
@@ -568,13 +570,9 @@ def conv(srcs: CL | Sequence[CL], pc: PackedConv, *, rowvec: torch.Tensor | None
     if impl == 0 and rows >= _TAP_MIN_ROWS and pc.tap_in is not None:
         # conv_in-like: im2col of the few input channels (one h16 row of <= 64 values per output voxel), then the
         # ordinary fused GEMM epilogue
-        lib = _lib.require_device()
-        Kp = round_up(pc.tap_in.K, 8)
-        x2 = torch.empty((a0.N, *od, Kp), dtype=H16, device=a0.t.device)
-        check(lib.b200_tap_gather(a0.t.data_ptr(), a0.C, a0.pitch, pc.geom(a0.N, a0.D, a0.H, a0.W), x2.data_ptr(), Kp,
-                                  _stream()), "b200_tap_gather")
+        x2 = tap_gather(a0, pc.geom(a0.N, a0.D, a0.H, a0.W), pc.k[0] * pc.k[1] * pc.k[2])
         pl = pc.tap_in
-        p = _conv_params([CL(x2, pl.K, a0.spatial_dims)], pl.w, pl.segs, (1, 1, 1), out_t, od, pc.cout,
+        p = _conv_params([x2], pl.w, pl.segs, (1, 1, 1), out_t, od, pc.cout,
                          DT_F32 if out_f32 else DT_H16, pl.bias, rowvec, act1, scale,
                          None if residual is None else residual.t, DT_H16, act2)
         igemm_raw(p)
@@ -590,12 +588,15 @@ def conv(srcs: CL | Sequence[CL], pc: PackedConv, *, rowvec: torch.Tensor | None
         return out
     p = _conv_params(srcs, pc.w, pc.segs, pc.stride, out_t, od, pc.cout, DT_F32 if out_f32 else DT_H16, pc.bias,
                      rowvec, act1, scale, None if residual is None else residual.t, DT_H16, act2, impl=impl)
-    if not out_f32:
+    if not out_f32 and gn_stats:
         part = _gn_partial_for(out, rows, len(pc.segs))
         if part is not None:
             p.gn_partial, p.gn_slots, p.gn_slot0 = part.data_ptr(), part.shape[1], 0
             p.gn_group = _gn_group(out)
-    igemm_raw(p)
+    if split_k:          # the one-argument call keeps substitutes of igemm_raw(p) working
+        igemm_raw(p)
+    else:
+        igemm_raw(p, split_k=False)
     return out
 
 
@@ -623,8 +624,8 @@ def as_rows(t: torch.Tensor, C_: int) -> CL:
 
 
 def linear(x: CL, pl: PackedLinear, *, residual: CL | None = None, act1: int = ACT_NONE, out_f32: bool = False,
-           impl: int = 0):
-    """y = x @ W^T + b over the channel dim of any CL (rows = voxels)."""
+           impl: int = 0, split_k: bool = True):
+    """y = x @ W^T + b over the channel dim of any CL (rows = voxels); ``split_k``: igemm_raw."""
     if x.C != pl.K:
         raise ValueError(f"linear expects {pl.K} input features, got {x.C}")
     if out_f32:
@@ -635,8 +636,23 @@ def linear(x: CL, pl: PackedLinear, *, residual: CL | None = None, act1: int = A
         out_t = out.t
     p = _conv_params([x], pl.w, pl.segs, (1, 1, 1), out_t, (x.D, x.H, x.W), pl.cout, DT_F32 if out_f32 else DT_H16,
                      pl.bias, None, act1, 1.0, None if residual is None else residual.t, DT_H16, ACT_NONE, impl=impl)
-    igemm_raw(p)
+    if split_k:          # the one-argument call keeps substitutes of igemm_raw(p) working
+        igemm_raw(p)
+    else:
+        igemm_raw(p, split_k=False)
     return out
+
+
+def tap_gather(x: CL, geom, taps: int) -> CL:
+    """b200_tap_gather: the im2col rows [N, OD, OH, OW, round_up(taps * C, 8)] of a convolution geometry ``geom``
+    (PackedConv.geom's 16 values), for a GEMM over K = taps * C."""
+    lib = _lib.require_device()
+    K = taps * x.C
+    od = tuple(geom[4:7])
+    out = torch.empty((x.N, *od, round_up(K, 8)), dtype=H16, device=x.t.device)
+    check(lib.b200_tap_gather(x.t.data_ptr(), x.C, x.pitch, geom, out.data_ptr(), out.shape[-1], _stream()),
+          "b200_tap_gather")
+    return CL(out, K, x.spatial_dims)
 
 
 # --------------------------------------------------------------------------------------------------
@@ -1493,3 +1509,41 @@ def frechet(mu_x: torch.Tensor, sigma_x: torch.Tensor, mu_y: torch.Tensor, sigma
     p.workspace, p.out, p.eigvals, p.rank = ws.data_ptr(), out.data_ptr(), _ptr(eig), _ptr(rank)
     check(lib.b200_frechet(C.byref(p), _stream()), "b200_frechet")
     return (out, eig, rank) if details else out
+
+
+# ------------------------------------------------------------------------------------------------
+# Perceptual distance (generativemodels_b200.losses): the network's input preparation and the feature distance.
+# ------------------------------------------------------------------------------------------------
+def perceptual_prep(x: torch.Tensor, y: torch.Tensor, strides: Sequence[Sequence[int]], S: int, OH: int, OW: int,
+                    idx: torch.Tensor | None, n_out: int, out: torch.Tensor) -> None:
+    """b200_perceptual_prep: ``n_out`` z-scored 3-channel images of x and of y into ``out[:n_out]`` and
+    ``out[n_out:]`` (h16 [2 * n_out, 1, OH, OW, 8]).  ``strides`` = the {image, channel, slice, row, column} element
+    strides of x and of y; ``idx`` (int64, on the device) picks the source images, None takes 0 .. n_out - 1."""
+    lib = _lib.require_device()
+    half = n_out * OH * OW * 8 * out.element_size()
+    check(lib.b200_perceptual_prep(x.data_ptr(), _metric_dt(x), (C.c_int64 * 5)(*strides[0]), y.data_ptr(),
+                                   _metric_dt(y), (C.c_int64 * 5)(*strides[1]), x.shape[1], S, OH, OW, _ptr(idx),
+                                   n_out, out.data_ptr(), out.data_ptr() + half, _stream()), "b200_perceptual_prep")
+
+
+def perceptual_distance(fx: torch.Tensor, fy: torch.Tensor, C_: int, image: torch.Tensor,
+                        image32: torch.Tensor | None = None) -> None:
+    """b200_perceptual_distance of two channels-last feature maps [B, D, H, W, pitch] (fp32 or h16) into the fp64
+    per-image values ``image`` [B] (and their fp32 copy ``image32``)."""
+    lib = _lib.require_device()
+    B = fx.shape[0]
+    HW = fx.shape[1] * fx.shape[2] * fx.shape[3]
+    dt = DT_F32 if fx.dtype == torch.float32 else DT_H16
+    pixel = torch.empty(B * HW, dtype=torch.float32, device=fx.device)
+    check(lib.b200_perceptual_distance(fx.data_ptr(), fy.data_ptr(), dt, B, HW, C_, fx.shape[-1], pixel.data_ptr(),
+                                       image.data_ptr(), _ptr(image32), _stream()), "b200_perceptual_distance")
+
+
+def perceptual_mean(image: torch.Tensor, counts: Sequence[int]) -> tuple[torch.Tensor, torch.Tensor]:
+    """b200_perceptual_mean: (fp64 [len(counts) + 1] group means and their sum, fp32 0-dim loss)."""
+    lib = _lib.require_device()
+    means = torch.empty(len(counts) + 1, dtype=torch.float64, device=image.device)
+    loss = torch.empty((), dtype=torch.float32, device=image.device)
+    check(lib.b200_perceptual_mean(image.data_ptr(), len(counts), (C.c_int32 * len(counts))(*counts),
+                                   means.data_ptr(), loss.data_ptr(), _stream()), "b200_perceptual_mean")
+    return means, loss
