@@ -174,7 +174,11 @@ def affine_table(mean, rstd, d_mean, d_rstd, gamma, beta, groups):
 
 def gn_affine(X, groups, eps, gamma, beta, stat=STAT_GN):
     """The affine table b200_groupnorm_stats / _fused compute from the inputs X [N, spatial, C]."""
-    mean, var, piv = group_moments(X, groups)
+    return stats_affine(*group_moments(X, groups), eps, gamma, beta, groups, stat)
+
+
+def stats_affine(mean, var, piv, eps, gamma, beta, groups, stat=STAT_GN):
+    """gn_affine from the float64 moments and pivots [N, groups] of the inputs."""
     s2 = var + eps
     rstd = 1.0 / torch.sqrt(s2)
     off = (mean - piv).abs()
