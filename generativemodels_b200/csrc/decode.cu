@@ -54,6 +54,11 @@ __global__ void __launch_bounds__(256) rows_linear_kernel(const h16* __restrict_
     for (int k0 = lane * 8; k0 < Kp; k0 += 256) {
       float wf[8];
       unpack8(__ldg(reinterpret_cast<const uint4*>(wr + k0)), wf);
+      if (k0 + 8 > K) {                    // W columns [K, Kp) are ignored: 0 x NaN there would poison the row
+#pragma unroll
+        for (int e = 0; e < 8; ++e)
+          if (k0 + e >= K) wf[e] = 0.f;
+      }
 #pragma unroll
       for (int m = 0; m < kRowsMax; ++m) {
         if (m < M) {

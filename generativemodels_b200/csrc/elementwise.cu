@@ -62,11 +62,12 @@ __global__ void nhwc_to_nchw_kernel(const T* __restrict__ x, int C, long long sp
 // 8 channels).  Output o = 2i + parity reads source coordinate s = i - 0.25 (even) or i + 0.25 (odd), so each axis has
 // two sets of taps and weights, picked by parity.
 // ------------------------------------------------------------------------------------------------
-// bilinear: s clamped at 0 (only the first even output is affected: it copies row 0)
+// bilinear: s clamped at 0 (only the first even output is affected: taps 0 and min(1, n - 1) with weights 1 and 0,
+// as ATen computes it, so an inf in row 0 stays inf)
 __device__ __forceinline__ void interp_taps_linear(int o, int n, int* idx, float* w) {
   const int i = o >> 1;
   if (o & 1)       { idx[0] = i;     idx[1] = min(i + 1, n - 1); w[0] = 0.75f; w[1] = 0.25f; }
-  else if (i == 0) { idx[0] = 0;     idx[1] = 0;                 w[0] = 1.0f;  w[1] = 0.0f;  }
+  else if (i == 0) { idx[0] = 0;     idx[1] = min(1, n - 1);     w[0] = 1.0f;  w[1] = 0.0f;  }
   else             { idx[0] = i - 1; idx[1] = i;                 w[0] = 0.25f; w[1] = 0.75f; }
 }
 // bicubic: upsample_bicubic2d's cubic convolution (A = -0.75) at fraction t = 0.75 (even) or 0.25 (odd), taps
@@ -342,7 +343,11 @@ __global__ void __launch_bounds__(256) interpolate_kernel(const InterpArgs a) {
         if (a.dims >= 2) interp_taps_linear_any(oh, a.H, a.OH, a.rh, hi, hw);
         if (a.dims == 3) interp_taps_linear_any(od, a.D, a.OD, a.rd, di, dw);
       }
-      const int TH = a.dims >= 2 ? T : 1, TD = a.dims == 3 ? 2 : 1;
+      // a linear-family axis with out == in is a copy: its one tap (weight 1) is read and the zero-weight partner
+      // skipped, so that inf stays inf instead of becoming inf * 0 = NaN
+      const bool lin = FAM == INTERP_FAM_LINEAR;
+      const int TW = lin && a.W == a.OW ? 1 : T;
+      const int TH = a.dims >= 2 && !(lin && a.H == a.OH) ? T : 1, TD = a.dims == 3 && a.D != a.OD ? 2 : 1;
 #pragma unroll
       for (int p = 0; p < 2; ++p) {
         if (p >= TD) break;
@@ -353,6 +358,7 @@ __global__ void __launch_bounds__(256) interpolate_kernel(const InterpArgs a) {
           float row[V];
 #pragma unroll
           for (int k = 0; k < T; ++k) {
+            if (k >= TW) break;
             float f[V];
             interp_load<V>(a.x, a.x_dt, xb + di[p] * a.xs[2] + hi[q] * a.xs[3] + wi[k] * a.xs[4], f);
 #pragma unroll

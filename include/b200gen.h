@@ -271,11 +271,16 @@ int b200_nhwc_to_nchw(const void* x, int32_t x_dtype, int32_t N, int32_t C, int6
 /* nn.Upsample(scale_factor=2, mode="bilinear" | "bicubic") on a 2-D NHWC h16 tensor [N][H][W][pitch] -> [N][2H][2W][pitch]
  * (SPADEDecoder's upsampling_mode, nets/spade_network.py:280,317), PyTorch's align_corners=False semantics: source
  * coordinate s = (dst + 0.5) / 2 - 0.5 per axis;
- *   B200_INTERP_BILINEAR: s clamped at 0, taps floor(s) and min(floor(s) + 1, in - 1);
+ *   B200_INTERP_BILINEAR: s clamped at 0, taps floor(s) and min(floor(s) + 1, in - 1) (the first even output: taps 0
+ *                         and min(1, in - 1) with weights 1 and 0, as ATen computes it: an inf in row 0 stays inf, an
+ *                         inf in row 1 makes it NaN);
  *   B200_INTERP_BICUBIC : s not clamped, taps floor(s) - 1 .. floor(s) + 2 each clamped to [0, in - 1], Keys cubic
  *                         convolution weights with A = -0.75 (upsample_bicubic2d), rows interpolated first.
- * At the fixed x2 scale the weights depend only on the output parity.  fp32 arithmetic, one rounding on the store;
- * pad channels are interpolated like the others (zeros stay zeros).  pitch % 8 == 0. */
+ * At the fixed x2 scale the weights depend only on the output parity and are dyadic (0.25 / 0.75; Keys weights at
+ * t = 0.25 / 0.75, at most 9 significant bits).  Arithmetic: along W within each source row an fp32 fma chain from 0
+ * over the taps (each product exact, so one rounding per sum), then along H an fp32 fma chain from 0 over those rows;
+ * one rounding on the store (fp16 saturates).  Every channel of the pitch is interpolated (zero pads stay zero).
+ * pitch % 8 == 0, x and y 16-byte aligned. */
 #define B200_INTERP_BILINEAR 0
 #define B200_INTERP_BICUBIC  1
 int b200_upsample2x_interp(const void* x, int32_t N, int32_t H, int32_t W, int32_t pitch, int32_t mode, void* y,
@@ -286,8 +291,9 @@ int b200_upsample2x_interp(const void* x, int32_t N, int32_t H, int32_t W, int32
  * (ceil_mode=False); requires 2 * padding <= kernel and in + 2 * padding >= kernel.
  *   B200_POOL_AVG: count_include_pad=True, i.e. the sum of the in-bounds taps divided by kernel^dims;
  *   B200_POOL_MAX: padding taps are -inf; a NaN tap makes the result NaN (PyTorch's max_pool semantics).
- * fp32 arithmetic, one rounding on the store (max is exact); pad channels stay zero.  pitch % 8 == 0, x and y
- * 16-byte aligned. */
+ * Arithmetic: avg sums the in-bounds taps in fp32 in d, h, w order from 0 (each partial sum rounded) and divides once
+ * (IEEE) by kernel^dims; max is exact.  One rounding on the store (fp16 saturates).  Every channel of the pitch is
+ * pooled (zero pads stay zero).  pitch % 8 == 0, x and y 16-byte aligned. */
 #define B200_POOL_AVG 0
 #define B200_POOL_MAX 1
 int b200_pool_s2(const void* x, int32_t N, int32_t D, int32_t H, int32_t W, int32_t pitch, int32_t dims,
@@ -309,7 +315,8 @@ int b200_pool_s2(const void* x, int32_t N, int32_t D, int32_t H, int32_t W, int3
  * scale_factor=0.5 but 0.5625, 2.6875, ... with size=8).  s = fma(r, dst + 0.5, -0.5) in fp32, one rounding, which is
  * ATen's r * (dst + 0.5) - 0.5 as its compilers contract it.
  *   NEAREST  : src = min(floor(dst * r), in - 1) (no identity shortcut: scale_factor=1.1 on 5 samples 0,0,1,2,3);
- *   linear family (LINEAR / BILINEAR / TRILINEAR): an axis with out == in is copied (taps dst, dst; weights 1, 0);
+ *   linear family (LINEAR / BILINEAR / TRILINEAR): an axis with out == in is copied (its one tap dst read with weight
+ *              1, so inf and NaN pass through);
  *              otherwise s is clamped at 0, i0 = min(floor(s), in - 1), i1 = i0 + (i0 < in - 1),
  *              l = clamp(s - i0, 0, 1), weights (1 - l, l);
  *   BICUBIC  : s not clamped, f = min(floor(s), in - 1), t = clamp(s - f, 0, 1), taps f - 1 .. f + 2 each clamped to
@@ -430,10 +437,16 @@ int b200_cache_append(const void* src, void* cache, int32_t B, int32_t T, int32_
                       const int32_t* pos_dev, void* stream);
 int b200_advance_i32(int32_t* p, int32_t delta, void* stream);
 /* Decode-time linear layers (one new token per sequence: M <= 8 rows, HBM/L2-bound GEMVs):
- *   out[m, o] = act( LN?(x[m, :]) . w[o, :] + bias[o] ) + res[m, o]
+ *   out[m, o] = act( LN?(x[m, :]) . w[o, :K] + bias[o] ) + res[m, o]
  * x h16 rows; ln_gamma / ln_beta (NULL = no LayerNorm; nn.LayerNorm semantics with b200_layernorm's arithmetic and
- * accuracy, the row rounded to h16 as the stand-alone kernel does); w = the K-major h16 matrix b200_igemm consumes (row pitch w_pitch, multiple of 8);
- * out h16 or fp32 (out_dtype).  (blocks/transformerblock.py:87-92, blocks/selfattention.py:103-110, 145.) */
+ * accuracy, the row rounded to h16 as the stand-alone kernel does); w = the K-major h16 matrix b200_igemm consumes (row
+ * pitch w_pitch, a multiple of 8 and >= round_up(K, 8), 16-byte aligned); bias fp32 or NULL; res h16 or NULL; out h16 or
+ * fp32 (out_dtype).  Arithmetic: each of a warp's 32 lanes sums 8 columns of every 256 in an fp32 fma chain
+ * (8 ceil(K / 256) terms), a 5-level butterfly folds the lanes, then the bias add, act (b200_small_linear's), the
+ * residual add in fp32 and one rounding on an h16 store (fp16 saturates).  Not read: x columns [K, x_pitch), w columns
+ * [K, w_pitch), res columns [O, r_pitch).  Not written: out columns [O, o_pitch).  B200_EINVAL for M outside 1..8,
+ * M * round_up(K, 8) * 2 > 48 KB, or a pitch below its row.  (blocks/transformerblock.py:87-92,
+ * blocks/selfattention.py:103-110, 145.) */
 int b200_rows_linear(const void* x, int32_t x_pitch, int32_t M, int32_t K, const float* ln_gamma,
                      const float* ln_beta, float ln_eps, const void* w, int32_t w_pitch, int32_t O, const float* bias,
                      int32_t act, const void* res, int32_t r_pitch, void* out, int32_t o_pitch, int32_t out_dtype,
@@ -581,7 +594,9 @@ int b200_repack_weight(const float* src, int32_t cout, int32_t cin, int32_t taps
  *   s[co] = gamma[co] / sqrt(var[co] + eps)
  *   w_out[co][j] = w[co][j] * s[co]                       for j < per_out (= cin * taps, the parameter's layout)
  *   b_out[co]    = beta[co] + (b[co] - mean[co]) * s[co]  (b == NULL: a convolution without bias, b = 0)
- * fp64 arithmetic, one rounding to fp32 per output.  All arrays fp32 device memory. */
+ * IEEE fp64 arithmetic (division, square root, multiplication), one rounding to fp32 per output: w_out is exact to
+ * that; b_out's multiply-add may be contracted into a double fma, which can move it to the neighbouring fp32 value.
+ * All arrays fp32 device memory.  B200_EINVAL for a NULL array other than b, cout or per_out < 1, or eps < 0. */
 int b200_batchnorm_fold(const float* w, const float* b, const float* gamma, const float* beta, const float* mean,
                         const float* var, float eps, int32_t cout, int64_t per_out, float* w_out, float* b_out,
                         void* stream);

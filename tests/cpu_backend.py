@@ -3,22 +3,20 @@ drives the real host code (generativemodels_b200: modules, weight packing, sched
 to end on a machine without a GPU.  It is never importable from the product package.
 
 The stand-in is marshalling: each method views its pointers as flat host tensors, calls the float64 reading of the
-entry point that the GPU contract tests hold the kernels to (tests/{igemm,norm,attention,elementwise}_emulator.py) and
-stores that reading's rounded result.  Only the entry points or outputs those readings do not cover are restated
-here: the GEMV of rows_linear, the pooling, interpolation and BatchNorm-fold entry points of the discriminator, SPADE
-and rescaler networks, weight repacking, the position counter of advance_i32 and the host queries."""
+entry point that the GPU contract tests hold the kernels to (tests/{igemm,norm,attention,elementwise,resample}_emulator.py)
+and stores that reading's rounded result.  Only weight repacking (compared bit for bit on the GPU), the position
+counter of advance_i32 and the host queries are restated here."""
 import ctypes as C
 
 import numpy as np
 import torch
-import torch.nn.functional as F
 
 from generativemodels_b200 import _lib, ops
 from tests import attention_emulator as A
 from tests import elementwise_emulator as W
 from tests import igemm_emulator as E
 from tests import norm_emulator as N
-from tests.rescaler_oracle import header_interpolate
+from tests import resample_emulator as R
 
 F64 = torch.float64
 
@@ -175,28 +173,21 @@ class FakeLib:
         return 0
 
     def b200_upsample2x_interp(self, x, N_, H, W_, pitch, mode, y, stream):
-        src = bf16(x, N_ * H * W_ * pitch).view(N_, H, W_, pitch).float().permute(0, 3, 1, 2)
-        m = "bilinear" if mode == _lib.INTERP_BILINEAR else "bicubic"
-        out = F.interpolate(src, scale_factor=2, mode=m).permute(0, 2, 3, 1)
-        store16(y, out)
+        store16(y, R.upsample2x_interp(bf16(x, N_ * H * W_ * pitch), N_, H, W_, pitch, mode).out)
         return 0
 
     def b200_pool_s2(self, x, N_, D, H, W_, pitch, dims, k, pad, mode, y, stream):
-        src = bf16(x, N_ * D * H * W_ * pitch).view(N_, D, H, W_, pitch).float().permute(0, 4, 1, 2, 3)
-        kk, pp, ss = ((k, k, k), (pad, pad, pad), 2) if dims == 3 else ((1, k, k), (0, pad, pad), (1, 2, 2))
-        if mode == _lib.POOL_AVG:
-            o = F.avg_pool3d(src, kk, ss, pp, count_include_pad=True)
-        else:
-            o = F.max_pool3d(src, kk, ss, pp)
-        store16(y, o.permute(0, 2, 3, 4, 1))
+        store16(y, R.pool_s2(bf16(x, N_ * D * H * W_ * pitch), N_, D, H, W_, pitch, dims, k, pad, mode).out)
         return 0
 
     def b200_interpolate(self, x, xdt, xs, y, ydt, ys, N_, C_, D, H, W_, OD, OH, OW, dims, mode, rd, rh, rw, stream):
         xs, ys = [int(v) for v in xs[:5]], [int(v) for v in ys[:5]]
-        src = _strided(x, xdt, xs, (N_, C_, D, H, W_)).reshape(N_, C_, *(D, H, W_)[3 - dims:])
-        out = header_interpolate(src, (OD, OH, OW)[3 - dims:], (rd, rh, rw)[3 - dims:], mode)
+        if R.vector_path(C_, xdt, xs, ys, int(x), int(y)):
+            C_ = (C_ + 7) // 8 * 8
+        src = _strided(x, xdt, xs, (N_, C_, D, H, W_))
+        r = R.interpolate(src, (OD, OH, OW)[3 - dims:], (rd, rh, rw)[3 - dims:], mode, ydt == _lib.DT_H16)
         dst = _strided(y, ydt, ys, (N_, C_, OD, OH, OW))
-        dst.copy_(out.reshape(N_, C_, OD, OH, OW).to(dst.dtype))
+        dst.copy_(r.out.to(dst.dtype))
         return 0
 
     def b200_axpy_h16(self, a, b, alpha, y, n, stream):
@@ -270,19 +261,12 @@ class FakeLib:
         return 0
 
     def b200_rows_linear(self, x, xp, M, K, g, b, eps, w, wp, O, bias, act, res, rp, out, op, odt, stream):
-        """The LayerNorm prologue is the norm reading's; the GEMV is restated in float64."""
-        xs = dense16(x, M, xp, K)
-        xs = N.rows_linear_ln(xs, M, K, K, f32(g, K), f32(b, K), eps).out if g else xs.view(M, K).to(F64)
-        y = xs @ rows16(w, O, wp, K).to(F64).t()
-        if bias:
-            y = y + f32(bias, O).to(F64)
-        y = W.act(y, torch.zeros_like(y), act)[0]
-        if res:
-            y = y + rows16(res, M, rp, O).to(F64)
+        r = W.rows_linear(dense16(x, M, xp, K), K, M, K, f32(g, K), f32(b, K), eps, dense16(w, O, wp, K), K, O,
+                          f32(bias, O), act, dense16(res, M, rp, O) if res else None, O, odt == _lib.DT_H16)
         if odt == _lib.DT_F32:
-            f32(out, M * op).view(M, op)[:, :O] = y.to(torch.float32)
+            f32(out, M * op).view(M, op)[:, :O] = r.out.to(torch.float32)
         else:
-            rows16(out, M, op, O).copy_(N.h16(y).to(ops.H16))
+            rows16(out, M, op, O).copy_(r.out.to(ops.H16))
         return 0
 
     def b200_cache_append(self, src, cache, B, T, L, pitch, pos_dev, stream):
@@ -404,11 +388,10 @@ class FakeLib:
         return 0
 
     def b200_batchnorm_fold(self, w, b, gamma, beta, mean, var, eps, cout, per, w_out, b_out, stream):
-        s = f32(gamma, cout).double() / (f32(var, cout).double() + eps).sqrt()
-        ww = f32(w, cout * per).view(cout, per).double()
-        bb = f32(b, cout).double() if b else torch.zeros(cout, dtype=torch.float64)
-        f32(w_out, cout * per).view(cout, per).copy_(ww * s[:, None])
-        f32(b_out, cout).copy_(f32(beta, cout).double() + (bb - f32(mean, cout).double()) * s)
+        rw, rb = W.batchnorm_fold(f32(w, cout * per), f32(b, cout), *(f32(p, cout) for p in (gamma, beta, mean, var)),
+                                  eps, cout, per)
+        store32(w_out, rw.out)
+        store32(b_out, rb.out)
         return 0
 
 

@@ -279,6 +279,41 @@ def small_linear(x, M, K, W, b, O, act_in, act_out):
     return _res(y, y_err, "f32")
 
 
+def rows_linear(x, x_pitch, M, K, ln_g, ln_b, eps, w, w_pitch, O, bias, act_code, res, r_pitch, out_h16):
+    """b200_rows_linear over [M, O]: act(LN?(x) . w[o, :K] + bias[o]) + res[m, o].  The staged row is
+    norm_emulator.rows_linear_ln's h16 row (its bound plus one 16-bit step) or x itself; each lane runs an fp32 fma
+    chain of 8 ceil(K / 256) terms, a 5-level warp butterfly folds the lanes and the bias adds once:
+    (8 ceil(K / 256) + 7) u (sum |x w| + |bias|); the residual add one rounding more.  Not read: x columns [K, x_pitch),
+    w columns [K, w_pitch), res columns [O, r_pitch)."""
+    if ln_g is not None:
+        ln = N.rows_linear_ln(x, M, K, x_pitch, ln_g, ln_b, eps)
+        X, X_err = ln.exact, ln.err + ulp16(ln.exact.abs() + ln.err)
+    else:
+        X = rows_of(x, M, x_pitch, K)
+        X_err = torch.zeros_like(X)
+    Wm = rows_of(w, O, w_pitch, K)
+    bb = torch.zeros(O, dtype=F64) if bias is None else bias[:O].to(F64)
+    t = X @ Wm.t() + bb[None]
+    n = 8 * math.ceil(K / 256) + 5
+    t_err = (n + 2) * U * (X.abs() @ Wm.abs().t() + bb.abs()[None]) + X_err @ Wm.abs().t()
+    y, y_err = act(t, t_err, act_code)
+    if res is not None:
+        y = y + rows_of(res, M, r_pitch, O)
+        y_err = y_err + U * y.abs()
+    return _res(y, y_err, "h16" if out_h16 else "f32")
+
+
+def batchnorm_fold(w, b, gamma, beta, mean, var, eps, cout, per_out):
+    """(w_out, b_out) of b200_batchnorm_fold: s = gamma / sqrt(var + eps) in IEEE double, w_out = fp32(w s) bit for bit;
+    b_out = fp32(beta + (b - mean) s) or one fp32 neighbour (nvcc may contract the double multiply-add into an fma,
+    which can move a midpoint)."""
+    s = gamma[:cout].to(F64) / torch.sqrt(var[:cout].to(F64) + float(f32(torch.tensor(eps, dtype=F64))))
+    wo = f32(w[:cout * per_out].to(F64).view(cout, per_out) * s[:, None])
+    bb = torch.zeros(cout, dtype=F64) if b is None else b[:cout].to(F64)
+    bo = beta[:cout].to(F64) + (bb - mean[:cout].to(F64)) * s
+    return copy(wo.reshape(-1)), _res(bo, torch.zeros_like(bo), "f32")
+
+
 def pred_x0(m, s, c):
     """x0 and its error from the model output m and the sample s per prediction type (before any clip)."""
     sa, sb = c.sqrt_alpha_prod_t, c.sqrt_beta_prod_t

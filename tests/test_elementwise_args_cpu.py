@@ -127,6 +127,71 @@ CASES = {
 }
 
 
+def interp(N=1, C=1, D=1, H=1, W=8, OD=1, OH=1, OW=4, dims=1, mode=_lib.INTERPOLATE_LINEAR, rd=1.0, rh=1.0, rw=2.0,
+           xs=ST):
+    return (P, 1, xs, Q, 1, ST, N, C, D, H, W, OD, OH, OW, dims, mode, rd, rh, rw, None)
+
+
+def rows_linear(x_pitch=64, M=2, K=64, g=None, b=None, w=Q, w_pitch=64, O=16, res=None, r_pitch=0, o_pitch=16):
+    return (P, x_pitch, M, K, g, b, 1e-5, w, w_pitch, O, None, 0, res, r_pitch, R, o_pitch, 0, None)
+
+
+def pool(pitch=8, x=P, dims=2, k=3, pad=1, mode=_lib.POOL_AVG, H=8):
+    return (x, 1, 1, H, 8, pitch, dims, k, pad, mode, Q, None)
+
+
+def up2(pitch=8, y=Q, mode=_lib.INTERP_BILINEAR, H=4):
+    return (P, 1, H, 4, pitch, mode, y, None)
+
+
+def bnf(gamma=Q, eps=1e-5, cout=4, per=9):
+    return (P, None, gamma, R, P, Q, eps, cout, per, R, P, None)
+
+
+NEG = (C.c_int64 * 5)(64, 16, 16, -16, 1)
+CASES.update({
+    "interpolate_W_2pow24_plus_1": ("b200_interpolate", interp(W=(1 << 24) + 1), interp(W=1 << 24)),
+    "interpolate_OW_2pow24_plus_1": ("b200_interpolate", interp(OW=(1 << 24) + 1), interp(OW=1 << 24)),
+    "interpolate_area_in_out_plus_out_2pow32_plus_1": (
+        "b200_interpolate", interp(W=640, OW=6700417, mode=_lib.INTERPOLATE_AREA),
+        interp(W=65535, OW=65536, mode=_lib.INTERPOLATE_AREA)),
+    "interpolate_bilinear_dims_1": ("b200_interpolate", interp(mode=_lib.INTERPOLATE_BILINEAR),
+                                    interp(mode=_lib.INTERPOLATE_BILINEAR, dims=2)),
+    "interpolate_ratio_0": ("b200_interpolate", interp(rw=0.0), interp(rw=0.5)),
+    "interpolate_ratio_inf": ("b200_interpolate", interp(rw=float("inf")), interp(rw=3.0e38)),
+    "interpolate_negative_stride": ("b200_interpolate", interp(xs=NEG), interp()),
+    "interpolate_D_2_with_dims_2": ("b200_interpolate", interp(D=2, OD=2, dims=2, mode=_lib.INTERPOLATE_NEAREST),
+                                    interp(dims=2, mode=_lib.INTERPOLATE_NEAREST)),
+    "rows_linear_M_9": ("b200_rows_linear", rows_linear(M=9), rows_linear(M=8)),
+    "rows_linear_M_0": ("b200_rows_linear", rows_linear(M=0), rows_linear(M=1)),
+    "rows_linear_w_pitch_below_Kp": ("b200_rows_linear", rows_linear(x_pitch=72, K=65, w_pitch=64),
+                                     rows_linear(x_pitch=72, K=65, w_pitch=72)),
+    "rows_linear_w_pitch_not_multiple_of_8": ("b200_rows_linear", rows_linear(w_pitch=68), rows_linear(w_pitch=72)),
+    "rows_linear_w_misaligned": ("b200_rows_linear", rows_linear(w=Q + 8), rows_linear()),
+    "rows_linear_x_pitch_below_K": ("b200_rows_linear", rows_linear(x_pitch=63), rows_linear(x_pitch=64)),
+    "rows_linear_o_pitch_below_O": ("b200_rows_linear", rows_linear(o_pitch=15), rows_linear(o_pitch=16)),
+    "rows_linear_r_pitch_below_O": ("b200_rows_linear", rows_linear(res=P, r_pitch=15), rows_linear(res=P, r_pitch=16)),
+    "rows_linear_gamma_without_beta": ("b200_rows_linear", rows_linear(g=Q), rows_linear(g=Q, b=R)),
+    "rows_linear_rows_past_48KB": ("b200_rows_linear", rows_linear(x_pitch=3080, M=8, K=3073, w_pitch=3080),
+                                   rows_linear(x_pitch=3080, M=8, K=3072, w_pitch=3080)),
+    "pool_s2_pitch_12": ("b200_pool_s2", pool(pitch=12), pool(pitch=16)),
+    "pool_s2_x_misaligned": ("b200_pool_s2", pool(x=P + 8), pool()),
+    "pool_s2_dims_1": ("b200_pool_s2", pool(dims=1), pool(dims=2)),
+    "pool_s2_mode_2": ("b200_pool_s2", pool(mode=2), pool(mode=_lib.POOL_MAX)),
+    "pool_s2_padding_above_half_kernel": ("b200_pool_s2", pool(k=3, pad=2), pool(k=4, pad=2)),
+    "pool_s2_kernel_0": ("b200_pool_s2", pool(k=0, pad=0), pool(k=1, pad=0)),
+    "pool_s2_input_below_kernel": ("b200_pool_s2", pool(k=4, pad=1, H=1), pool(k=4, pad=1, H=2)),
+    "upsample2x_pitch_4": ("b200_upsample2x_interp", up2(pitch=4), up2(pitch=8)),
+    "upsample2x_y_misaligned": ("b200_upsample2x_interp", up2(y=Q + 2), up2()),
+    "upsample2x_mode_2": ("b200_upsample2x_interp", up2(mode=2), up2(mode=_lib.INTERP_BICUBIC)),
+    "upsample2x_H_0": ("b200_upsample2x_interp", up2(H=0), up2(H=1)),
+    "batchnorm_fold_gamma_null": ("b200_batchnorm_fold", bnf(gamma=None), bnf()),
+    "batchnorm_fold_eps_negative": ("b200_batchnorm_fold", bnf(eps=-1e-5), bnf(eps=0.0)),
+    "batchnorm_fold_cout_0": ("b200_batchnorm_fold", bnf(cout=0), bnf(cout=1)),
+    "batchnorm_fold_per_out_0": ("b200_batchnorm_fold", bnf(per=0), bnf(per=1)),
+})
+
+
 @pytest.fixture(scope="module")
 def lib():
     return _lib.load()

@@ -820,3 +820,85 @@ def test_vq_argmin_gather_matches_emulator(cuda_device, lib, name, M, D, K, ste,
     sync_ok(lib.b200_vq_argmin_gather(xd.data_ptr(), M, D, xp, cd.data_ptr(), K, idx2.data_ptr(), None, 0, None, ste,
                                       None, None, stream()))
     assert torch.equal(idx2.cpu(), idx), f"{name}: indices depend on the optional outputs"
+
+
+# ------------------------------------------------------------------------------------------------------------------
+# rows_linear (decode GEMV) and batchnorm_fold
+# ------------------------------------------------------------------------------------------------------------------
+ACT_GELU = E.ACT_GELU
+RL_K = [1, 7, 8, 9, 255, 256, 257, 3072]
+RL = ([(f"M{M}_K{K}", M, K, 24, True, True, E.ACT_NONE, False, False, 0) for M in (1, 3, 8) for K in RL_K]
+      + [(f"M{M}_K257_gelu_res", M, 257, 40, True, True, ACT_GELU, True, False, 16) for M in range(1, 9)]
+      + [("no_ln_bias_null_f32", 5, 100, 33, False, False, E.ACT_NONE, False, True, 8),
+         ("relu_res_f32", 4, 64, 17, False, True, E.ACT_RELU, True, True, 0),
+         ("silu", 2, 96, 9, True, False, E.ACT_SILU, False, False, 0),
+         ("c5_context_few_rows_K1_O256", 2, 1, 256, False, False, E.ACT_NONE, False, False, 0),
+         ("cxr_context_dim_K1024_O512", 2, 1024, 512, False, False, E.ACT_NONE, False, False, 0),
+         ("decode_qkv_ln_K512", 8, 512, 512, True, True, E.ACT_NONE, False, False, 0),
+         ("decode_mlp1_ln_gelu_K512_O2048", 8, 512, 2048, True, True, ACT_GELU, False, False, 0),
+         ("decode_mlp2_res_K2048_O512", 8, 2048, 512, False, True, E.ACT_NONE, True, False, 0),
+         ("decode_logits_f32_K512_O257", 8, 512, 257, False, True, E.ACT_NONE, False, True, 0),
+         ("grid_loops", 2, 64, -1, False, True, E.ACT_NONE, False, False, 0)])
+
+
+@pytest.mark.parametrize("name,M,K,O,ln,has_b,act,has_res,out_f32,w_extra", RL, ids=[c[0] for c in RL])
+def test_rows_linear_matches_emulator(cuda_device, lib, name, M, K, O, ln, has_b, act, has_res, out_f32, w_extra):
+    """x columns [K, x_pitch), W columns [K, w_pitch) (the chunk pad included) and residual columns past O hold NaN;
+    output columns [O, o_pitch) and rows past M are not written.  O = -1: one past 8 * sm_count * 8 outputs, so the
+    capped grid takes a second pass."""
+    if O < 0:
+        O = 64 * lib.b200_sm_count() + 1
+    g = gen(name)
+    Kp = (K + 7) // 8 * 8
+    xp, wp, rp, op = K + 3, Kp + w_extra, O + 5, O + 8
+    x = nan_rows(h16_of(torch.randn(M, K, generator=g) + 0.5), xp, 1)
+    w = nan_rows(h16_of(torch.randn(O, K, generator=g) / math.sqrt(K)), wp, 0)
+    bias = (0.1 * torch.randn(O, generator=g)).float() if has_b else None
+    gam, bet = ((1 + 0.1 * torch.randn(K, generator=g)).float(), (0.1 * torch.randn(K, generator=g)).float()) if ln \
+        else (None, None)
+    res = nan_rows(h16_of(torch.randn(M, O, generator=g)), rp, 0) if has_res else None
+    want = E.rows_linear(x, xp, M, K, gam, bet, 1e-5, w, wp, O, bias, act, res, rp, not out_f32)
+    dev = [None if t is None else t.cuda() for t in (x, w, bias, gam, bet, res)]
+    xd, wd, bd, gd, btd, rd = dev
+    ptr = lambda t: None if t is None else t.data_ptr()
+    outs = []
+    for _ in range(2):
+        y = (sentinel32 if out_f32 else sentinel16)((M + 1) * op).cuda()
+        rc = lib.b200_rows_linear(xd.data_ptr(), xp, M, K, ptr(gd), ptr(btd), 1e-5, wd.data_ptr(), wp, O, ptr(bd), act,
+                                  ptr(rd), rp, y.data_ptr(), op, DT_F32 if out_f32 else DT_H16, stream())
+        sync_ok(rc)
+        outs.append(y.cpu())
+    y = outs[0]
+    assert torch.equal(bits(outs[1]), bits(y)), f"{name}: a second call stores different bits"
+    body = y.view(M + 1, op)
+    assert torch.isnan(body[:M, O:].float()).all() and torch.isnan(body[M:].float()).all(), f"{name}: footprint"
+    ratio_report("rows_linear", name, check_values(name, want, body[:M, :O].double()))
+
+
+BNF = [("cout8_per27_bias", 8, 27, True, 1e-5, 1.0), ("cout64_per576_no_bias", 64, 576, False, 1e-5, 1.0),
+       ("var_plus_eps_tiny", 16, 9, True, 1e-30, 0.0), ("large_weight_512x12288", 512, 12288, True, 1e-3, 1.0)]
+
+
+@pytest.mark.parametrize("name,cout,per,has_b,eps,var_scale", BNF, ids=[c[0] for c in BNF])
+def test_batchnorm_fold_matches_emulator(cuda_device, lib, name, cout, per, has_b, eps, var_scale):
+    """w_out bit for bit; b_out fp32(beta + (b - mean) s) or one fp32 neighbour."""
+    g = gen(name)
+    w = torch.randn(cout * per, generator=g).float()
+    b = torch.randn(cout, generator=g).float() if has_b else None
+    gamma, beta, mean = (torch.randn(cout, generator=g).float() for _ in range(3))
+    var = (var_scale * torch.rand(cout, generator=g)).float()
+    if var_scale == 0:
+        var[::2] = 1e-30
+    ww, wb = E.batchnorm_fold(w, b, gamma, beta, mean, var, eps, cout, per)
+    dev = [None if t is None else t.cuda() for t in (w, b, gamma, beta, mean, var)]
+    outs = []
+    for _ in range(2):
+        wo, bo = sentinel32(cout * per + 40).cuda(), sentinel32(cout + 40).cuda()
+        rc = lib.b200_batchnorm_fold(*(None if t is None else t.data_ptr() for t in dev), eps, cout, per, wo.data_ptr(),
+                                     bo.data_ptr(), stream())
+        sync_ok(rc)
+        outs.append((wo.cpu(), bo.cpu()))
+    (wo, bo), (wo2, bo2) = outs
+    assert torch.equal(bits(wo), bits(wo2)) and torch.equal(bits(bo), bits(bo2)), f"{name}: repeats differ"
+    check_region(name, wo, 0, cout * per, ww)
+    ratio_report("batchnorm_fold_b", name, check_region(name, bo, 0, cout, wb))

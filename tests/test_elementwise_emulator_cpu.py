@@ -481,3 +481,73 @@ def test_vq_mutants_differ(dt):
         bad = int((hist != r.hist).sum()) + (dup.numel() - M)
         print(f"\nMUTANT vq_tiled_tail_written_from_duplicate {FL_IDS[FLAVOURS.index(dt)]} differs at {bad} entries")
         assert bad > 0
+
+
+# ------------------------------------------------------------------------------------------------------------------
+# rows_linear (decode GEMV) and batchnorm_fold
+# ------------------------------------------------------------------------------------------------------------------
+def _rows_linear_case(M, K, O, flavour, ln=True):
+    g = torch.Generator().manual_seed(1000 * M + K)
+    x = (torch.randn(M, K, generator=g) + 0.5).to(flavour)
+    w = (torch.randn(O, K, generator=g) / K ** 0.5).to(flavour)
+    bias = (0.1 * torch.randn(O, generator=g)).float()
+    gam, bet = (1 + 0.1 * torch.randn(K, generator=g)).float(), (0.1 * torch.randn(K, generator=g)).float()
+    res = torch.randn(M, O, generator=g).to(flavour)
+    return x, w, bias, (gam, bet) if ln else (None, None), res
+
+
+@pytest.mark.parametrize("flavour", FLAVOURS, ids=["fp16", "bf16"])
+@pytest.mark.parametrize("M,K,O,ln,act", [(1, 1, 8, False, E.ACT_NONE), (3, 257, 40, True, E.ACT_GELU),
+                                          (8, 512, 64, True, E.ACT_NONE), (5, 3072, 16, False, E.ACT_RELU)])
+def test_rows_linear_reading_against_float64_linear(flavour, M, K, O, ln, act):
+    """F.linear of F.layer_norm in float64, the activation, the residual: inside the reading's bound."""
+    with E.storage(flavour):
+        x, w, bias, (gam, bet), res = _rows_linear_case(M, K, O, flavour, ln)
+        want = E.rows_linear(x.reshape(-1), K, M, K, gam, bet, 1e-5, w.reshape(-1), K, O, bias, act, res.reshape(-1), O,
+                             True)
+        X = x.double()
+        if ln:
+            X = F.layer_norm(X, (K,), gam.double(), bet.double(), 1e-5)
+        t = F.linear(X, w.double(), bias.double())
+        y = {E.ACT_NONE: t, E.ACT_GELU: F.gelu(t), E.ACT_RELU: F.relu(t)}[act] + res.double()
+        assert (E.excess(want, E.h16(y)) <= 1).all()
+
+
+def _rl_report(name, want, got):
+    r = float(E.excess(want, got).max())
+    print(f"\nMUTANT rows_linear {name} rejected by {r:.3g}x")
+    assert r > 1, name
+
+
+@pytest.mark.parametrize("flavour", FLAVOURS, ids=["fp16", "bf16"])
+def test_rows_linear_bound_rejects_mutants(flavour):
+    M, K, O = 8, 257, 48
+    with E.storage(flavour):
+        x, w, bias, (gam, bet), res = _rows_linear_case(M, K, O, flavour)
+        args = lambda xx, ww, rr: (xx.reshape(-1), K, M, K, gam, bet, 1e-5, ww.reshape(-1), K, O, bias, E.ACT_GELU,
+                                   rr.reshape(-1), O, True)
+        want = E.rows_linear(*args(x, w, res))
+        X = E.N.rows_linear_ln(x.reshape(-1), M, K, K, gam, bet, 1e-5).out
+        t = X @ w.double().t()
+        b, r = bias.double(), res.double()
+        # the last 8-column chunk dropped (columns 256 of 257)
+        w_cut = w.clone()
+        w_cut[:, 256:] = 0
+        _rl_report("last chunk dropped", want, E.h16(E.gelu_erf(X @ w_cut.double().t() + b) + r))
+        _rl_report("bias after act", want, E.h16(E.gelu_erf(t) + b + r))
+        _rl_report("residual before act", want, E.h16(E.gelu_erf(t + b + r)))
+        good = E.gelu_erf(t + b) + r
+        _rl_report("lane m takes row m - 1", want, E.h16(torch.cat([good[:1], good[:-1]])))
+
+
+def test_batchnorm_fold_reading_against_float64():
+    g = torch.Generator().manual_seed(5)
+    cout, per = 16, 27
+    w, b, gamma, beta, mean = (torch.randn(n, generator=g).float() for n in (cout * per, cout, cout, cout, cout))
+    var = torch.rand(cout, generator=g).float()
+    rw, rb = E.batchnorm_fold(w, b, gamma, beta, mean, var, 1e-5, cout, per)
+    s = gamma.double() / (var.double() + float(torch.tensor(1e-5, dtype=torch.float32))).sqrt()
+    assert torch.equal(rw.out, (w.double().view(cout, per) * s[:, None]).float().double().reshape(-1))
+    assert (E.excess(rb, (beta.double() + (b.double() - mean.double()) * s).float().double()) <= 1).all()
+    rw0, rb0 = E.batchnorm_fold(w, None, gamma, beta, mean, var, 1e-5, cout, per)
+    assert torch.equal(rb0.exact, beta.double() - mean.double() * s)
