@@ -7,6 +7,7 @@ keys as generative/networks/nets/diffusion_model_unet.py (reference lines cited 
 * the up path never materialises ``torch.cat([h, skip])`` raw: GroupNorm and the 1x1 skip conv read both tensors;
 * attention runs as the flash-style wgmma kernel, as wgmma GEMMs (QK^T, PV with V^T from an operand-swapped projection) or, for tiny heads /
   a handful of context tokens, the CUDA-core online-softmax kernel.
+DiffusionModelEncoder, the reference's classifier built on the same down path, lives here as it does in the reference.
 Inference only (``torch.no_grad`` semantics); there is no CPU path.
 """
 from __future__ import annotations
@@ -18,10 +19,11 @@ import torch
 import torch.nn as nn
 
 from ... import ops
-from ...ops import ACT_SILU, CL
+from ...losses._common import forward_only
+from ...ops import ACT_RELU, ACT_SILU, CL
 from ..blocks.spade_norm import SPADE
-from .._holders import (Convolution, f32, on_input_device, packed_linear, packed_linear_geglu, packed_linear_stack,
-                        require_cuda)
+from .._holders import (Convolution, _Cached, f32, on_input_device, packed_linear, packed_linear_geglu,
+                        packed_linear_stack, require_cuda)
 
 __all__ = ["DiffusionModelUNet"]
 
@@ -50,15 +52,17 @@ def _context_cl(context: torch.Tensor) -> CL:
     return ops.to_cl(context.permute(0, 2, 1).unsqueeze(2).contiguous())
 
 
-def _few_rows_linear(x: CL, pl) -> torch.Tensor:
-    """Projection of a token matrix to packed rows [N, S, pitch].  A handful of tokens in total (the context of a
-    classifier-free-guidance step: one token per sample) goes through the GEMV kernel — a 128-row tensor-core tile
-    spends its pipeline latency on two rows, 14 of them per C5 UNet forward."""
+def _few_rows_linear(x: CL, pl, act: int = ops.ACT_NONE, out_f32: bool = False) -> torch.Tensor:
+    """act(projection) of a token matrix to packed rows [N, S, pitch] (h16, or fp32 with ``out_f32``).  A handful of
+    tokens in total (the context of a classifier-free-guidance step: one token per sample) goes through the GEMV
+    kernel — a 128-row tensor-core tile spends its pipeline latency on two rows, 14 of them per C5 UNet forward."""
     rows = x.N * x.spatial
     if rows <= 8 and x.C * rows * 2 <= 32 * 1024:
-        y = ops.rows_linear(x.t.reshape(rows, x.pitch), x.C, pl)
-        return y.reshape(x.N, x.spatial, y.shape[-1])
-    return _rows(ops.linear(x, pl))
+        y = ops.rows_linear(x.t.reshape(rows, x.pitch), x.C, pl, act=act, out_f32=out_f32)
+    else:
+        y = ops.linear(x, pl, act1=act, out_f32=out_f32)
+        y = y if out_f32 else y.t
+    return y.reshape(x.N, x.spatial, y.shape[-1])
 
 
 def _sdp(owner: nn.Module, xq: CL, xkv: CL, heads: int, dh: int, scale: float, residual: CL | None,
@@ -663,6 +667,23 @@ def time_embedding(module: nn.Module, x: torch.Tensor, timesteps: torch.Tensor,
     return emb
 
 
+def _down_path(module: nn.Module, x: torch.Tensor, timesteps: torch.Tensor, context: torch.Tensor | None,
+               class_labels: torch.Tensor | None) -> tuple[CL, list[CL], TimeEmb, CL | None]:
+    """Time (+ class) embedding, ``conv_in`` and the down blocks of the UNet (diffusion_model_unet.py:1887-1916) and
+    of DiffusionModelEncoder (2087-2111) -> (h, skip list, embedding, context rows)."""
+    require_cuda(x, module)
+    emb = project_time_embedding(module, time_embedding(module, x, timesteps, class_labels))
+    if context is not None and module.with_conditioning is False:
+        raise ValueError("model should have with_conditioning = True if context is provided")
+    ctx = _context_cl(context) if context is not None else None
+    h = module.conv_in(ops.to_cl(x))
+    down_block_res_samples: list[CL] = [h]
+    for downsample_block in module.down_blocks:
+        h, res_samples = downsample_block(hidden_states=h, temb=emb, context=ctx)
+        down_block_res_samples.extend(res_samples)
+    return h, down_block_res_samples, emb, ctx
+
+
 class DiffusionModelUNet(nn.Module):
     """diffusion_model_unet.py:1646-1943 — same constructor, same forward signature, same state_dict."""
 
@@ -769,16 +790,7 @@ class DiffusionModelUNet(nn.Module):
     @on_input_device
     def _forward(self, x, timesteps, context, class_labels, down_block_additional_residuals,
                  mid_block_additional_residual, seg):
-        require_cuda(x, self)
-        emb = project_time_embedding(self, time_embedding(self, x, timesteps, class_labels))
-        if context is not None and self.with_conditioning is False:
-            raise ValueError("model should have with_conditioning = True if context is provided")
-        ctx = _context_cl(context) if context is not None else None
-        h = self.conv_in(ops.to_cl(x))
-        down_block_res_samples: list[CL] = [h]
-        for downsample_block in self.down_blocks:
-            h, res_samples = downsample_block(hidden_states=h, temb=emb, context=ctx)
-            down_block_res_samples.extend(res_samples)
+        h, down_block_res_samples, emb, ctx = _down_path(self, x, timesteps, context, class_labels)
         if down_block_additional_residuals is not None:
             down_block_res_samples = [
                 ops.axpy(s, r if isinstance(r, CL) else ops.to_cl(r), 1.0)
@@ -796,4 +808,97 @@ class DiffusionModelUNet(nn.Module):
         h = ops.groupnorm(h, norm.num_groups, norm.eps, norm.weight, norm.bias, act=ACT_SILU)
         y = self.out[2](h, out_f32=True)
         out = ops.from_cl_f32(y, self.out_channels, self.spatial_dims)
+        return out if x.dtype == torch.float32 else out.to(x.dtype)
+
+
+class DiffusionModelEncoder(nn.Module, _Cached):
+    """diffusion_model_unet.py:1946-2115 — the classifier of Wolleb et al. 2022 ("Diffusion Models for Medical Anomaly
+    Detection"): the UNet's time embedding and down path followed by ``out = Sequential(Linear(4096, 512), ReLU,
+    Dropout(0.1), Linear(512, out_channels))`` on the flattened last feature map.  Same constructor, attributes and
+    ``state_dict`` as the reference, including its quirks: every level downsamples, the last one too
+    (``is_final_block`` compares ``i`` with ``len(num_channels)``); there is no middle block; the head takes exactly
+    4096 features; an integer ``num_res_blocks`` is not expanded (the reference indexes it and raises ``TypeError``).
+
+    Inference only, like every network here: ``forward`` computes no gradients, and a call with grad enabled on an
+    ``x`` that requires grad raises ``RuntimeError`` (classifier guidance needs d logits / d x, which this library does
+    not compute).  Dropout is never applied, so train mode computes what eval mode does.  CPU tensors raise.
+
+    ``forward`` returns fp32 logits ``[N, out_channels]`` cast to ``x.dtype``.  The head reads the channels-last
+    feature map directly: the first Linear's weight columns are permuted once, when packed, from the reference's
+    channels-first flattening; Linear + bias + ReLU and Linear + bias run as GEMV (a few samples) or GEMM launches."""
+
+    def __init__(self, spatial_dims: int, in_channels: int, out_channels: int,
+                 num_res_blocks: Sequence[int] | int = (2, 2, 2, 2), num_channels: Sequence[int] = (32, 64, 64, 64),
+                 attention_levels: Sequence[bool] = (False, False, True, True), norm_num_groups: int = 32,
+                 norm_eps: float = 1e-6, resblock_updown: bool = False, num_head_channels: int | Sequence[int] = 8,
+                 with_conditioning: bool = False, transformer_num_layers: int = 1,
+                 cross_attention_dim: int | None = None, num_class_embeds: int | None = None,
+                 upcast_attention: bool = False) -> None:
+        super().__init__()
+        if with_conditioning is True and cross_attention_dim is None:
+            raise ValueError("DiffusionModelEncoder expects dimension of the cross-attention conditioning "
+                             "(cross_attention_dim) when using with_conditioning.")
+        if cross_attention_dim is not None and with_conditioning is False:
+            raise ValueError("DiffusionModelEncoder expects with_conditioning=True when specifying the "
+                             "cross_attention_dim.")
+        if any((out_channel % norm_num_groups) != 0 for out_channel in num_channels):
+            raise ValueError("DiffusionModelEncoder expects all num_channels being multiple of norm_num_groups")
+        if len(num_channels) != len(attention_levels):
+            raise ValueError("DiffusionModelEncoder expects num_channels being same size of attention_levels")
+        if isinstance(num_head_channels, int):
+            num_head_channels = ensure_tuple_rep(num_head_channels, len(attention_levels))
+        if len(num_head_channels) != len(attention_levels):
+            raise ValueError("num_head_channels should have the same length as attention_levels. For the i levels "
+                             "without attention, i.e. `attention_level[i]=False`, the num_head_channels[i] will be "
+                             "ignored.")
+        self.in_channels = in_channels
+        self.block_out_channels = num_channels
+        self.out_channels = out_channels
+        self.num_res_blocks = num_res_blocks
+        self.attention_levels = attention_levels
+        self.num_head_channels = num_head_channels
+        self.with_conditioning = with_conditioning
+
+        self.conv_in = Convolution(spatial_dims, in_channels, num_channels[0], strides=1, kernel_size=3, padding=1)
+        time_embed_dim = num_channels[0] * 4
+        self.time_embed = nn.Sequential(nn.Linear(num_channels[0], time_embed_dim), nn.SiLU(),
+                                        nn.Linear(time_embed_dim, time_embed_dim))
+        self.num_class_embeds = num_class_embeds
+        if num_class_embeds is not None:
+            self.class_embedding = nn.Embedding(num_class_embeds, time_embed_dim)
+
+        self.down_blocks = nn.ModuleList([])
+        output_channel = num_channels[0]
+        for i in range(len(num_channels)):
+            input_channel = output_channel
+            output_channel = num_channels[i]
+            is_final_block = i == len(num_channels)      # never true: the reference downsamples at every level
+            self.down_blocks.append(get_down_block(
+                spatial_dims, input_channel, output_channel, time_embed_dim, num_res_blocks[i], norm_num_groups,
+                norm_eps, not is_final_block, resblock_updown, attention_levels[i] and not with_conditioning,
+                attention_levels[i] and with_conditioning, num_head_channels[i], transformer_num_layers,
+                cross_attention_dim, upcast_attention))
+
+        self.out = nn.Sequential(nn.Linear(4096, 512), nn.ReLU(), nn.Dropout(0.1), nn.Linear(512, self.out_channels))
+
+    def forward(self, x: torch.Tensor, timesteps: torch.Tensor, context: torch.Tensor | None = None,
+                class_labels: torch.Tensor | None = None) -> torch.Tensor:
+        forward_only(type(self).__name__, x)
+        with torch.no_grad():
+            return self._forward(x, timesteps, context, class_labels)
+
+    @on_input_device
+    def _forward(self, x, timesteps, context, class_labels):
+        h, _, _, _ = _down_path(self, x, timesteps, context, class_labels)
+        fc1, fc2 = self.out[0], self.out[3]
+        S = h.spatial
+        if S * h.C != fc1.in_features:
+            raise RuntimeError(f"mat1 and mat2 shapes cannot be multiplied ({h.N}x{S * h.C} and "
+                               f"{fc1.in_features}x{fc1.out_features})")
+        pl1 = self._cached(("out.0", h.C, h.pitch, S), (fc1.weight, fc1.bias),
+                           lambda: ops.PackedLinear.channels_first_input(fc1.weight, fc1.bias, h.C, h.pitch, S))
+        pl2 = self._cached(("out.3",), (fc2.weight, fc2.bias), lambda: ops.PackedLinear(fc2.weight, fc2.bias))
+        hidden = _few_rows_linear(ops.as_rows(h.t.reshape(h.N, S * h.pitch), S * h.pitch), pl1, act=ACT_RELU)
+        logits = _few_rows_linear(ops.as_rows(hidden.reshape(h.N, -1), fc1.out_features), pl2, out_f32=True)
+        out = logits.reshape(h.N, -1)[:, :self.out_channels].contiguous()
         return out if x.dtype == torch.float32 else out.to(x.dtype)

@@ -124,13 +124,8 @@ class SPADEEncoder(nn.Module, _Cached):
         """``name`` with its input columns moved from channels-first (c * S + s) to channels-last (s * pitch + c)
         order; the columns of pad channels are zero."""
         lin = getattr(self, name)
-
-        def build():
-            w = ops._src_f32(lin.weight)
-            wp = torch.zeros((w.shape[0], S, pitch), dtype=torch.float32, device=w.device)
-            wp[:, :, :C_] = w.view(w.shape[0], C_, S).transpose(1, 2)
-            return ops.PackedLinear(wp.view(w.shape[0], S * pitch), lin.bias)
-        return self._cached((name, C_, pitch, S), (lin.weight, lin.bias), build)
+        return self._cached((name, C_, pitch, S), (lin.weight, lin.bias),
+                            lambda: ops.PackedLinear.channels_first_input(lin.weight, lin.bias, C_, pitch, S))
 
     def _features(self, x: torch.Tensor) -> CL:
         h = ops.to_cl(x)

@@ -306,6 +306,17 @@ class PackedLinear:
         return self
 
     @classmethod
+    def channels_first_input(cls, weight: torch.Tensor, bias: torch.Tensor | None, C_: int, pitch: int,
+                             S: int) -> "PackedLinear":
+        """An nn.Linear over the channels-first flattening of a [C_, S] feature map (column c * S + s) with its input
+        columns moved to the channels-last order s * pitch + c, so it reads the rows of a CL (``[N, S * pitch]``)
+        directly; the columns of pad channels are zero."""
+        w = _src_f32(weight)
+        wp = torch.zeros((w.shape[0], S, pitch), dtype=torch.float32, device=w.device)
+        wp[:, :, :C_] = w.view(w.shape[0], C_, S).transpose(1, 2)
+        return cls(wp.view(w.shape[0], S * pitch), bias)
+
+    @classmethod
     def from_packed(cls, w16: torch.Tensor, cout: int, K: int, bias: torch.Tensor | None) -> "PackedLinear":
         self = cls.__new__(cls)
         self.cout, self.K, self.w = cout, K, w16
