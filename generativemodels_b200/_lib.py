@@ -116,6 +116,12 @@ class PndmCoef(C.Structure):
                 ("v_alpha", C.c_float), ("v_beta", C.c_float), ("prediction_type", C.c_int32)]
 
 
+class DpmCoef(C.Structure):
+    _fields_ = [("alpha_s", C.c_float), ("sigma_s", C.c_float), ("c_x", C.c_float), ("w", C.c_float * 3),
+                ("c_z", C.c_float), ("clip_min", C.c_float), ("clip_max", C.c_float),
+                ("prediction_type", C.c_int32), ("clip", C.c_int32)]
+
+
 class RepackBlock(C.Structure):
     _fields_ = [("col0", C.c_int32), ("cin0", C.c_int32), ("cs", C.c_int32), ("ntaps", C.c_int32),
                 ("tap", C.c_int16 * 8)]
@@ -235,6 +241,11 @@ LOSS_SIGNATURES = {
     "b200_spectral_distance": [_P, _I32, _P, _F, _I32, _P, _P, _P, _P],
     "b200_adversarial": [_P, _P, _P, _P, _I32, _I32, _I32, _I32, _P, _P, _P, _P, _P],
 }
+# the multistep sampler's entry point; mirrors include/b200gen_samplers.h exactly
+SAMPLER_SIGNATURES = {
+    "b200_dpm_solver_step": [_P, _P, C.POINTER(_P), _I32, _P, C.POINTER(DpmCoef), _P, _P, _I64, _P],
+}
+DPM_MAX_HIST = 2
 FFT_MAX_N, SPECTRAL_PARTIALS, ADV_MAX_OUTPUTS, ADV_PARTIALS = 4096, 1024, 8, 2048
 REDUCTION_NONE, REDUCTION_MEAN, REDUCTION_SUM = 0, 1, 2
 ADV_BCE, ADV_HINGE, ADV_LEAST_SQUARES, ADV_LEAST_SQUARES_RAW = 0, 1, 2, 3
@@ -258,13 +269,13 @@ def load():
             "(generativemodels_b200/csrc/build.sh). There is no fallback path.")
     lib = C.CDLL(str(LIB_PATH))
     for name, argtypes in {**SIGNATURES, **METRIC_SIGNATURES, **FID_SIGNATURES, **PERCEPTUAL_SIGNATURES,
-                            **LOSS_SIGNATURES}.items():
+                            **LOSS_SIGNATURES, **SAMPLER_SIGNATURES}.items():
         fn = getattr(lib, name)  # AttributeError if the .so does not export it
         fn.argtypes = argtypes
         fn.restype = _RESTYPES.get(name, C.c_int)
     for which, struct in enumerate((IgemmParams, GnStatsParams, GnApplyParams, DdimCoef, DdpmCoef, PndmCoef, IgemmSeg,
                                     FlashParams, KlCoef, RepackBlock, SsimParams, SsimCombineParams,
-                                    FidMomentsParams, FrechetParams)):
+                                    FidMomentsParams, FrechetParams, DpmCoef)):
         c_size = lib.b200_abi_sizeof(which)
         if c_size != C.sizeof(struct):
             raise B200Error(f"ABI mismatch: {struct.__name__} is {C.sizeof(struct)} bytes in Python but {c_size} in "

@@ -2,6 +2,7 @@
 #include "common.cuh"
 #include "../../include/b200gen_metrics.h"
 #include "../../include/b200gen_fid.h"
+#include "../../include/b200gen_samplers.h"
 
 namespace b200 {
 
@@ -75,6 +76,7 @@ extern "C" int b200_abi_sizeof(int which) {
     case 11: return (int)sizeof(b200_ssim_combine_params);
     case 12: return (int)sizeof(b200_fid_moments_params);
     case 13: return (int)sizeof(b200_frechet_params);
+    case 14: return (int)sizeof(b200_dpm_coef);
     default: return -1;
   }
 }

@@ -1,0 +1,102 @@
+// The DPM-Solver++ multistep step (DPMSolverMultistepScheduler.step): x0 from the model output, optional clip, then
+// the update as one weighted sum of the sample, x0, up to two earlier x0 estimates and the noise.  The host folds the
+// solver's formulas into those weights; the kernel only streams memory.  Contract: include/b200gen_samplers.h.
+#include "common.cuh"
+#include "../../include/b200gen_samplers.h"
+
+namespace b200 {
+namespace {
+
+__device__ __forceinline__ void dpm_one(const b200_dpm_coef& c, float m, float s, float h0, float h1, float z, int nh,
+                                        bool has_noise, float& p, float& x0) {
+  if (c.prediction_type == B200_PRED_EPSILON) x0 = fmaf(-c.sigma_s, m, s) / c.alpha_s;
+  else if (c.prediction_type == B200_PRED_V) x0 = fmaf(c.alpha_s, s, -c.sigma_s * m);
+  else x0 = m;
+  if (c.clip) x0 = fminf(fmaxf(x0, c.clip_min), c.clip_max);
+  p = c.c_x * s;
+  p = fmaf(c.w[0], x0, p);
+  if (nh > 0) p = fmaf(c.w[1], h0, p);
+  if (nh > 1) p = fmaf(c.w[2], h1, p);
+  if (has_noise) p = fmaf(c.c_z, z, p);
+}
+
+__device__ __forceinline__ float4 ld4(const float* p, long long i) {
+  return __ldg(reinterpret_cast<const float4*>(p) + i);
+}
+
+// Up to 7 fp32 streams per element: pure HBM streaming, so 128-bit accesses when every pointer is 16-byte aligned
+// (VEC = 1) and a scalar tail for n % 4; VEC = 0 is the scalar path for any alignment.  NH = number of history tensors.
+template <int VEC, int NH>
+__global__ void __launch_bounds__(256) dpm_step_kernel(const float* __restrict__ m_in, const float* __restrict__ x,
+                                                       const float* __restrict__ h0, const float* __restrict__ h1,
+                                                       const float* __restrict__ noise, b200_dpm_coef c,
+                                                       float* __restrict__ prev, float* __restrict__ x0_out,
+                                                       long long n) {
+  const long long tid = (long long)blockIdx.x * blockDim.x + threadIdx.x, nthr = (long long)gridDim.x * blockDim.x;
+  const bool has_noise = noise != nullptr;
+  long long done = 0;
+  if (VEC) {
+    const long long nv = n >> 2;
+    const float4 zero = make_float4(0.f, 0.f, 0.f, 0.f);
+    for (long long i = tid; i < nv; i += nthr) {
+      const float4 m = ld4(m_in, i), s = ld4(x, i);
+      const float4 a = NH > 0 ? ld4(h0, i) : zero, b = NH > 1 ? ld4(h1, i) : zero;
+      const float4 z = has_noise ? ld4(noise, i) : zero;
+      float4 p, o;
+      dpm_one(c, m.x, s.x, a.x, b.x, z.x, NH, has_noise, p.x, o.x);
+      dpm_one(c, m.y, s.y, a.y, b.y, z.y, NH, has_noise, p.y, o.y);
+      dpm_one(c, m.z, s.z, a.z, b.z, z.z, NH, has_noise, p.z, o.z);
+      dpm_one(c, m.w, s.w, a.w, b.w, z.w, NH, has_noise, p.w, o.w);
+      reinterpret_cast<float4*>(prev)[i] = p;
+      reinterpret_cast<float4*>(x0_out)[i] = o;
+    }
+    done = nv << 2;
+  }
+  for (long long i = done + tid; i < n; i += nthr) {
+    float p, o;
+    dpm_one(c, m_in[i], x[i], NH > 0 ? h0[i] : 0.f, NH > 1 ? h1[i] : 0.f, has_noise ? noise[i] : 0.f, NH, has_noise,
+            p, o);
+    prev[i] = p;
+    x0_out[i] = o;
+  }
+}
+
+unsigned grid_for(long long work) {
+  long long b = (work + 255) / 256;
+  const long long cap = 16ll * sm_count();
+  return (unsigned)(b < 1 ? 1 : (b > cap ? cap : b));
+}
+
+template <int VEC>
+cudaError_t launch(int nh, const float* m, const float* s, const float* h0, const float* h1, const float* z,
+                   const b200_dpm_coef& c, float* prev, float* x0, long long n, cudaStream_t stream) {
+  const unsigned grid = grid_for(VEC ? (n + 3) / 4 : n);
+  if (nh == 0) return launch_kernel(dpm_step_kernel<VEC, 0>, grid, 256, 0, stream, m, s, h0, h1, z, c, prev, x0, n);
+  if (nh == 1) return launch_kernel(dpm_step_kernel<VEC, 1>, grid, 256, 0, stream, m, s, h0, h1, z, c, prev, x0, n);
+  return launch_kernel(dpm_step_kernel<VEC, 2>, grid, 256, 0, stream, m, s, h0, h1, z, c, prev, x0, n);
+}
+
+}  // namespace
+}  // namespace b200
+
+extern "C" int b200_dpm_solver_step(const float* model_out, const float* sample, const float* const* hist,
+                                    int32_t n_hist, const float* noise, const b200_dpm_coef* c, float* prev_sample,
+                                    float* pred_x0, int64_t n, void* stream_v) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
+  B200_CHECK_ARG(model_out && sample && c && prev_sample && pred_x0 && n >= 1, "dpm_solver_step: bad arguments");
+  B200_CHECK_ARG(n_hist >= 0 && n_hist <= B200_DPM_MAX_HIST && (n_hist == 0 || hist),
+                 "dpm_solver_step: n_hist must be 0..%d with a history array", B200_DPM_MAX_HIST);
+  B200_CHECK_ARG(c->prediction_type == B200_PRED_EPSILON || c->prediction_type == B200_PRED_SAMPLE ||
+                 c->prediction_type == B200_PRED_V, "dpm_solver_step: unknown prediction_type %d", c->prediction_type);
+  const float* h[2] = {nullptr, nullptr};
+  for (int k = 0; k < n_hist; ++k) {
+    h[k] = hist[k];
+    B200_CHECK_ARG(h[k], "dpm_solver_step: null history tensor %d", k);
+  }
+  const bool vec = (((uintptr_t)model_out | (uintptr_t)sample | (uintptr_t)h[0] | (uintptr_t)h[1] | (uintptr_t)noise |
+                     (uintptr_t)prev_sample | (uintptr_t)pred_x0) & 15) == 0;
+  if (vec) B200_CUDA(b200::launch<1>(n_hist, model_out, sample, h[0], h[1], noise, *c, prev_sample, pred_x0, n, stream));
+  else B200_CUDA(b200::launch<0>(n_hist, model_out, sample, h[0], h[1], noise, *c, prev_sample, pred_x0, n, stream));
+  B200_LAUNCH_CHECK("dpm_step_kernel");
+  return B200_OK;
+}
