@@ -12,8 +12,8 @@ class SamplersFakeLib(cpu_backend.FakeLib):
     def b200_dpm_solver_step(self, m, s, hist, n_hist, nz, c, prev, x0o, n, stream):
         assert 0 <= n_hist <= _lib.DPM_MAX_HIST and prev and x0o
         rp, rx = E.abi_step(f32(m, n), f32(s, n), [f32(hist[k], n) for k in range(n_hist)], f32(nz, n), _obj(c), n)
-        store32(prev, rp.out)
-        store32(x0o, rx.out)
+        store32(prev, rp)
+        store32(x0o, rx)
         return 0
 
 

@@ -52,9 +52,6 @@ from tests import igemm_emulator
 
 pytestmark = pytest.mark.gpu
 
-C_LIP = 1.5
-ACC = 2.0 ** -16
-REL = 2.0 ** -17
 FP16 = ops.H16 is torch.float16
 SENT16, SENT32 = 0x7FFF, 0x7FFFFFFF          # NaN in fp16, bf16 and fp32: "never written"
 
@@ -331,43 +328,9 @@ def emulate(c: Case, g: Geom, t):
     return t
 
 
-def gemm_only(c: Case, g: Geom, t, with_bias=False):
-    """The emulator's fp32 [N, OD, OH, OW, GEMM columns] of the case with no epilogue: on |A| and |W| (mag), or on
-    the operands themselves plus the bias (the GEGLU inputs a and gate)."""
-    ncols = c.cout if c.act1 == ACT_GEGLU else c.cols
-    m = replace(c, out_cols=ncols, out_f32=True, out_pad=0, out_off=0, res=None, stat=False, gn=0, act1=ACT_NONE,
-                act2=ACT_NONE, scale=1.0, rowvec=None, row_bias=False, bias=with_bias)
-    gm = Geom(m, 1)
-    tm = {k: (v if with_bias else v.abs()) for k, v in t.items() if k.startswith("a") or k == "w"}
-    if with_bias:
-        tm["bias"] = t["bias"]
-    tm["out"] = torch.full((gm.out_len,), SENT32, dtype=torch.int32).view(torch.float32)
-    igemm_emulator.emulate(fill(m, gm, host_ptrs(tm)))
-    return tm["out"].numpy()[gm.footprint(m)].astype(np.float64)
-
-
-def ulp16(x):
-    mant, emin = (10, -14) if FP16 else (7, -126)
-    m = np.maximum(np.abs(x), 2.0 ** emin)
-    return np.exp2(np.floor(np.log2(m)) - mant)
-
-
 def bound(c: Case, g: Geom, t, got, want):
-    mag = gemm_only(c, g, t)
-    if c.act1 == ACT_GEGLU:
-        # out[j] = a * gelu(gate) with a, gate the [32 a | 32 gate] column groups of the GEMM (+ bias)
-        pre = gemm_only(c, g, t, with_bias=True)
-        sel = lambda x, off: x.reshape(*x.shape[:-1], -1, 2, 32)[..., off, :].reshape(*x.shape[:-1], -1)
-        a, gate, ea, eg = sel(pre, 0), sel(pre, 1), ACC * sel(mag, 0), ACC * sel(mag, 1)
-        from scipy.special import erf
-        gelu = 0.5 * gate * (1 + erf(gate / 2 ** 0.5))
-        acc_err = np.abs(gelu) * ea + (np.abs(a) + ea) * 1.2 * eg
-    else:
-        acc_err = abs(c.scale) * ACC * mag
-    tol = C_LIP * acc_err + REL * (np.abs(want) + 1)
-    if not c.out_f32:
-        tol = tol + ulp16(np.maximum(np.abs(got), np.abs(want)))
-    return tol
+    """igemm_emulator.bound on the case's struct over the CPU operands."""
+    return igemm_emulator.bound(fill(c, g, host_ptrs(t)), got, want, scale=c.scale)
 
 
 # ------------------------------------------------------------------------------------------------------------------
