@@ -1,6 +1,7 @@
-"""Shadow calls: every C-ABI call a network makes runs on the real library AND on the CPU stand-in
-(tests/cpu_backend.FakeLib, tests/samplers_backend.SamplersFakeLib) with the call's own inputs, and the two are
-compared under the bound of the entry point's family.  Test infrastructure only.
+"""Shadow calls: every C-ABI call a network, metric or loss makes runs on the real library AND on the CPU stand-in
+(StandIn below: tests/losses_backend.LossesFakeLib, which carries the metric, FID and perceptual entry points, and
+tests/samplers_backend.SamplersFakeLib) with the call's own inputs, and the two are compared under the bound of the
+entry point's family.  Test infrastructure only.
 
     with abi_shadow.shadow(monkeypatch) as sh:
         model(x)
@@ -19,14 +20,19 @@ For each b200_* call the proxy installed in place of _lib.require_device()
      cloned struct or array (the caller's struct is never touched: ops caches parameter templates);
   5. compares every region the stand-in stored (cpu_backend.RECORDER reports the view and the emulator's Result)
      with the device's bytes under the family's rule: elementwise / norm / attention excess <= 1, copies (resampling,
-     weight repacking, VQ indices) bit for bit, GroupNorm affine tables by affine_excess; b200_igemm under
+     weight repacking, VQ indices, the perceptual input preparation) bit for bit, GroupNorm affine tables by
+     affine_excess; the metric and loss outputs under the bounds of tests/{metrics,fid,perceptual,losses}_emulator.py
+     (fp32 and fp64 values per element, the FFT's spectra norm-wise per (side, image)); b200_ssim's partial slots
+     summed per item, against the float64 sums of the kernel's own maps when it stores them and against the reading's
+     sums within the sum of its per-voxel bounds always; b200_igemm under
      igemm_emulator.bound on its footprint (calls of more than 8192 output voxels per sample on the deterministic
      subset igemm_emulator.sample_voxels; the footprint, padding and partial-sum checks below see every voxel),
      padding columns +0, GroupNorm partials summed over slots against the
      float64 sums of the kernel's own stored output and softmax partials against the kernel's own fp32 rows, as
      tests/test_igemm_contract_gpu.py does;
   6. checks the footprint: every other byte of every touched segment is bit-identical before and after the call,
-     except the declared scratch (split-K split_ws, the flash workspace, the GroupNorm statistics workspace).
+     except the declared scratch (split-K split_ws, the flash workspace, the GroupNorm statistics workspace, the MMD,
+     Frechet, spectral-distance and adversarial workspaces).
 
 Each call is logged with a compact argument signature, its worst excess and, for b200_igemm, the planner's column
 tile and split factor and the store path (the predicates of tests/test_igemm_contract_gpu.py's docstring), so that a
@@ -49,16 +55,33 @@ from tests import attention_emulator as A
 from tests import cpu_backend
 from tests import elementwise_emulator as W
 from tests import igemm_emulator as E
+from tests import losses_backend
+from tests import losses_emulator as LE
+from tests import metrics_emulator as ME
 from tests import norm_emulator as N
 from tests import samplers_backend
 
 PASSTHROUGH = {"b200_sm_count", "b200_igemm_split_workspace_bytes", "b200_attention_flash_workspace_bytes",
                "b200_groupnorm_workspace_bytes", "b200_igemm_plan", "b200_version", "b200_act_dtype",
-               "b200_device_check", "b200_last_error_string", "b200_abi_sizeof"}
-ARGTYPES = {**_lib.SIGNATURES, **_lib.SAMPLER_SIGNATURES}
+               "b200_device_check", "b200_last_error_string", "b200_abi_sizeof", "b200_ssim_workspace_bytes",
+               "b200_mmd_workspace_bytes", "b200_frechet_workspace_bytes"}
+ARGTYPES = {**_lib.SIGNATURES, **_lib.METRIC_SIGNATURES, **_lib.FID_SIGNATURES, **_lib.PERCEPTUAL_SIGNATURES,
+            **_lib.LOSS_SIGNATURES, **_lib.SAMPLER_SIGNATURES}
 GN_PARTIAL_REL = 2e-4          # GroupNorm partial sums vs the kernel's own output (test_igemm_contract_gpu.py)
 SOFTMAX_SUM_REL = 1e-5         # softmax partial sums vs the kernel's own rows (test_igemm_contract_gpu.py)
 _SIGNED = {1: torch.int8, 2: torch.int16, 4: torch.int32, 8: torch.int64}
+
+
+class StandIn(losses_backend.LossesFakeLib, samplers_backend.SamplersFakeLib):
+    """The CPU stand-in of every entry point: the network, metric, FID, perceptual and loss stand-ins, and the
+    sampler's."""
+
+
+def _excess(got, want, tol):
+    """|got - want| / tol elementwise (torch, float64); equal values (NaN included) are 0, other non-finite ones inf."""
+    same = (got == want) | (torch.isnan(got) & torch.isnan(want))
+    ratio = ((got - want).abs() / tol).nan_to_num(math.inf, math.inf)
+    return torch.where(same, torch.zeros_like(ratio), ratio)
 
 
 # ----------------------------------------------------------------------------------------------------------------
@@ -267,7 +290,7 @@ class Call:
 class Shadow:
     real: object
     memory: object
-    stand_in: object = field(default_factory=samplers_backend.SamplersFakeLib)
+    stand_in: object = field(default_factory=StandIn)
     calls: list = field(default_factory=list)
     violations: list = field(default_factory=list)
 
@@ -337,6 +360,7 @@ class _Compare:
         self.worst = 0.0
         self.paths = []
         self.voxels = None
+        self.slot_sums = None
         self.mask = {b: torch.zeros(s, dtype=torch.bool) for b, s in segs.items()}
         self.host = {b: t.data_ptr() for b, t in emu.items()}
         self.pre_host = {b: t.data_ptr() for b, t in pre.items()}
@@ -409,8 +433,13 @@ class _Compare:
         for view, r in records:
             self.mark_view(view)
             got = self.device_view(view)
+            if isinstance(r, ME.SlotSums):         # compared summed per item, in entry_specific
+                self.slot_sums = r
+                continue
             if isinstance(r, N.Affine):
                 ex = N.affine_excess(r, got)
+            elif isinstance(r, LE.Spectra):
+                ex = LE.norm_excess(r, got.reshape(r.out.shape))
             else:
                 got = got.reshape(r.out.shape)
                 fam = W if isinstance(r, W.Result) else N if isinstance(r, N.Result) else A
@@ -436,6 +465,21 @@ class _Compare:
             self.paths.append(f"flash dh{a.dh}")
             if a.workspace:
                 self.mark(a.workspace, a.workspace_bytes)
+        elif self.name == "b200_ssim":
+            self.ssim_slots(o[0])
+        elif self.name == "b200_mmd":
+            self.mark(o[7], int(self.sh.real.b200_mmd_workspace_bytes(o[6])))
+        elif self.name == "b200_frechet":
+            self.mark(o[0].workspace, int(self.sh.real.b200_frechet_workspace_bytes(o[0].F)))
+        elif self.name == "b200_spectral_distance":
+            if o[6]:
+                self.mark(o[6], _lib.SPECTRAL_PARTIALS * 8)
+        elif self.name == "b200_adversarial":
+            self.mark(o[9], _lib.ADV_PARTIALS * 8)
+        elif self.name == "b200_perceptual_distance" and o[9]:
+            image, image32 = (self.f64_at(o[8], o[3]), self.post_at(o[9], o[3], torch.float32))
+            if not torch.equal(image.float().view(torch.int32), image32.view(torch.int32)):
+                self.note(math.inf, "image32 is not the fp32 rounding of the kernel's own image")
         elif self.name in ("b200_groupnorm_stats", "b200_groupnorm_fused", "b200_groupnorm_from_partials_ex"):
             p = o[0]
             if p.partial:
@@ -445,6 +489,32 @@ class _Compare:
                 for i in range(2):
                     if o[1][i]:
                         self.paths.append(f"gn_from_partials gw{(o[3][i] or 8) if o[3] is not None else 8}")
+
+    def post_at(self, ptr, count, dtype):
+        b = self.seg_of(ptr)
+        es = torch.empty((), dtype=dtype).element_size()
+        assert (ptr - b) % es == 0
+        return self.post[b].view(dtype)[(ptr - b) // es:(ptr - b) // es + count]
+
+    def f64_at(self, ptr, count):
+        return self.post_at(ptr, count, torch.float64)
+
+    def ssim_slots(self, p):
+        """The partial slots of b200_ssim, whose layout is the device's own: per item, the sum over its slots against
+        the float64 sum of the kernel's own stored maps (within fp64 summation error) and against the reading's sum
+        (within the sum of the per-voxel bounds, metrics_emulator.slot_sums)."""
+        nbytes = int(self.sh.real.b200_ssim_workspace_bytes(C.byref(p)))
+        slots = nbytes // (16 * p.N)
+        self.mark(p.partials, nbytes)
+        dev = self.f64_at(p.partials, p.N * slots * 2).view(p.N, slots, 2).sum(1)
+        r = self.slot_sums
+        self.note(_excess(dev, r.exact, r.err).max(), "SSIM partial slots vs the reading's sums")
+        count = p.C * (p.D - p.kd + 1) * (p.H - p.kh + 1) * (p.W - p.kw + 1)
+        for k, ptr in enumerate((p.ssim_map, p.cs_map)):
+            if ptr:
+                own = self.post_at(ptr, p.N * count, torch.float32).double().view(p.N, count)
+                tol = (count + slots + 2) * ME.E53 * own.abs().sum(1)
+                self.note(_excess(dev[:, k], own.sum(1), tol).max(), "SSIM partial slots vs the kernel's own map")
 
     def igemm(self, p):
         nsm = int(self.sh.real.b200_sm_count())

@@ -10,7 +10,8 @@ bound reads:
          add): the bound is zero and the GPU test compares bits.  16-bit stores are fp32 -> 16-bit RN; fp16
          saturates at +-65504 (cvt.rn.satfinite), which is part of the rounding.
   h16    |got - out| <= ulp16(max(|got|, |out|)) + err;
-  f32    |got - out| <= ulp32(max(|got|, |out|)) + err.
+  f32    |got - out| <= ulp32(max(|got|, |out|)) + err;
+  f64    |got - out| <= ulp64(max(|got|, |out|)) + err (the double outputs of the metric and loss entry points).
 
 err collects the fp32 terms of each kernel's arithmetic, with u = 2^-24 the unit roundoff of fp32:
 
@@ -55,16 +56,21 @@ def ulp32(x):
     return torch.exp2(torch.floor(torch.log2(m)) - 23)
 
 
+def ulp64(x):
+    m = x.abs().clamp_min(2.0 ** -1022)
+    return torch.exp2(torch.floor(torch.log2(m)) - 52)
+
+
 @dataclass
 class Result:
     exact: torch.Tensor
     out: torch.Tensor
     err: torch.Tensor
-    kind: str                      # "copy", "h16" or "f32"
+    kind: str                      # "copy", "h16", "f32" or "f64"
 
 
 def _res(exact, err, kind):
-    out = exact if kind == "copy" else (h16(exact) if kind == "h16" else f32(exact))
+    out = exact if kind in ("copy", "f64") else (h16(exact) if kind == "h16" else f32(exact))
     return Result(exact, out, err, kind)
 
 
@@ -75,7 +81,7 @@ def copy(out):
 def tolerance(r: Result, got):
     if r.kind == "copy":
         return r.err
-    ulp = ulp16 if r.kind == "h16" else ulp32
+    ulp = {"h16": ulp16, "f32": ulp32, "f64": ulp64}[r.kind]
     return ulp(torch.maximum(got.abs(), r.out.abs())) + r.err
 
 

@@ -1,11 +1,24 @@
 """Float64 reading of the FID entry points of include/b200gen_fid.h (b200_fid_moments, b200_frechet), the contract the
 GPU tests hold the kernels to and the CPU stand-in (tests/fid_backend.py) computes with.  Inputs are converted to fp64
 exactly, as the kernels load them; the factor follows the header's pivot and stop rule, the eigenvalues come from
-numpy's eigvalsh and the header's cutoff drops the rounding-level ones."""
+numpy's eigvalsh and the header's cutoff drops the rounding-level ones.
+
+Bounds (e = 2^-53, the fp64 unit roundoff), which the f64 tolerance adds one ulp to:
+  mu (``moments_bound``): n values summed in fp64 in any order, then one division: (n + 2) e sum |x| / n.
+  sigma: each centred value c = x - mu' (mu' the device's mean) rounds once, the Gram's n fp64 fmas round once each,
+  and the scaling by fp64(1 / (n - 1)) twice: (n + 4) e sum_k |c_ki c_kj| / (n - 1).  The device's mean error
+  d = mu' - mu enters as d_j sum_k c_ki + d_i sum_k c_kj + n d_i d_j; the exact centred columns sum to 0, so only
+  n d_i d_j / (n - 1) is left, with |d| bounded as above.
+  b200_frechet (``frechet_bounds``): the distance within 1e-8 S, S = tr Sigma_x + tr Sigma_y + |mu_x - mu_y|^2 (the
+  scale of every term; tests/test_fid_gpu.py holds its sweep to the same bound), the eigenvalues within
+  max(F, 4) 2^-52 max(mu_max, 0) (the backward error of the factor, the two GEMMs and the bisection, relative to the
+  largest eigenvalue; at least the few roundings that form a 1 x 1 or 2 x 2 M) and the rank exactly.
+"""
 import numpy as np
 import torch
 
 F64 = torch.float64
+E53 = 2.0 ** -53
 
 
 def fid_moments(x):
@@ -14,6 +27,25 @@ def fid_moments(x):
     mu = x.mean(0)
     c = x - mu
     return mu, c.T @ c / (x.shape[0] - 1)
+
+
+def moments_bound(x):
+    """(mu_err [F], sigma_err [F, F]) of ``moments_bound`` in the module docstring, for a 2-D [n, F] view."""
+    x = x.to(F64)
+    n = x.shape[0]
+    ax = x.abs()
+    mu_err = (n + 2) * E53 * ax.sum(0) / n
+    c = (x - x.mean(0)).abs()
+    return mu_err, ((n + 4) * E53 * (c.T @ c) + n * torch.outer(mu_err, mu_err)) / (n - 1)
+
+
+def frechet_bounds(mu_x, sx, mu_y, sy, eig):
+    """(distance bound, eigenvalue bound) of ``frechet_bounds`` in the module docstring, float64."""
+    mu_x, sx, mu_y, sy = (np.asarray(t, dtype=np.float64) for t in (mu_x, sx, mu_y, sy))
+    d = mu_x - mu_y
+    S = abs(float(np.trace(sx) + np.trace(sy) + d @ d))
+    top = float(eig[-1]) if np.isfinite(eig[-1]) else 0.0
+    return 1e-8 * S, max(mu_x.shape[0], 4) * 2.0 ** -52 * max(top, 0.0)
 
 
 def pivoted_cholesky(s):

@@ -1,17 +1,18 @@
 """TEST-ONLY CPU stand-in for the perceptual entry points of libb200gen.so (include/b200gen_perceptual.h), on HOST
 pointers: tests/fid_backend.FidFakeLib extended by b200_perceptual_prep, b200_perceptual_distance and
 b200_perceptual_mean, each viewing its pointers as host tensors and storing what the float64 reading of the contract
-(tests/perceptual_emulator.py) computes.  install() routes the product's C-ABI calls to it, the ResNet-50's
-convolutions included."""
+(tests/perceptual_emulator.py) computes, with its bound, through cpu_backend's reporting stores.  install() routes
+the product's C-ABI calls to it, the ResNet-50's convolutions included."""
 import ctypes as C
 
 import torch
 
 from generativemodels_b200 import _lib, ops
+from tests import elementwise_emulator as W
 from tests import fid_backend
 from tests import igemm_emulator as IE
 from tests import perceptual_emulator as E
-from tests.cpu_backend import _np, _strided, bf16, f32, rows16
+from tests.cpu_backend import _np, _strided, bf16, f32, put, rows16, store32
 
 
 class PerceptualFakeLib(fid_backend.FidFakeLib):
@@ -23,7 +24,7 @@ class PerceptualFakeLib(fid_backend.FidFakeLib):
             z = E.prep(E.gather(src, S, ids))
             o = torch.zeros(n_out, OH, OW, 8, dtype=ops.H16)
             o[..., :3] = z.permute(0, 2, 3, 1).to(ops.H16)
-            bf16(out, o.numel()).copy_(o.reshape(-1))
+            put(bf16(out, o.numel()), W.copy(o.reshape(-1).to(torch.float64)))
         return 0
 
     def b200_perceptual_distance(self, x, y, dt, B, HW, C_, pitch, pixel, image, image32, stream):
@@ -31,18 +32,22 @@ class PerceptualFakeLib(fid_backend.FidFakeLib):
             fx, fy = (f32(p, B * HW * pitch).view(B, HW, pitch)[..., :C_] for p in (x, y))
         else:
             fx, fy = (rows16(p, B * HW, pitch, C_).reshape(B, HW, C_) for p in (x, y))
-        v = E.distance(fx, fy)
-        _np(image, B, C.c_double)[:] = v.numpy()
+        px = E.pixel_distance(fx, fy)
+        v = px.mean(1)
+        eimg = E.image_bound(px)
+        if pixel:
+            store32(pixel, W.Result(px, W.f32(px), E.pixel_bound(px), "f32"))
+        put(torch.from_numpy(_np(image, B, C.c_double)), W.Result(v, v, eimg, "f64"))
         if image32:
-            f32(image32, B).copy_(v.float())
+            store32(image32, W.Result(v, W.f32(v), eimg, "f32"))
         return 0
 
     def b200_perceptual_mean(self, image, n_groups, counts, means, loss, stream):
         cnt = [counts[g] for g in range(n_groups)]
         img = torch.from_numpy(_np(image, sum(cnt), C.c_double).copy())
-        m = E.mean(img, cnt)
-        _np(means, n_groups + 1, C.c_double)[:] = m.numpy()
-        f32(loss, 1)[0] = float(m[-1])
+        m, em = E.mean(img, cnt), E.mean_bound(img, cnt)
+        put(torch.from_numpy(_np(means, n_groups + 1, C.c_double)), W.Result(m, m, em, "f64"))
+        store32(loss, W.Result(m[-1:], W.f32(m[-1:]), em[-1:], "f32"))
         return 0
 
 

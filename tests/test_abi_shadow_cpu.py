@@ -290,7 +290,7 @@ def test_unknown_pointer_and_unknown_entry_fail(monkeypatch):
         with pytest.raises(AssertionError, match="no allocator segment"):
             _lib.require_device().b200_pndm_step(*bad)
         with pytest.raises(AssertionError, match="neither a host query"):
-            _lib.require_device().b200_ssim
+            _lib.require_device().b200_not_an_entry_point
 
 
 BIG = T.gemm("shadow_sampled_rows", "lean", None, 9000, 64, 64, out_pad=8)
