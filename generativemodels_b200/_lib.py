@@ -122,6 +122,12 @@ class DpmCoef(C.Structure):
                 ("prediction_type", C.c_int32), ("clip", C.c_int32)]
 
 
+class UniPCCoef(C.Structure):
+    _fields_ = [("alpha_s", C.c_float), ("sigma_s", C.c_float), ("c_last", C.c_float), ("v", C.c_float * 4),
+                ("c_xc", C.c_float), ("u", C.c_float * 3), ("clip_min", C.c_float), ("clip_max", C.c_float),
+                ("prediction_type", C.c_int32), ("clip", C.c_int32)]
+
+
 class RepackBlock(C.Structure):
     _fields_ = [("col0", C.c_int32), ("cin0", C.c_int32), ("cs", C.c_int32), ("ntaps", C.c_int32),
                 ("tap", C.c_int16 * 8)]
@@ -241,11 +247,13 @@ LOSS_SIGNATURES = {
     "b200_spectral_distance": [_P, _I32, _P, _F, _I32, _P, _P, _P, _P],
     "b200_adversarial": [_P, _P, _P, _P, _I32, _I32, _I32, _I32, _P, _P, _P, _P, _P],
 }
-# the multistep sampler's entry point; mirrors include/b200gen_samplers.h exactly
+# the multistep samplers' entry points; mirrors include/b200gen_samplers.h exactly
 SAMPLER_SIGNATURES = {
     "b200_dpm_solver_step": [_P, _P, C.POINTER(_P), _I32, _P, C.POINTER(DpmCoef), _P, _P, _I64, _P],
+    "b200_unipc_step": [_P, _P, _P, C.POINTER(_P), _I32, C.POINTER(UniPCCoef), _P, _P, _P, _I64, _P],
 }
 DPM_MAX_HIST = 2
+UNIPC_MAX_HIST = 3
 FFT_MAX_N, SPECTRAL_PARTIALS, ADV_MAX_OUTPUTS, ADV_PARTIALS = 4096, 1024, 8, 2048
 REDUCTION_NONE, REDUCTION_MEAN, REDUCTION_SUM = 0, 1, 2
 ADV_BCE, ADV_HINGE, ADV_LEAST_SQUARES, ADV_LEAST_SQUARES_RAW = 0, 1, 2, 3
@@ -275,7 +283,7 @@ def load():
         fn.restype = _RESTYPES.get(name, C.c_int)
     for which, struct in enumerate((IgemmParams, GnStatsParams, GnApplyParams, DdimCoef, DdpmCoef, PndmCoef, IgemmSeg,
                                     FlashParams, KlCoef, RepackBlock, SsimParams, SsimCombineParams,
-                                    FidMomentsParams, FrechetParams, DpmCoef)):
+                                    FidMomentsParams, FrechetParams, DpmCoef, UniPCCoef)):
         c_size = lib.b200_abi_sizeof(which)
         if c_size != C.sizeof(struct):
             raise B200Error(f"ABI mismatch: {struct.__name__} is {C.sizeof(struct)} bytes in Python but {c_size} in "

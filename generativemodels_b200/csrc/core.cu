@@ -77,6 +77,7 @@ extern "C" int b200_abi_sizeof(int which) {
     case 12: return (int)sizeof(b200_fid_moments_params);
     case 13: return (int)sizeof(b200_frechet_params);
     case 14: return (int)sizeof(b200_dpm_coef);
+    case 15: return (int)sizeof(b200_unipc_coef);
     default: return -1;
   }
 }

@@ -1,6 +1,8 @@
-// The DPM-Solver++ multistep step (DPMSolverMultistepScheduler.step): x0 from the model output, optional clip, then
-// the update as one weighted sum of the sample, x0, up to two earlier x0 estimates and the noise.  The host folds the
-// solver's formulas into those weights; the kernel only streams memory.  Contract: include/b200gen_samplers.h.
+// The multistep sampler steps.  DPM-Solver++ (DPMSolverMultistepScheduler.step): x0 from the model output, optional
+// clip, then the update as one weighted sum of the sample, x0, up to two earlier x0 estimates and the noise.  UniPC
+// (UniPCMultistepScheduler.step): the same x0, then the corrector as a weighted sum of the previous corrected sample, x0
+// and up to three earlier x0 estimates, then the predictor from that.  The host folds the solvers' formulas into those
+// weights; the kernels only stream memory.  Contract: include/b200gen_samplers.h.
 #include "common.cuh"
 #include "../../include/b200gen_samplers.h"
 
@@ -76,6 +78,83 @@ cudaError_t launch(int nh, const float* m, const float* s, const float* h0, cons
   return launch_kernel(dpm_step_kernel<VEC, 2>, grid, 256, 0, stream, m, s, h0, h1, z, c, prev, x0, n);
 }
 
+__device__ __forceinline__ void unipc_one(const b200_unipc_coef& c, float m, float s, float l, float h0, float h1,
+                                          float h2, int nh, bool has_last, float& p, float& x0, float& xc) {
+  if (c.prediction_type == B200_PRED_EPSILON) x0 = fmaf(-c.sigma_s, m, s) / c.alpha_s;
+  else if (c.prediction_type == B200_PRED_V) x0 = fmaf(c.alpha_s, s, -c.sigma_s * m);
+  else x0 = m;
+  if (c.clip) x0 = fminf(fmaxf(x0, c.clip_min), c.clip_max);
+  xc = s;
+  if (has_last) {
+    xc = c.c_last * l;
+    xc = fmaf(c.v[0], x0, xc);
+    if (nh > 0) xc = fmaf(c.v[1], h0, xc);
+    if (nh > 1) xc = fmaf(c.v[2], h1, xc);
+    if (nh > 2) xc = fmaf(c.v[3], h2, xc);
+  }
+  p = c.c_xc * xc;
+  p = fmaf(c.u[0], x0, p);
+  if (nh > 0) p = fmaf(c.u[1], h0, p);
+  if (nh > 1) p = fmaf(c.u[2], h1, p);
+}
+
+// Up to 6 fp32 streams in and 3 out per element, vectorised as dpm_step_kernel.  NH = number of history tensors,
+// LAST = whether the corrector runs (a previous corrected sample is given).
+template <int VEC, int NH, bool LAST>
+__global__ void __launch_bounds__(256) unipc_step_kernel(const float* __restrict__ m_in, const float* __restrict__ x,
+                                                         const float* __restrict__ last, const float* __restrict__ h0,
+                                                         const float* __restrict__ h1, const float* __restrict__ h2,
+                                                         b200_unipc_coef c, float* __restrict__ prev,
+                                                         float* __restrict__ x0_out, float* __restrict__ xc_out,
+                                                         long long n) {
+  const long long tid = (long long)blockIdx.x * blockDim.x + threadIdx.x, nthr = (long long)gridDim.x * blockDim.x;
+  long long done = 0;
+  if (VEC) {
+    const long long nv = n >> 2;
+    const float4 zero = make_float4(0.f, 0.f, 0.f, 0.f);
+    for (long long i = tid; i < nv; i += nthr) {
+      const float4 m = ld4(m_in, i), s = ld4(x, i), l = LAST ? ld4(last, i) : zero;
+      const float4 a = NH > 0 ? ld4(h0, i) : zero, b = NH > 1 ? ld4(h1, i) : zero, d = NH > 2 ? ld4(h2, i) : zero;
+      float4 p, o, q;
+      unipc_one(c, m.x, s.x, l.x, a.x, b.x, d.x, NH, LAST, p.x, o.x, q.x);
+      unipc_one(c, m.y, s.y, l.y, a.y, b.y, d.y, NH, LAST, p.y, o.y, q.y);
+      unipc_one(c, m.z, s.z, l.z, a.z, b.z, d.z, NH, LAST, p.z, o.z, q.z);
+      unipc_one(c, m.w, s.w, l.w, a.w, b.w, d.w, NH, LAST, p.w, o.w, q.w);
+      reinterpret_cast<float4*>(prev)[i] = p;
+      reinterpret_cast<float4*>(x0_out)[i] = o;
+      reinterpret_cast<float4*>(xc_out)[i] = q;
+    }
+    done = nv << 2;
+  }
+  for (long long i = done + tid; i < n; i += nthr) {
+    float p, o, q;
+    unipc_one(c, m_in[i], x[i], LAST ? last[i] : 0.f, NH > 0 ? h0[i] : 0.f, NH > 1 ? h1[i] : 0.f,
+              NH > 2 ? h2[i] : 0.f, NH, LAST, p, o, q);
+    prev[i] = p;
+    x0_out[i] = o;
+    xc_out[i] = q;
+  }
+}
+
+template <int VEC, bool LAST>
+cudaError_t launch_unipc_last(int nh, const float* m, const float* s, const float* l, const float* const* h,
+                              const b200_unipc_coef& c, float* prev, float* x0, float* xc, long long n,
+                              cudaStream_t stream) {
+  const unsigned grid = grid_for(VEC ? (n + 3) / 4 : n);
+  const float *h0 = h[0], *h1 = h[1], *h2 = h[2];
+  if (nh == 0) return launch_kernel(unipc_step_kernel<VEC, 0, LAST>, grid, 256, 0, stream, m, s, l, h0, h1, h2, c, prev, x0, xc, n);
+  if (nh == 1) return launch_kernel(unipc_step_kernel<VEC, 1, LAST>, grid, 256, 0, stream, m, s, l, h0, h1, h2, c, prev, x0, xc, n);
+  if (nh == 2) return launch_kernel(unipc_step_kernel<VEC, 2, LAST>, grid, 256, 0, stream, m, s, l, h0, h1, h2, c, prev, x0, xc, n);
+  return launch_kernel(unipc_step_kernel<VEC, 3, LAST>, grid, 256, 0, stream, m, s, l, h0, h1, h2, c, prev, x0, xc, n);
+}
+
+template <int VEC>
+cudaError_t launch_unipc(int nh, const float* m, const float* s, const float* l, const float* const* h,
+                         const b200_unipc_coef& c, float* prev, float* x0, float* xc, long long n, cudaStream_t stream) {
+  if (l) return launch_unipc_last<VEC, true>(nh, m, s, l, h, c, prev, x0, xc, n, stream);
+  return launch_unipc_last<VEC, false>(nh, m, s, l, h, c, prev, x0, xc, n, stream);
+}
+
 }  // namespace
 }  // namespace b200
 
@@ -98,5 +177,30 @@ extern "C" int b200_dpm_solver_step(const float* model_out, const float* sample,
   if (vec) B200_CUDA(b200::launch<1>(n_hist, model_out, sample, h[0], h[1], noise, *c, prev_sample, pred_x0, n, stream));
   else B200_CUDA(b200::launch<0>(n_hist, model_out, sample, h[0], h[1], noise, *c, prev_sample, pred_x0, n, stream));
   B200_LAUNCH_CHECK("dpm_step_kernel");
+  return B200_OK;
+}
+
+extern "C" int b200_unipc_step(const float* model_out, const float* sample, const float* last, const float* const* hist,
+                               int32_t n_hist, const b200_unipc_coef* c, float* prev_sample, float* pred_x0,
+                               float* corrected, int64_t n, void* stream_v) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
+  B200_CHECK_ARG(model_out && sample && c && prev_sample && pred_x0 && corrected && n >= 1,
+                 "unipc_step: bad arguments");
+  B200_CHECK_ARG(n_hist >= 0 && n_hist <= B200_UNIPC_MAX_HIST && (n_hist == 0 || hist),
+                 "unipc_step: n_hist must be 0..%d with a history array", B200_UNIPC_MAX_HIST);
+  B200_CHECK_ARG(c->prediction_type == B200_PRED_EPSILON || c->prediction_type == B200_PRED_SAMPLE ||
+                 c->prediction_type == B200_PRED_V, "unipc_step: unknown prediction_type %d", c->prediction_type);
+  const float* h[3] = {nullptr, nullptr, nullptr};
+  for (int k = 0; k < n_hist; ++k) {
+    h[k] = hist[k];
+    B200_CHECK_ARG(h[k], "unipc_step: null history tensor %d", k);
+  }
+  const bool vec = (((uintptr_t)model_out | (uintptr_t)sample | (uintptr_t)last | (uintptr_t)h[0] | (uintptr_t)h[1] |
+                     (uintptr_t)h[2] | (uintptr_t)prev_sample | (uintptr_t)pred_x0 | (uintptr_t)corrected) & 15) == 0;
+  if (vec) B200_CUDA(b200::launch_unipc<1>(n_hist, model_out, sample, last, h, *c, prev_sample, pred_x0, corrected, n,
+                                           stream));
+  else B200_CUDA(b200::launch_unipc<0>(n_hist, model_out, sample, last, h, *c, prev_sample, pred_x0, corrected, n,
+                                       stream));
+  B200_LAUNCH_CHECK("unipc_step_kernel");
   return B200_OK;
 }
