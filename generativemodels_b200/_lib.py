@@ -128,6 +128,12 @@ class UniPCCoef(C.Structure):
                 ("prediction_type", C.c_int32), ("clip", C.c_int32)]
 
 
+class SASolverCoef(C.Structure):
+    _fields_ = [("alpha_s", C.c_float), ("sigma_s", C.c_float), ("c_last", C.c_float), ("v", C.c_float * 3),
+                ("c_zlast", C.c_float), ("c_xc", C.c_float), ("u", C.c_float * 3), ("c_z", C.c_float),
+                ("clip_min", C.c_float), ("clip_max", C.c_float), ("prediction_type", C.c_int32), ("clip", C.c_int32)]
+
+
 class RepackBlock(C.Structure):
     _fields_ = [("col0", C.c_int32), ("cin0", C.c_int32), ("cs", C.c_int32), ("ntaps", C.c_int32),
                 ("tap", C.c_int16 * 8)]
@@ -251,9 +257,11 @@ LOSS_SIGNATURES = {
 SAMPLER_SIGNATURES = {
     "b200_dpm_solver_step": [_P, _P, C.POINTER(_P), _I32, _P, C.POINTER(DpmCoef), _P, _P, _I64, _P],
     "b200_unipc_step": [_P, _P, _P, C.POINTER(_P), _I32, C.POINTER(UniPCCoef), _P, _P, _P, _I64, _P],
+    "b200_sa_solver_step": [_P, _P, _P, _P, C.POINTER(_P), _I32, _P, C.POINTER(SASolverCoef), _P, _P, _P, _I64, _P],
 }
 DPM_MAX_HIST = 2
 UNIPC_MAX_HIST = 3
+SA_SOLVER_MAX_HIST = 2
 FFT_MAX_N, SPECTRAL_PARTIALS, ADV_MAX_OUTPUTS, ADV_PARTIALS = 4096, 1024, 8, 2048
 REDUCTION_NONE, REDUCTION_MEAN, REDUCTION_SUM = 0, 1, 2
 ADV_BCE, ADV_HINGE, ADV_LEAST_SQUARES, ADV_LEAST_SQUARES_RAW = 0, 1, 2, 3
@@ -283,7 +291,8 @@ def load():
         fn.restype = _RESTYPES.get(name, C.c_int)
     for which, struct in enumerate((IgemmParams, GnStatsParams, GnApplyParams, DdimCoef, DdpmCoef, PndmCoef, IgemmSeg,
                                     FlashParams, KlCoef, RepackBlock, SsimParams, SsimCombineParams,
-                                    FidMomentsParams, FrechetParams, DpmCoef, UniPCCoef)):
+                                    FidMomentsParams, FrechetParams, DpmCoef, UniPCCoef,
+                                    SASolverCoef)):
         c_size = lib.b200_abi_sizeof(which)
         if c_size != C.sizeof(struct):
             raise B200Error(f"ABI mismatch: {struct.__name__} is {C.sizeof(struct)} bytes in Python but {c_size} in "

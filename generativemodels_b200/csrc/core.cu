@@ -78,6 +78,7 @@ extern "C" int b200_abi_sizeof(int which) {
     case 13: return (int)sizeof(b200_frechet_params);
     case 14: return (int)sizeof(b200_dpm_coef);
     case 15: return (int)sizeof(b200_unipc_coef);
+    case 16: return (int)sizeof(b200_sa_solver_coef);
     default: return -1;
   }
 }

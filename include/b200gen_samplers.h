@@ -2,7 +2,8 @@
  * b200gen_samplers.h — the multistep sampler steps of libb200gen.so's C-ABI: one fused elementwise pass of
  * DPMSolverMultistepScheduler.step (DPM-Solver++, Lu et al. 2022, arXiv 2211.01095; orders 1-3 of the ODE form,
  * orders 1-2 of the SDE form) and one of UniPCMultistepScheduler.step (UniPC, Zhao et al. 2023, arXiv 2302.04867;
- * the data-prediction form, predictor orders 1-3 with the UniC corrector).
+ * the data-prediction form, predictor orders 1-3 with the UniC corrector) and one of SASolverScheduler.step
+ * (SA-Solver, Xue et al. 2023, arXiv 2309.05019; the data-prediction form of the stochastic Adams predictor-corrector).
  */
 #ifndef B200GEN_SAMPLERS_H_
 #define B200GEN_SAMPLERS_H_
@@ -15,10 +16,12 @@ extern "C" {
 
 /* ------------------------------------------------------------------------------------------------
  * The conventions of b200gen.h hold (return codes, no allocation, no synchronisation, work enqueued on `stream`).
- * b200_abi_sizeof(14) is sizeof(b200_dpm_coef), b200_abi_sizeof(15) is sizeof(b200_unipc_coef).
+ * b200_abi_sizeof(14) is sizeof(b200_dpm_coef), b200_abi_sizeof(15) is sizeof(b200_unipc_coef),
+ * b200_abi_sizeof(16) is sizeof(b200_sa_solver_coef).
  * ------------------------------------------------------------------------------------------------ */
 #define B200_DPM_MAX_HIST 2
 #define B200_UNIPC_MAX_HIST 3
+#define B200_SA_SOLVER_MAX_HIST 2
 
 /* The solver's coefficients for one step, folded on the host in float64 and rounded once to fp32.  alpha_s, sigma_s
  * are sqrt(alphas_cumprod[s]) and sqrt(1 - alphas_cumprod[s]) of the current timestep s. */
@@ -66,6 +69,33 @@ typedef struct {
 int b200_unipc_step(const float* model_out, const float* sample, const float* last, const float* const* hist,
                     int32_t n_hist, const b200_unipc_coef* c, float* prev_sample, float* pred_x0, float* corrected,
                     int64_t n, void* stream);
+
+/* SA-Solver's corrector and predictor for one step, each folded on the host in float64 and rounded once to fp32. */
+typedef struct {
+  float alpha_s, sigma_s;       /* of the current timestep, to form x0 as in b200_dpm_solver_step                */
+  float c_last;                 /* corrector: weight of the previous step's start sample                         */
+  float v[3];                   /* corrector: weights of x0 and of hist[0], hist[1]                              */
+  float c_zlast;                /* corrector: weight of the previous step's noise                                */
+  float c_xc;                   /* predictor: weight of the corrected sample                                     */
+  float u[3];                   /* predictor: weights of x0 and of hist[0], hist[1]                              */
+  float c_z;                    /* predictor: weight of this step's noise                                        */
+  float clip_min, clip_max;
+  int32_t prediction_type, clip;
+} b200_sa_solver_coef;
+
+/* b200_sa_solver_step: over n fp32 elements, with s = sample, m = model_out, in fp32:
+ *   x0 as in b200_dpm_solver_step (prediction type, then the clip)
+ *   xc = s                                                                     if last == NULL
+ *   xc = c_last * last;  xc = fma(v[0], x0, xc);  xc = fma(v[k + 1], hist[k], xc) for k < n_hist;
+ *        xc = fma(c_zlast, last_noise, xc) if last_noise != NULL                                      otherwise
+ *   p  = c_xc * xc;  p = fma(u[0], x0, p);  p = fma(u[k + 1], hist[k], p) for k < n_hist;
+ *        p = fma(c_z, noise, p) if noise != NULL
+ *   prev_sample = p,  pred_x0 = x0,  corrected = xc.
+ * hist is a host array of n_hist (0..B200_SA_SOLVER_MAX_HIST) device pointers, the previous x0 estimates, newest
+ * first.  last_noise needs last.  Any alignment; the outputs must not overlap the inputs or each other. */
+int b200_sa_solver_step(const float* model_out, const float* sample, const float* last, const float* last_noise,
+                        const float* const* hist, int32_t n_hist, const float* noise, const b200_sa_solver_coef* c,
+                        float* prev_sample, float* pred_x0, float* corrected, int64_t n, void* stream);
 
 #ifdef __cplusplus
 }
