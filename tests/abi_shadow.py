@@ -1,6 +1,6 @@
-"""Shadow calls: every C-ABI call a network, metric or loss makes runs on the real library AND on the CPU stand-in
-(StandIn below: tests/losses_backend.LossesFakeLib, which carries the metric, FID and perceptual entry points, and
-tests/samplers_backend.SamplersFakeLib) with the call's own inputs, and the two are compared under the bound of the
+"""Shadow calls: every C-ABI call a network, metric, loss, scheduler or inferer makes runs on the real library AND on
+the CPU stand-in (StandIn below: tests/losses_backend.LossesFakeLib, which carries the metric, FID and perceptual entry
+points, and tests/{unipc,sa_solver}_backend's stand-ins, which carry the three sampler steps) with the call's own inputs, and the two are compared under the bound of the
 entry point's family.  Test infrastructure only.
 
     with abi_shadow.shadow(monkeypatch) as sh:
@@ -36,7 +36,8 @@ For each b200_* call the proxy installed in place of _lib.require_device()
 
 Each call is logged with a compact argument signature, its worst excess and, for b200_igemm, the planner's column
 tile and split factor and the store path (the predicates of tests/test_igemm_contract_gpu.py's docstring), so that a
-test can assert which kernel paths the networks reached.
+test can assert which kernel paths the networks reached.  The scheduler and inferer entry points carry path labels
+too (step_paths), derived from the call's arguments with the predicates the .cu files choose their kernels by.
 """
 from __future__ import annotations
 
@@ -59,7 +60,8 @@ from tests import losses_backend
 from tests import losses_emulator as LE
 from tests import metrics_emulator as ME
 from tests import norm_emulator as N
-from tests import samplers_backend
+from tests import sa_solver_backend
+from tests import unipc_backend
 
 PASSTHROUGH = {"b200_sm_count", "b200_igemm_split_workspace_bytes", "b200_attention_flash_workspace_bytes",
                "b200_groupnorm_workspace_bytes", "b200_igemm_plan", "b200_version", "b200_act_dtype",
@@ -72,9 +74,9 @@ SOFTMAX_SUM_REL = 1e-5         # softmax partial sums vs the kernel's own rows (
 _SIGNED = {1: torch.int8, 2: torch.int16, 4: torch.int32, 8: torch.int64}
 
 
-class StandIn(losses_backend.LossesFakeLib, samplers_backend.SamplersFakeLib):
+class StandIn(losses_backend.LossesFakeLib, unipc_backend.UniPCFakeLib, sa_solver_backend.SASolverFakeLib):
     """The CPU stand-in of every entry point: the network, metric, FID, perceptual and loss stand-ins, and the
-    sampler's."""
+    three sampler steps' (DPM-Solver++, UniPC, SA-Solver)."""
 
 
 def _excess(got, want, tol):
@@ -276,6 +278,52 @@ def igemm_path(p, plan):
 
 
 # ----------------------------------------------------------------------------------------------------------------
+# the scheduler and inferer paths (generativemodels_b200/csrc/{samplers,elementwise}.cu)
+# ----------------------------------------------------------------------------------------------------------------
+def _vec_kind(ptrs, n):
+    """The step kernels' access path: 'scalar' (VEC = 0) unless every pointer the entry point ORs into its alignment
+    test is 16-byte aligned; then 'vec', or 'tail' when n % 4 elements are left to the scalar tail."""
+    if any((p or 0) % 16 for p in ptrs):
+        return "scalar"
+    return "vec" if n % 4 == 0 else "tail"
+
+
+def step_paths(name, o):
+    """Path labels of one call of a scheduler / inferer entry point from its arguments `o` (the ctypes objects),
+    with the kernel-selection predicates of the entry point; () for other entry points."""
+    def hist(arr, nh):
+        return [int(arr[k] or 0) for k in range(nh)]
+    if name == "b200_dpm_solver_step":
+        m, s, h, nh, z, c, prev, x0, n = o[:9]
+        return (f"dpm nh{nh}" + (" noise" if z else ""),
+                "dpm step " + _vec_kind([m, s, *hist(h, nh), z, prev, x0], n))
+    if name == "b200_unipc_step":
+        m, s, last, h, nh, c, prev, x0, xc, n = o[:10]
+        return (f"unipc nh{nh}" + (" last" if last else ""),
+                "unipc step " + _vec_kind([m, s, last, *hist(h, nh), prev, x0, xc], n))
+    if name == "b200_sa_solver_step":
+        m, s, last, zl, h, nh, z, c, prev, x0, xc, n = o[:12]
+        zl = zl if last else None                       # the kernel reads last_noise only with last
+        return (f"sa nh{nh}" + (" last" if last else "") + (" zl" if zl else "") + (" z" if z else ""),
+                "sa step " + _vec_kind([m, s, last, zl, *hist(h, nh), z, prev, x0, xc], n))
+    if name == "b200_ddim_step":
+        m, s, z, c, prev, x0, n = o[:7]
+        return ("ddim" + (" noise" if z else ""), "ddim step " + _vec_kind([m, s, z, prev, x0], n))
+    if name == "b200_ddpm_step":
+        z, c = o[2], o[4]
+        return (f"ddpm var{c.var_mode}" if z else "ddpm no noise",)      # var_mode is read only with noise
+    if name == "b200_pndm_step":
+        return (f"pndm nh{o[2].n_hist}",)
+    if name == "b200_ddpm_kl":
+        return ("ddpm_kl t0" if o[3].is_t0 else "ddpm_kl t",)
+    if name == "b200_add_noise":
+        return ("add_noise +" if o[4] > 0 else "add_noise -",)
+    if name == "b200_scale_f32":
+        return ("scale div" if o[2] != 1.0 else "scale mul",)
+    return ()
+
+
+# ----------------------------------------------------------------------------------------------------------------
 # the proxy
 # ----------------------------------------------------------------------------------------------------------------
 @dataclass
@@ -458,6 +506,7 @@ class _Compare:
 
     def entry_specific(self):
         o = [_obj(a) for a in self.args]
+        self.paths += step_paths(self.name, o)
         if self.name == "b200_igemm":
             self.igemm(o[0])
         elif self.name == "b200_attention_flash":
